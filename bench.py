@@ -12,6 +12,7 @@ required hostname anti-affinity, 200 000 pre-existing pods (cluster-capacity_b20
   e2e       the same metric through the C-ABI with HOST buffers: ccsim_load_nodes (H2D from pinned memory) +
             ccsim_set_templates + ccsim_run + result read-back inside the timed region
   roofline  algorithmic bytes (SURVEY.md §8d: 96 B per predicate-eval for C4) / wave-kernel time vs the measured HBM peak
+            (MEASURED_PEAKS.json when present, else the H100 SXM data-sheet figure, marked as such)
   cpu_baseline / --impl reference: the CPU oracle (a port of the reference's loop; no Go toolchain exists to run the
             reference itself) on the box's host cores, on a bounded prefix of the same workload.
 
@@ -55,35 +56,29 @@ def select_workload(key):
     WORKLOAD, B_EVAL, MAX_LIMIT, MAKE = WORKLOADS[key]
 
 
-def profiled_traffic():
-    """dram__bytes_read+write per launch of the wave kernel from the committed ncu --set full capture (profiles/)."""
-    # (C5: the capture is of an earlier build of the streaming kernel — 53 ms per launch — with the same DRAM-side behaviour: the
-    #  4-byte memo column of the wave's template, 4 MB, comes from HBM every wave because the 64 columns, 256 MB, do not fit the L2)
-    for name in ("r2_wave_%s_traffic.json" % WKEY, "r2_stream_%s_traffic.json" % WKEY, "r1_wave_c4_traffic.json" if WKEY == "c4" else ""):
-        try:
-            with open(os.path.join(ROOT, "profiles", name)) as f:
-                return float(json.load(f)["traffic_bytes_per_launch"])
-        except Exception:
-            pass
-    return None
-
-
 def measured_peak():
     try:
         with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
             return float(json.load(f)["hbm_gbs"]), "measured"
     except Exception:
-        return 6650.0, "fallback"
+        return 3350.0, "datasheet (H100 SXM HBM3; not reached)"
 
 
 class ClockSampler(threading.Thread):
-    """nvidia-smi clocks/throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks/throttle reasons during the timed region, and the card's name and power limit (read-only queries)."""
 
     def __init__(self, index):
         super().__init__(daemon=True)
         self.index = index
         self.rows = []
         self.stop_flag = threading.Event()
+        self.card = {}
+        try:
+            out = subprocess.run(["nvidia-smi", "-i", str(index), "--query-gpu=name,power.limit", "--format=csv,noheader,nounits"],
+                                 capture_output=True, text=True, timeout=10).stdout.strip().split(",")
+            self.card = {"name": out[0].strip(), "power_limit_w": float(out[1])}
+        except Exception:
+            pass
 
     def run(self):
         q = ("clocks.sm,clocks.max.sm,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
@@ -103,7 +98,8 @@ class ClockSampler(threading.Thread):
         mx = [int(r[1]) for r in self.rows if len(r) > 1 and r[1].isdigit()]
         names = ["hw_slowdown", "hw_thermal_slowdown", "sw_thermal_slowdown", "sw_power_cap"]
         reasons = sorted({names[i] for r in self.rows for i in range(4) if len(r) > 2 + i and r[2 + i] == "Active"})
-        return {"sm_mhz": int(np.median(sm)) if sm else None, "sm_max_mhz": max(mx) if mx else None,
+        return {"gpu": self.card.get("name"), "power_limit_w": self.card.get("power_limit_w"),
+                "sm_mhz": int(np.median(sm)) if sm else None, "sm_max_mhz": max(mx) if mx else None,
                 "reasons": reasons, "samples": len(sm)}
 
 
@@ -242,12 +238,12 @@ def latency_block(st, kernel_ms, sm_mhz):
         cyc = {n: st["phase_cycles"][i] / w for i, n in enumerate(names)}
         out.update({"candidates_replayed_per_wave": st["candidates"] / w, "waves_that_raised_the_bar": st["bar_raised_waves"],
                     "cycles_per_wave_cta0": cyc, "cycles_per_wave_total": sum(cyc.values()),
-                    "us_per_wave_from_cycles": (sum(cyc.values()) / (sm_mhz or 1965)) if sm_mhz else None})
+                    "us_per_wave_from_cycles": (sum(cyc.values()) / sm_mhz) if sm_mhz else None})
     elif st["engine"].startswith("streaming"):
         names = ("scan_mbarrier_wait_filter_argmax", "barriers_prefetch_issue_block_argmax", "exchange_l2_round_trip", "commit_barrier")
         cyc = {n: st["phase_cycles"][i] / w for i, n in enumerate(names)}
         out.update({"stale_memo_rescored_per_wave_cta0": st["candidates"] / w, "cycles_per_wave_cta0": cyc, "cycles_per_wave_total": sum(cyc.values()),
-                    "us_per_wave_from_cycles": (sum(cyc.values()) / (sm_mhz or 1965)) if sm_mhz else None})
+                    "us_per_wave_from_cycles": (sum(cyc.values()) / sm_mhz) if sm_mhz else None})
     return out
 
 
@@ -265,7 +261,7 @@ def run_reference(args):
     if rank != 0:
         return
     snap, tmpl, ctr = MAKE(world if args.mode == "sharded" else 1)     # the same workload as our arm at this N
-    steps = max(1, min(args.steps, 3))
+    steps = args.steps
     evals = placed = 0
     dt = 0.0
     threads = cores = pods = 0
@@ -321,6 +317,16 @@ def pinned_snapshot(snap):
     return s2, nbytes
 
 
+def dump_outputs(out_dir, result):
+    """What the timed path returned in its last step (the whole pod -> node sequence, the FitError histogram, the counts), as float64
+    arrays (node indices and counts are exact below 2^53). Inputs are seeded, so two builds can be compared file by file."""
+    os.makedirs(out_dir, exist_ok=True)
+    arrays = {"pod_node": np.asarray(result["pod_node"]), "reason_hist": np.asarray(result["reason_hist"]),
+              "run_summary": np.array([result["placed"], result["stop_code"], result["preempt_no_victims"]])}
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), a.astype(np.float64))
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -332,7 +338,10 @@ def main():
     ap.add_argument("--no-objects", action="store_true", help="skip the e2e_objects leg (plugin call from Node/Pod JSON)")
     ap.add_argument("--workload", default="c4", choices=sorted(WORKLOADS), help="c4 (default: the metric's 100k-node configuration) or c5 (1M nodes x 64 podspecs)")
     ap.add_argument("--mode", default="sharded", choices=["sharded", "replicas"], help="N>1: node-sharded run or independent replicas")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="after the timed steps, write what the last timed step returned as DIR/<name>.npy (float64)")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be >= 1")
     select_workload(args.workload)
     if args.impl == "reference":
         return run_reference(args)
@@ -465,7 +474,7 @@ def main():
             "gpu_launches": int(launches),
             "clocks": sampler.summary(),
             "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                         "traffic": profiled_traffic() if world == 1 else None, "peak_kind": peak_kind,
+                         "peak_kind": peak_kind,
                          "algorithmic_bytes_per_launch": ref_evals * B_EVAL / args.steps,
                          "achieved_physical": achieved_phys, "frac_physical": achieved_phys / peak,
                          "physical_bytes_per_launch": evals * B_EVAL / args.steps,
@@ -474,7 +483,7 @@ def main():
                                  "(placed+1) x N x %d B (every pod attempt of the reference loop streams every node row) over the wave kernel's CUDA-event "
                                  "time vs the measured HBM copy peak — and may exceed 1: the multi-commit engine decides ~placed/waves reference cycles per "
                                  "pass over the (shared-memory resident) node tile and the streaming engine reads 24 B of the 72 B row; achieved_physical "
-                                 "counts one row per node and PASS actually made; `traffic` is ncu's dram bytes per launch (profiles/)" % B_EVAL},
+                                 "counts one row per node and PASS actually made" % B_EVAL},
         }
         # ---- parity on the timed configuration (and the CPU baseline: the same oracle run serves both) ----
         # N=1: the oracle runs the WHOLE analysis of the timed snapshot when that fits ~40 s (C4: ~18 s on 16 threads) and
@@ -494,9 +503,11 @@ def main():
             line["parity"] = None
         # ---- the reference-facing plugin call: framework.New + SyncWithClient + Run + Report from Node / Pod JSON in host memory ----
         if WKEY == "c4" and world == 1 and not args.no_objects:
-            line["e2e_objects"] = objects_leg(last_result, local, max(1, min(args.steps, 2)))
+            line["e2e_objects"] = objects_leg(last_result, local, args.steps)
             parity_ok = parity_ok and line["e2e_objects"]["same_sequence_as_flat_run"]
         print(json.dumps(line), flush=True)
+        if args.dump_outputs:
+            dump_outputs(args.dump_outputs, last_result)
     eng.close()
     if world > 1:
         dist.barrier()

@@ -1,4 +1,4 @@
-"""Builds libccsim.so in-tree for sm_100a (nvcc cross-compiles without a GPU)."""
+"""Builds libccsim.so in-tree for sm_90a (H100; nvcc cross-compiles without a GPU)."""
 import os
 import subprocess
 
@@ -9,7 +9,7 @@ DEPS = SRC + sorted(glob.glob(os.path.join(_HERE, "csrc", "*.cuh"))) + [os.path.
 OUT = os.path.join(_HERE, "libccsim.so")
 # -fmad=false: the float64 scorers (BalancedAllocation, Go's math.Log) must round every operation on its own, like Go on amd64;
 # they use __dmul_rn/__dadd_rn intrinsics already, the flag keeps a plain a*b+c written later from being contracted silently
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-fmad=false", "-std=c++17", "-shared",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-fmad=false", "-std=c++17", "-shared",
               "-Xcompiler", "-fPIC", "-lcudart", "-ldl"]
 
 
@@ -21,7 +21,7 @@ HOST_OUT = os.path.join(_HERE, "libcchost.so")
 
 
 def build(force=False, verbose=False):
-    """libccsim.so (CUDA, sm_100a) then libcchost.so (C++ host side, links libccsim via $ORIGIN rpath).
+    """libccsim.so (CUDA, sm_90a) then libcchost.so (C++ host side, links libccsim via $ORIGIN rpath).
     CCSIM_NO_REBUILD=1 (set by GPU-box job scripts): use the shipped libraries as they are, whatever the source mtimes say."""
     if os.environ.get("CCSIM_NO_REBUILD") and os.path.exists(OUT) and os.path.exists(HOST_OUT) and not force:
         return OUT

@@ -1,4 +1,4 @@
-// ccsim_device.cuh — device-side data layout and the per-node predicate / score functions (sm_100a).
+// ccsim_device.cuh — device-side data layout and the per-node predicate / score functions (sm_90a).
 //
 // One predicate-eval = one (pod attempt, node) pair through eval_node(): what checkNode does once in the reference
 // (vendor/k8s.io/kubernetes/pkg/scheduler/schedule_one.go:644-666 -> framework/runtime/framework.go:897-930), followed
@@ -12,7 +12,7 @@
 #include <limits.h>
 #include "../../include/ccsim.h"
 
-#define CCSIM_MAX_GRID 160  /* >= SM count of the part (B200: 148) */
+#define CCSIM_MAX_GRID 160  /* >= SM count of the part (H100 SXM: 132) */
 #define SLOT_STRIDE 16      /* 64-bit words per CTA slot: one 128-byte L2 line per CTA (sharing a line between writers costs ~2x) */
 
 struct DevCounter {

@@ -1,4 +1,4 @@
-// ccsim_engine.cu — libccsim.so: the B200 cluster-capacity hot path behind the C-ABI of include/ccsim.h.
+// ccsim_engine.cu — libccsim.so: the H100 cluster-capacity hot path behind the C-ABI of include/ccsim.h.
 //
 // Replaces the reference's sequential schedule-one-pod-then-update loop
 // (pkg/framework/simulator.go:356-381 driving vendor/k8s.io/kubernetes/pkg/scheduler/schedule_one.go:66-148) by ONE
@@ -9,7 +9,7 @@
 //     warp-shuffle + shared-memory arg-max over packed (score, ~index) keys,
 //     all-to-all exchange of one 64-bit tagged key per CTA (and per normalisation class) through L2 — this is the
 //     only grid-wide synchronisation of the wave (no atomics, no fences: the tag makes each word self-validating),
-//     every CTA redundantly reduces the 148 keys, the owner CTA commits the winner row (NodeInfo.update,
+//     every CTA redundantly reduces the keys of all CTAs (one per SM), the owner CTA commits the winner row (NodeInfo.update,
 //     framework/types.go:409-427), every CTA updates its replica of the per-domain counters.
 //
 // The node state is mutated in place in HBM/L2; only the owner CTA ever reads or writes a given row, so no
@@ -1228,8 +1228,7 @@ static int run_prepare(ccsim_handle *h, int64_t max_pods) {
     p.sample_k = kf;
   }
   LeanParams lp; memset(&lp, 0, sizeof(lp));
-  // measured on B200 (profiles/r1_kernel_variants.md): at 768 threads the lean kernel beats the generic resident kernel on
-  // every eligible workload (C2 2.50 vs 2.67, C3 2.64 vs 2.84, C4 4.27 vs 4.95 us/wave); CCSIM_FORCE_GENERIC overrides.
+  // the lean kernel (768 threads) takes every eligible workload; CCSIM_FORCE_GENERIC overrides.
   // normalised soft scorers / ImageLocality columns run in the generic kernel only (multi-phase waves)
   bool has_pref = false, has_soft = false;
   for (auto &T : h->h_templates) {
@@ -1381,8 +1380,9 @@ static int run_prepare(ccsim_handle *h, int64_t max_pods) {
     ccsim_stream_prep_kernel<<<std::min<long long>(8LL * h->sm_count, (sp.n_pad + 255) / 256), 256, 0, s>>>(p, sp);
     h->launches++;
     CK(cudaGetLastError());
-    // resident free_* columns when the chunk fits next to the memo ring (24 B per node: up to ~8k nodes per SM)
-    const size_t smem_resf = (size_t)STREAM_STAGES_RES * STREAM_TILE * 4 + (size_t)sp.chunk_pad * 24 + 128;
+    // resident free_* columns when the chunk fits next to the memo ring (24 B per node: up to ~7.8k nodes per SM)
+    sp.res_rows = (p.chunk + 31) & ~31;
+    const size_t smem_resf = (size_t)STREAM_STAGES_RES * STREAM_TILE * 4 + (size_t)sp.res_rows * 24 + 128;
     stream_mode = masks ? 1 : ((smem_resf + sizeof(StreamShared) + 1024 <= h->smem_optin && sp.tiles <= STREAM_STAGES_RES && !getenv("CCSIM_STREAM_ALL")) ? 2 : 0);
     kern = stream_mode == 1 ? (const void *)ccsim_wave_stream_kernel<1> : stream_mode == 2 ? (const void *)ccsim_wave_stream_kernel<2> : (const void *)ccsim_wave_stream_kernel<0>;
     smem = stream_mode == 2 ? smem_resf : (size_t)STREAM_STAGES * STREAM_TILE * (masks ? 40 : 24) + 128;

@@ -11,7 +11,7 @@
 //   one (LDS dom, LDS counter, compare) per PodTopologySpread / InterPodAffinity term,
 // then REDUX arg-max, the tagged-word exchange through L2, and the commit by the owner CTA.
 // The hot record is AoS with a stride of an odd number of 16-byte units: LDS.128 by consecutive threads is then
-// bank-conflict free (B300_MICROARCH.md, "smem crossbar BW 128/N B/cyc/SM").
+// bank-conflict free (each quarter-warp's 8 x 16 B requests land on distinct bank groups).
 #pragma once
 #include "ccsim_device.cuh"
 
@@ -519,8 +519,8 @@ __global__ void __launch_bounds__(LEAN_THREADS, 1) ccsim_wave_lean_kernel(const 
               if (ci.is_aff) { atomicAdd((unsigned long long *)&ls.aff_total, (unsigned long long)ci.inc); ls.dirty = 1; }
             } else {
               // the winner's domain id: from this CTA's tile if it owns the node, else from the whole-cluster column (L2).
-              // (Carrying the ids with the exchanged key — as extra words or packed into the key's low bits — was measured and is
-              //  not faster: profiles/r1_kernel_variants.md.)
+              // (Carrying the ids with the exchanged key instead — as extra words or packed into the key's low bits — lengthens every
+              //  CTA's exchange for a lookup only the non-owner CTAs make.)
               const int32_t dom = mine ? reinterpret_cast<const int32_t *>(rec + (size_t)jw * su)[10 + lp.counter_slot[j]] : ci.gtopo[g];
               if (dom >= 0) {
                 int32_t *cnt = smem_cnt + p.counters[j].smem_off;

@@ -44,7 +44,8 @@ struct StreamParams {
   int32_t chunk_pad;              // nodes per CTA, padded to a multiple of STREAM_TILE
   int32_t tiles;                  // chunk_pad / STREAM_TILE
   long long n_pad;                // grid * chunk_pad
-  int32_t use_masks, pad;
+  int32_t use_masks;
+  int32_t res_rows;               // MODE 2: resident rows per CTA (chunk rounded up to a warp; <= chunk_pad)
 };
 
 struct __align__(16) StreamShared {
@@ -101,8 +102,8 @@ __global__ void ccsim_stream_prep_kernel(const DevParams p, const StreamParams s
 }
 
 // MODE 0: everything streamed (24 B per node and wave); 1: + taint/static words (40 B); 2: the free_* columns of the CTA's chunk stay in
-// shared memory for the whole run (20 B per node: 1M nodes fit in the 148 SMs' shared memory) and only the score memo column of the
-// wave's template is streamed (4 B per node and wave)
+// shared memory for the whole run (24 B per node, sized by the chunk rather than its tile padding: 1M nodes fit in the 132 SMs' shared
+// memory of an H100) and only the score memo column of the wave's template is streamed (4 B per node and wave)
 template <int MODE>
 __global__ void __launch_bounds__(STREAM_BLOCK, 1) ccsim_wave_stream_kernel(const DevParams p, const StreamParams sp) {
   constexpr bool MASKS = MODE == 1, RESF = MODE == 2;
@@ -116,7 +117,7 @@ __global__ void __launch_bounds__(STREAM_BLOCK, 1) ccsim_wave_stream_kernel(cons
   longlong2 *r_free = reinterpret_cast<longlong2 *>(smem_raw + NST * STAGE_BYTES);
   // A generation number per node instead of invalidating 64 memo entries at every commit: a memo entry is (generation << 12 |
   // score + 1) and is valid only while the node's generation stands (NodeInfo.Generation, framework/types.go:409-427).
-  int2 *r_pg = reinterpret_cast<int2 *>(r_free + sp.chunk_pad);
+  int2 *r_pg = reinterpret_cast<int2 *>(r_free + sp.res_rows);
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int cta = blockIdx.x;
   const long long base = (long long)cta * sp.chunk_pad;           // this CTA's first padded row
@@ -150,7 +151,7 @@ __global__ void __launch_bounds__(STREAM_BLOCK, 1) ccsim_wave_stream_kernel(cons
     c.sw.least_w_cpu = tp.least_w_cpu; c.sw.least_w_mem = tp.least_w_mem;
   }
   if (RESF)
-    for (int j = threadIdx.x; j < sp.chunk_pad; j += STREAM_BLOCK) {
+    for (int j = threadIdx.x; j < sp.res_rows; j += STREAM_BLOCK) {
       r_free[j] = make_longlong2(sp.f_cpu[(long long)blockIdx.x * sp.chunk_pad + j], sp.f_mem[(long long)blockIdx.x * sp.chunk_pad + j]);
       r_pg[j] = make_int2(sp.f_pods[(long long)blockIdx.x * sp.chunk_pad + j], 0);
     }
@@ -237,7 +238,7 @@ __global__ void __launch_bounds__(STREAM_BLOCK, 1) ccsim_wave_stream_kernel(cons
         while (!mbar_try_wait(&ss.full[0], (uint32_t)(k & 1))) { }
         if (dbg) { const long long c0 = clock64(); dbg_wait += c0 - dbg_t; dbg_t = c0; }
         const int32_t *memo_s = reinterpret_cast<const int32_t *>(smem_raw);      // stage q = tile q: contiguous
-        const int cpad = sp.chunk_pad;
+        const int cpad = sp.res_rows;     // rows behind it are padding (free_pods = INT_MIN): never feasible
         uint32_t best32 = 0u;
         auto node = [&](int off, bool check) {
           if (check && off == pend_off) {  // the node committed a moment ago: wait for the urgent part of its commit
@@ -267,7 +268,7 @@ __global__ void __launch_bounds__(STREAM_BLOCK, 1) ccsim_wave_stream_kernel(cons
         #pragma unroll 2
         for (int off = tid; off < pt; off += STREAM_THREADS) node(off, false);
         #pragma unroll
-        for (int off = pt + tid; off < pt + STREAM_TILE; off += STREAM_THREADS) node(off, true);
+        for (int off = pt + tid; off < min(pt + STREAM_TILE, cpad); off += STREAM_THREADS) node(off, true);
         if (best32) {
           const int boff = (int)(0xfffffu - (best32 & 0xfffffu));
           best = pack_key((int32_t)(best32 >> 20) - 1, (uint32_t)(p.node_base + (long long)cta * p.chunk + boff));

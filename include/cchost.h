@@ -1,5 +1,5 @@
 /*
- * cchost.h — C-ABI of the host side of the hot path: the B200 counterpart of the reference's pkg/framework API.
+ * cchost.h — C-ABI of the host side of the hot path: the H100 counterpart of the reference's pkg/framework API.
  *
  *   cc_new               <- framework.New(kubeSchedulerConfig, kubeConfig, simulatedPod, maxPods, excludeNodes)
  *                           (pkg/framework/simulator.go:107-158)

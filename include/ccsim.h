@@ -1,5 +1,5 @@
 /*
- * ccsim.h — C-ABI of the B200 cluster-capacity hot path ("libccsim.so").
+ * ccsim.h — C-ABI of the H100 cluster-capacity hot path ("libccsim.so").
  *
  * This is the drop-in boundary of SURVEY.md §8(b): plain pointers and sizes, no torch / C++ types.
  * It replaces, for the simulated pod stream, what the reference drives through the embedded

@@ -1,4 +1,4 @@
-# development check of the wave kernels on ONE B200: randomized differential tests, parity suites, full-size runs, then the C4 bench line
+# development check of the wave kernels on ONE H100: randomized differential tests, parity suites, full-size runs, then the C4 bench line
 export CCSIM_NO_REBUILD=1
 for f in tests/test_gpu_stress.py tests/test_gpu_parity.py tests/test_gpu_sharded_one_gpu.py tests/test_gpu_fullsize.py; do
   timeout 300 python -m pytest $f -m gpu -q -x 2>&1 | tail -3

@@ -1,5 +1,5 @@
-// Microbenchmark: latency/throughput of warp arg-max primitives on sm_100a with 1 vs 24 resident warps per SM.
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o redux_bench redux_bench.cu
+// Microbenchmark: latency/throughput of warp arg-max primitives on sm_90a with 1 vs 24 resident warps per SM.
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o redux_bench redux_bench.cu
 #include <cstdio>
 #include <cuda_runtime.h>
 __device__ __forceinline__ unsigned shfl_max(unsigned v) {
@@ -23,16 +23,18 @@ template <int MODE> __global__ void k(unsigned *out, long long *cyc, int iters) 
 }
 int main() {
   unsigned *out; long long *cyc, h;
-  cudaMalloc(&out, 148 * 1024 * 4); cudaMalloc(&cyc, 8);
+  int sms = 0;
+  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, 0);     // one CTA per SM
+  cudaMalloc(&out, (size_t)sms * 1024 * 4); cudaMalloc(&cyc, 8);
   const int iters = 2000;
   const char *names[] = {"__reduce_max_sync (REDUX)", "shfl butterfly max", "ballot", "__syncthreads"};
   for (int threads : {32, 256, 768}) {
     for (int mode = 0; mode < 4; mode++) {
       for (int rep = 0; rep < 2; rep++) {
-        if (mode == 0) k<0><<<148, threads>>>(out, cyc, iters);
-        if (mode == 1) k<1><<<148, threads>>>(out, cyc, iters);
-        if (mode == 2) k<2><<<148, threads>>>(out, cyc, iters);
-        if (mode == 3) k<3><<<148, threads>>>(out, cyc, iters);
+        if (mode == 0) k<0><<<sms, threads>>>(out, cyc, iters);
+        if (mode == 1) k<1><<<sms, threads>>>(out, cyc, iters);
+        if (mode == 2) k<2><<<sms, threads>>>(out, cyc, iters);
+        if (mode == 3) k<3><<<sms, threads>>>(out, cyc, iters);
         cudaDeviceSynchronize();
       }
       cudaMemcpy(&h, cyc, 8, cudaMemcpyDeviceToHost);

@@ -1,11 +1,11 @@
-"""Markdown table of the committed bench lines (profiles/r2_bench_*.json) for README.md:  python scripts/results_table.py"""
+"""Markdown table of saved bench lines (one bench.py JSON line per file) for README.md:  python scripts/results_table.py DIR/*.json"""
 import glob
 import json
 import os
+import sys
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 rows = []
-for f in sorted(glob.glob(os.path.join(ROOT, "profiles", "r2_bench_*.json"))):
+for f in sorted(sum((glob.glob(a) for a in sys.argv[1:]), [])):
     try:
         d = json.loads(open(f).read().strip().splitlines()[-1])
     except Exception:
@@ -15,7 +15,7 @@ for f in sorted(glob.glob(os.path.join(ROOT, "profiles", "r2_bench_*.json"))):
                      d["ms_per_step"], d.get("placements_per_sec"), d["value"], None, None, None, d["cpu_baseline"]["sample"].split(" (")[0]))
         continue
     lat = d["roofline"].get("latency", {})
-    rows.append((os.path.basename(f), d["config"]["workload"].split(":")[0], "%d x B200, %s" % (d["n_gpus"], lat.get("engine", "?")), d["config"]["nodes"], d["ms_per_step"],
+    rows.append((os.path.basename(f), d["config"]["workload"].split(":")[0], "%d x H100, %s" % (d["n_gpus"], lat.get("engine", "?")), d["config"]["nodes"], d["ms_per_step"],
                  d["placements_per_sec"], d["value"], d["e2e"]["value"], lat.get("placements_per_wave"), lat.get("us_per_wave"),
                  "parity ok, %d placements%s" % (d["parity"]["checked_placements"], "" if d["parity"]["full_run"] else " (prefix)") if d.get("parity") else ""))
 print("| file | workload | arm | nodes | ms / analysis | placements/s | evals/s | e2e evals/s (flat C-ABI) | placements / wave | us / wave | check |")

@@ -1,5 +1,5 @@
-"""SASS evidence for profiles/: per-kernel instruction-mnemonic histogram of libccsim.so (cuobjdump -sass) and the lines that prove
-the bulk-async (TMA) / mbarrier / warp-reduction instructions. Run here (no GPU):  python scripts/sass_summary.py > profiles/r2_sass_summary.txt"""
+"""SASS evidence: per-kernel instruction-mnemonic histogram of libccsim.so (cuobjdump -sass) and the lines that prove the bulk-async
+(TMA) / mbarrier / warp-reduction instructions. No GPU needed:  python scripts/sass_summary.py > sass_summary.txt"""
 import collections
 import os
 import re
@@ -24,7 +24,7 @@ for line in out.splitlines():
         if re.match(r"(UBLKCP|UTMALDG|SYNCS|CREDUX|REDUX|VOTE|BAR|MEMBAR|FENCE|ST\.E\.64\.STRONG\.SYS|LD\.E\.64\.STRONG\.SYS)", op):
             if len(proof[kern]) < 400:
                 proof[kern].append(line.strip()[:120])
-print("SASS summary of", os.path.relpath(so, ROOT), "(sm_100a, nvcc %s)" % subprocess.run(["nvcc", "--version"], capture_output=True, text=True).stdout.split("release ")[-1].split(",")[0])
+print("SASS summary of", os.path.relpath(so, ROOT), "(sm_90a, nvcc %s)" % subprocess.run(["nvcc", "--version"], capture_output=True, text=True).stdout.split("release ")[-1].split(",")[0])
 for k in sorted(hist):
     tot = sum(hist[k].values())
     print("\n== %s: %d instructions" % (k, tot))

@@ -16,7 +16,7 @@ ap = argparse.ArgumentParser()
 ap.add_argument("--layout", default="contiguous")
 ap.add_argument("--m", type=int, default=8)
 ap.add_argument("--cap", type=int, default=128)
-ap.add_argument("--grid", type=int, default=148)
+ap.add_argument("--grid", type=int, default=132)
 ap.add_argument("--nodelta", action="store_true")
 ap.add_argument("--waves", type=int, default=0)
 ap.add_argument("--n", type=int, default=100_000)

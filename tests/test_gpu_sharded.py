@@ -31,7 +31,7 @@ def _worker(rank, world, port, which, q):
     elif which == "c5":            # several node-local templates: the streaming (TMA) engine over node shards
         snap, tmpl, ctr = synth.c5(n=300_001, n_templates=9)
         limit = 1500
-    elif which == "c4_wide":      # enough nodes per shard for full grids: the multi-commit replay sees 2 x 148 candidate lists
+    elif which == "c4_wide":      # enough nodes per shard for full grids: the multi-commit replay sees 2 x grid candidate lists
         snap, tmpl, ctr = synth.c4(n=120_001, n_existing=200_000, zones=32, racks=1024, regions=8)
         limit = 3000
     else:                          # spread only: nodes take several clones, winners re-enter the replay ("second life")
