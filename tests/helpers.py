@@ -39,6 +39,77 @@ def from_encoded(enc):
     return snap, ts, ctr, nd["taint_dict"], nd["scalar_names"], enc["names"]
 
 
+# ---- which kernel runs a workload ------------------------------------------------------------------------------------
+GRID_NODES, MAX_GRID = 512, 160                   # persistent grid: one CTA per SM, one per 512 nodes for small clusters
+MULTI_TILE, MULTI_M, MULTI_EPT = 768, 16, 3       # multi-commit kernel: one node per thread, 16 candidates per tile, 3 per thread
+MULTI_PAY_BITS, MULTI_GT, MULTI_IDX_BITS = 27, 6, 20
+
+
+def run_stats(eng):
+    """What the last run() of `eng` did: the kernel that ran ("engine") and its wave statistics (Engine.run_stats)."""
+    return eng.run_stats()
+
+
+def device_sm_count(device=0):
+    engine = importlib.import_module("cluster-capacity_b200.engine")
+    with engine.Engine(device=device) as eng:
+        return eng.device_info()["sm_count"]
+
+
+def persistent_grid(n, sm_count, world=1):
+    """CTAs per rank of the persistent wave kernels: sized from the largest node shard."""
+    shard = -(-n // world)
+    return max(1, min(sm_count, MAX_GRID, -(-shard // GRID_NODES)))
+
+
+def multi_eligible(snap, tmpl, ctr, sm_count):
+    """Whether ENGINE_AUTO runs this single-GPU workload on the multi-commit kernel (ccsim_multi.cuh) instead of the lean
+    sequential one. This restates the host's rule on purpose, apart from it: if the rule drifts, a test that asserts the engine
+    fails. The workload must already be lean-eligible (one template, one taint word, no PreferNoSchedule taints, counters in
+    shared memory)."""
+    if len(tmpl) != 1 or not ctr or snap.n >= 1 << MULTI_IDX_BITS or tmpl[0].n_aff:       # no required pod affinity
+        return False
+    t = tmpl[0]
+    grid = persistent_grid(snap.n, sm_count)
+    if -(-snap.n // grid) > MULTI_TILE or grid * MULTI_M > MULTI_EPT * MULTI_TILE:
+        return False
+    if any(c.inc < 0 for c in ctr):                   # feasibility must be monotone within a wave
+        return False
+    reads = [t.pts[c].counter for c in range(t.n_pts)] if t.filter_enable & abi.PL_POD_TOPOLOGY_SPREAD else []
+    reads += [t.anti_counter[a] for a in range(t.n_anti)] if t.filter_enable & abi.PL_INTER_POD_AFFINITY else []
+    if sum(ctr[j].topo_col >= 0 for j in reads) > MULTI_GT:
+        return False
+    if any(c.topo_col >= 0 and c.inc != 0 and reads.count(j) != 1 for j, c in enumerate(ctr)):
+        return False
+    bits = 0                                          # payload: dom + 1 (0..max domains) per topology column + a zero guard bit
+    for col in {c.topo_col for c in ctr if c.topo_col >= 0}:
+        bits += max([1] + [c.n_domains for c in ctr if c.topo_col == col]).bit_length() + 1
+    return bits <= MULTI_PAY_BITS
+
+
+def expected_engine(snap, tmpl, ctr, sm_count):
+    """The kernel ENGINE_AUTO picks for a lean-eligible, counter-coupled workload."""
+    return "multi-commit" if multi_eligible(snap, tmpl, ctr, sm_count) else "lean sequential"
+
+
+def sparse_eligibility_case(n, max_skew, every=40, zones=8):
+    """Identical nodes of which every `every`-th matches the template's node selector: with every >= 40 a tile of up to 640 nodes has
+    at most 16 feasible nodes, so no tile has unseen candidates and the replay bar comes from the best key alone; all keys share one
+    score. Required anti-affinity on the hostname (a node takes one clone) and a zone spread constraint with the given maxSkew."""
+    i = np.arange(n)
+    static = (i % every == 0).astype(np.uint64)
+    zone = ((i // every) % zones).astype(np.int32)
+    snap = abi.Snapshot(n, np.full(n, 8000), np.full(n, 16 << 30), np.full(n, 110), static_mask=static.reshape(1, n), topo=[zone])
+    ctr = [abi.make_counter(0, np.zeros(zones, np.int32), inc=1), abi.make_counter(-1, np.zeros(n, np.int32), inc=1)]
+    t = abi.default_template(100, 128 << 20)
+    t.flags |= abi.TF_HAS_NODE_SELECTOR
+    t.sel_mask[0] = 1
+    t.n_pts = 1
+    t.pts[0].counter, t.pts[0].max_skew, t.pts[0].self_match, t.pts[0].min_zero = 0, max_skew, 1, 0
+    t.n_anti, t.anti_counter[0] = 1, 1
+    return snap, [t], ctr
+
+
 def reason_text(r, taint_dict, scalar_names):
     if r < abi.R_FIXED_COUNT:
         return abi.REASON_TEXT[r]

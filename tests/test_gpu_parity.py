@@ -5,6 +5,8 @@ import importlib
 import numpy as np
 import pytest
 
+import helpers
+
 abi = importlib.import_module("cluster-capacity_b200._abi")
 synth = importlib.import_module("cluster-capacity_b200.synth")
 from oracle import binding as oracle  # noqa: E402
@@ -13,21 +15,26 @@ pytestmark = pytest.mark.gpu
 GiB, MiB = 1 << 30, 1 << 20
 
 
-def gpu_run(snap, tmpl, ctr=(), max_pods=0, engine_kind=abi.ENGINE_SEQUENTIAL):
+def gpu_run(snap, tmpl, ctr=(), max_pods=0, engine_kind=abi.ENGINE_SEQUENTIAL, stats=None):
+    """One run; `stats`, when given, is a dict that receives the run's statistics (helpers.run_stats)."""
     engine = importlib.import_module("cluster-capacity_b200.engine")
     with engine.Engine(device=0, engine=engine_kind) as eng:
         eng.load_nodes(snap)
         eng.set_templates(tmpl, ctr)
         res = eng.run(max_pods)
         counts, first = eng.node_counts(0)
+        if stats is not None:
+            stats.update(helpers.run_stats(eng), sm_count=eng.device_info()["sm_count"])
     return res, counts, first
 
 
-def check(snap, tmpl, ctr=(), max_pods=0, threads=4):
+def check(snap, tmpl, ctr=(), max_pods=0, threads=4, auto_engine=None):
     """Sequential engine (one winner per wave: evals/waves equal the reference-equivalent count) AND the default engine
-    (AUTO: batched tie-run waves when the template is node-local) against the oracle."""
+    (AUTO: batched tie-run waves when the template is node-local) against the oracle. `auto_engine`: the kernel AUTO must run."""
     want = oracle.run(snap, tmpl, ctr, max_pods=max_pods, threads=threads)
-    auto, acounts, _ = gpu_run(snap, tmpl, ctr, max_pods, abi.ENGINE_AUTO)
+    stats = {}
+    auto, acounts, _ = gpu_run(snap, tmpl, ctr, max_pods, abi.ENGINE_AUTO, stats)
+    assert auto_engine is None or stats["engine"] == auto_engine, stats
     assert auto.placed == want.placed and auto.stop_code == want.stop_code
     assert np.array_equal(auto.pod_node, want.pod_node), "AUTO engine: placement sequence differs from the oracle"
     assert np.array_equal(auto.reason_hist, want.reason_hist)
@@ -287,7 +294,9 @@ def test_multi_commit_waves_match_the_sequential_loop(built, limit):
     per exchange, pod -> node sequence identical to one-winner-per-wave, --max-limit cuts in the middle of a wave."""
     snap, tmpl, ctr = synth.c4(n=60000, n_existing=90000, zones=32, racks=512, regions=8)
     want = oracle.run(snap, tmpl, ctr, max_pods=limit or 2500, threads=8)
-    got, counts, _ = gpu_run(snap, tmpl, ctr, limit or 2500, abi.ENGINE_AUTO)
+    stats = {}
+    got, counts, _ = gpu_run(snap, tmpl, ctr, limit or 2500, abi.ENGINE_AUTO, stats)
+    assert stats["engine"] == helpers.expected_engine(snap, tmpl, ctr, stats["sm_count"]) == "multi-commit", stats
     assert got.placed == want.placed and got.stop_code == want.stop_code
     assert np.array_equal(got.pod_node, want.pod_node)
     if got.placed > 100:
@@ -312,5 +321,5 @@ def test_multi_commit_zone_anti_affinity_and_missing_keys(built):
     t.anti_counter[0] = 0
     t.n_pts = 1
     t.pts[0].counter, t.pts[0].max_skew, t.pts[0].self_match, t.pts[0].min_zero = 1, 3, 1, 0
-    got = check(snap, [t], ctr)
+    got = check(snap, [t], ctr, auto_engine="multi-commit")
     assert got.stop_code == abi.STOP_UNSCHEDULABLE and got.placed > 200   # nodes without the zone label are not bound by the anti-affinity term

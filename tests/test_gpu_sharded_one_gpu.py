@@ -9,6 +9,8 @@ import threading
 import numpy as np
 import pytest
 
+import helpers
+
 abi = importlib.import_module("cluster-capacity_b200._abi")
 synth = importlib.import_module("cluster-capacity_b200.synth")
 from oracle import binding as oracle  # noqa: E402
@@ -53,7 +55,11 @@ CASES = {
     "c4_limit": (lambda: synth.c4(n=9000, n_existing=15000, zones=16, racks=128, regions=4), 700, "multi-commit"),
     "spread": (lambda: (lambda s, t, c: (s, [_no_anti(t[0])], c[:3]))(*synth.c4(n=7000, n_existing=9000, zones=8, racks=64, regions=4)), 900, "multi-commit"),
     "c5": (lambda: synth.c5(n=9001, n_templates=9), 1200, "streaming"),
+    # every 40th node feasible, one score for all: each rank publishes more than 256 candidates (40 CTAs per rank at world 2), so the
+    # bar is raised on the ranks and again over the union of their summaries (at world 4 the union alone overflows)
+    "sparse": (lambda: helpers.sparse_eligibility_case(40000, max_skew=10 ** 6), 500, "multi-commit"),
 }
+BAR_RAISED = {"sparse"}
 
 
 def _no_anti(t):
@@ -61,11 +67,19 @@ def _no_anti(t):
     return t
 
 
+@pytest.fixture(scope="module")
+def sm_count(built):
+    return helpers.device_sm_count()
+
+
 @pytest.mark.parametrize("world", [2, 4])
 @pytest.mark.parametrize("which", sorted(CASES))
-def test_sharded_engines_on_one_gpu_match_the_oracle(built, which, world):
+def test_sharded_engines_on_one_gpu_match_the_oracle(built, sm_count, which, world):
     make, limit, engine_name = CASES[which]
     snap, tmpl, ctr = make()
+    grid = helpers.persistent_grid(snap.n, sm_count, world)     # the ranks' persistent grids run side by side on this one device
+    if world * grid > sm_count:
+        pytest.skip("%d ranks x %d CTAs do not fit on %d SMs" % (world, grid, sm_count))
     runs = [limit, (limit or 0) // 2 + 7, limit]        # several runs per handle: epoch / buffer parity carry over
     wants = [oracle.run(snap, tmpl, ctr, max_pods=lim, threads=4, memo=True) for lim in runs]
     for kind in (abi.ENGINE_AUTO, abi.ENGINE_SEQUENTIAL):
@@ -82,3 +96,5 @@ def test_sharded_engines_on_one_gpu_match_the_oracle(built, which, world):
                 assert sum(r.evals for r in res) == w.evals
             elif engine_name:
                 assert all(engine_name in s["engine"] for s in stats), stats
+                if which in BAR_RAISED:
+                    assert all(s["bar_raised_waves"] > 0 for s in stats), stats

@@ -1,22 +1,34 @@
-"""GPU: randomized differential test of the engines ENGINE_AUTO picks (multi-commit waves, tie-run batching, lean, generic) against the
-CPU oracle: spread / anti-affinity templates with random domain counts, skews, self-match flags, missing labels, minDomains, limits."""
+"""Randomized differential tests of the engines ENGINE_AUTO picks (multi-commit waves, tie-run batching, lean, generic) against the
+CPU oracle: spread / anti-affinity templates with random domain counts, skews, self-match flags, missing labels, minDomains, limits.
+The coupled-template tests also assert which kernel ran; a CPU test checks that the generator keeps reaching the multi-commit one."""
 import importlib
 
 import numpy as np
 import pytest
 
+import helpers
+
 abi = importlib.import_module("cluster-capacity_b200._abi")
 from oracle import binding as oracle  # noqa: E402
 
-pytestmark = pytest.mark.gpu
 GiB, MiB = 1 << 30, 1 << 20
+H100_SXM_SMS = 132
 
 
-def random_case(seed):
+@pytest.fixture(scope="module")
+def sm_count(built):
+    return helpers.device_sm_count()
+
+
+def random_case(seed, sm_count):
+    """A counter-coupled workload. Cluster sizes run from one CTA to the largest cluster the multi-commit kernel takes on this
+    device (sm_count x 768 nodes: every tile full) and one node past it (the lean sequential kernel). Domain counts of 2^b - 1
+    make the last domain's payload field all ones; 2^b needs one more bit."""
     rng = np.random.default_rng(1000 + seed)
-    n = int(rng.choice([200, 600, 3000, 9000, 40000, 90000, 110000]))      # 1 CTA ... the largest tile the multi-commit kernel takes
+    largest = sm_count * helpers.MULTI_TILE
+    n = int(rng.choice([200, 600, 3000, 9000, 40000, 90000, largest - 1, largest, largest + 1], p=[.1, .1, .1, .1, .1, .1, .15, .2, .05]))
     n_topo = int(rng.integers(1, 4))
-    doms = [int(rng.choice([3, 8, 40, 300, 2000])) for _ in range(n_topo)]
+    doms = [int(rng.choice([3, 7, 8, 40, 255, 256, 300, 2000, 2047], p=[.14, .14, .14, .14, .12, .12, .1, .05, .05])) for _ in range(n_topo)]
     topo = []
     for d in doms:
         col = rng.integers(0, d, n).astype(np.int32)
@@ -53,9 +65,18 @@ def random_case(seed):
     return snap, [t], ctr, limit
 
 
+def test_random_cases_reach_the_multi_commit_kernel():
+    """At least 42 of the 48 coupled cases run on the multi-commit kernel of an H100 SXM, and at least one is a deliberate fallback:
+    a change to the generator must not quietly move the stress tests back onto the lean kernel."""
+    elig = [helpers.multi_eligible(*random_case(seed, H100_SXM_SMS)[:3], H100_SXM_SMS) for seed in range(48)]
+    assert sum(elig) >= 42, [s for s, e in enumerate(elig) if not e]
+    assert not all(elig)
+
+
+@pytest.mark.gpu
 @pytest.mark.parametrize("seed", range(48))
-def test_random_coupled_templates(built, seed):
-    snap, tmpl, ctr, limit = random_case(seed)
+def test_random_coupled_templates(built, sm_count, seed):
+    snap, tmpl, ctr, limit = random_case(seed, sm_count)
     cap = limit or 4000                               # keep the single-thread oracle in seconds
     want = oracle.run(snap, tmpl, ctr, max_pods=cap, threads=8)
     engine = importlib.import_module("cluster-capacity_b200.engine")
@@ -64,17 +85,21 @@ def test_random_coupled_templates(built, seed):
             eng.load_nodes(snap)
             eng.set_templates(tmpl, ctr)
             got = eng.run(cap)
+            stats = helpers.run_stats(eng)
         assert got.placed == want.placed and got.stop_code == want.stop_code, (seed, kind)
         assert np.array_equal(got.pod_node, want.pod_node), (seed, kind)
         assert np.array_equal(got.reason_hist, want.reason_hist), (seed, kind)
+        if kind == abi.ENGINE_AUTO:
+            assert stats["engine"] == helpers.expected_engine(snap, tmpl, ctr, sm_count), (seed, snap.n, stats)
 
 
+@pytest.mark.gpu
 @pytest.mark.parametrize("seed", range(48))
-def test_random_coupled_templates_forced_look_ahead(built, seed, monkeypatch):
+def test_random_coupled_templates_forced_look_ahead(built, sm_count, seed, monkeypatch):
     """The multi-commit kernel with its look-ahead forced on for every PodTopologySpread term in every wave (CCSIM_DEBUG_FLAGS=32):
     candidates published from closed cells start dormant, wake up when a minimum move lifts the limit over their cell, crowd the
     tiles' lists (waves without a placement are repeated strictly) — the pod -> node sequence must not change."""
-    snap, tmpl, ctr, limit = random_case(seed)
+    snap, tmpl, ctr, limit = random_case(seed, sm_count)
     cap = limit or 4000
     want = oracle.run(snap, tmpl, ctr, max_pods=cap, threads=8)
     engine = importlib.import_module("cluster-capacity_b200.engine")
@@ -83,6 +108,8 @@ def test_random_coupled_templates_forced_look_ahead(built, seed, monkeypatch):
         eng.load_nodes(snap)
         eng.set_templates(tmpl, ctr)
         got = eng.run(cap)
+        stats = helpers.run_stats(eng)
+    assert stats["engine"] == helpers.expected_engine(snap, tmpl, ctr, sm_count), (seed, snap.n, stats)
     assert got.placed == want.placed and got.stop_code == want.stop_code, seed
     assert np.array_equal(got.pod_node, want.pod_node), seed
     assert np.array_equal(got.reason_hist, want.reason_hist), seed
@@ -131,6 +158,7 @@ def random_node_local_case(seed):
     return snap, tmpl, [], int(rng.choice([0, 0, 0, 57, 333, 5000]))
 
 
+@pytest.mark.gpu
 @pytest.mark.parametrize("seed", range(16))
 def test_random_node_local_templates(built, seed):
     snap, tmpl, ctr, limit = random_node_local_case(seed)
