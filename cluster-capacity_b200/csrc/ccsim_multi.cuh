@@ -33,8 +33,11 @@
 //                and polls its local copy — an all-gather of world x grid lines fused into the persistent kernel.
 // Replay: ONE warp, no barrier inside: <= 8 candidates per lane in registers; a round is arg-max (REDUX) -> commit (lane q =
 //   counter term q: cell += inc, over-limit test, PTS-minimum tracking, all from registers) -> kill the candidates sitting in
-//   a cell that just filled (field compare against the shuffled cell id). ~250 cycles per reference cycle instead of the
-//   ~2000 of a block-wide round (two barriers over 24 warps); the other 23 warps wait at the barrier that ends the wave.
+//   a cell that just filled (SWAR field test against the OR-reduced filled cells). Measured on C4 (one H100 80GB HBM3, 400 W
+//   power limit, CCSIM_DEBUG_FLAGS=8: replay cycles minus set-up over rounds, so minimum moves, wake-ups and the hand-off after
+//   the loop are included): ~890 cycles per reference cycle, ~1 310 before the round was cut down to its dependent chain
+//   (three REDUX, one LDS/STS) — against ~2000 for a block-wide round (two barriers over 24 warps). The other 23 warps wait at
+//   the barrier that ends the wave. -DMULTI_ROUND_PROFILE splits those cycles (scripts/round_profile.sh).
 //   Row updates of the winners are done by each node's own thread after that barrier (a thread owns its node).
 // Look-ahead waves: a PodTopologySpread minimum move that REOPENS closed domains would end the wave (the reopened nodes were
 //   rejected by the scan and are in nobody's list). When a term's limit is about to move, the scan publishes the nodes of its
@@ -65,6 +68,25 @@
 static_assert(MULTI_M == SLOT_STRIDE, "the keys of a CTA's list fill exactly one slot line");
 static_assert(4 + 2 * MULTI_CAP <= CCSIM_MAX_GRID * SLOT_STRIDE, "node shards: a rank's summary fits its region of the line buffer");
 
+// Round profile (profiling builds only: -DMULTI_ROUND_PROFILE; the hooks expand to nothing otherwise, and the shipped library's
+// SASS is the same with and without them). CTA 0's replay warp adds up, over the run, the cycles of: the common round (arg-max ->
+// commit -> kill), the minimum-move handling of each term, the rebuilds, and what follows the loop (the hand-off of the winners to
+// their threads, the look-ahead decision, barrier R); and the events: rounds, minimum moves per term, rebuilds, rounds that kill.
+// The kernel prints the table when the run ends (scripts/round_profile.sh).
+#define RP_ROUND 0
+#define RP_REBUILD 1
+#define RP_AFTER 2
+#define RP_KILL 3                 /* (event count only) */
+#define RP_MINMOVE 4              /* + term q */
+#define RP_N (RP_MINMOVE + MULTI_GT)
+#ifdef MULTI_ROUND_PROFILE
+#define RPROF(...) __VA_ARGS__
+#define RP_ADD(i, cyc, n) do { if (cta == 0 && lane == 0) { ms.rp_cyc[i] += (cyc); ms.rp_cnt[i] += (n); } } while (0)
+#else
+#define RPROF(...)
+#define RP_ADD(i, cyc, n) do { } while (0)
+#endif
+
 // cross-GPU line buffers inside every rank's exchange allocation (64-bit words): [parity][source rank][CTA][16]
 #define XLEAN_WORDS (2 * CCSIM_MAX_WORLD * SLOT_STRIDE)
 #define XLINES_OFF XLEAN_WORDS
@@ -90,6 +112,9 @@ struct __align__(16) MultiShared {
   int32_t relax[LEAN_MAX_TERMS];                    // per Filter term: this wave's look-ahead over the limit (0: strict), see "dormant candidates"
   int32_t force_strict, st_relaxed, st_empty, pad_r;
   long long ph[8], tc0, st_cand, st_overflow, st_rounds;       // CTA 0 / thread 0: clock cycles per phase, replay statistics
+#ifdef MULTI_ROUND_PROFILE
+  long long rp_cyc[RP_N], rp_cnt[RP_N], rp_t;                  // CTA 0's replay warp: cycles and events per part of the replay
+#endif
 };
 
 __shared__ MultiShared ms;
@@ -198,7 +223,8 @@ __global__ void __launch_bounds__(LEAN_THREADS, 1) ccsim_wave_multi_kernel(const
   }
   if (tid == 0) { ls.aff_total = p.templates[0].aff_total_init; ls.winner = -1; ls.stop = 0; ls.dirty = 1; ms.accepted = 0; ms.dead = 0; ms.stopb = 0; ms.n_gt = 0; ms.ncand = 0; ms.delta = 1u << MULTI_IDX_BITS; ms.force_strict = 0; ms.st_relaxed = 0; ms.st_empty = 0;
                   for (int q = 0; q < LEAN_MAX_TERMS; q++) ms.relax[q] = 0;
-                  for (int q = 0; q < 8; q++) ms.ph[q] = 0; ms.tc0 = 0; ms.st_cand = 0; ms.st_overflow = 0; ms.st_rounds = 0; }
+                  for (int q = 0; q < 8; q++) ms.ph[q] = 0; ms.tc0 = 0; ms.st_cand = 0; ms.st_overflow = 0; ms.st_rounds = 0;
+                  RPROF(for (int q = 0; q < RP_N; q++) ms.rp_cyc[q] = ms.rp_cnt[q] = 0; ms.rp_t = 0;) }
   ms.mult[tid] = 0;
   __syncthreads();
   for (int c = 0; c < ls.tmpl.n_pts; c++) lean_pts_recount(p, smem_cnt, c);
@@ -567,9 +593,15 @@ __global__ void __launch_bounds__(LEAN_THREADS, 1) ccsim_wave_multi_kernel(const
         // commits this wave may still decide: --max-limit (simulator.go:300-305), the output capacity, MULTI_MAX_ACC
         long long room = p.pod_cap - k;
         if (p.max_pods > 0 && p.max_pods - k < room) room = p.max_pods - k;
-        const int32_t acc_limit = room < MULTI_MAX_ACC ? (int32_t)room : MULTI_MAX_ACC;
-        int rounds = 0;
+        // (pinned: recomputing it from the kernel parameters inside the round costs two constant loads and a 64-bit compare)
+        const int32_t acc_limit = (int32_t)pin_u32(room < MULTI_MAX_ACC ? (uint32_t)room : (uint32_t)MULTI_MAX_ACC);
         bool ended_by_rescan = false;
+        // the round's per-lane constants: this lane's term field in the payload, in place, and its guard bit; whether the term
+        // tracks a PTS minimum; the lowest key that may still win (0 never does)
+        const uint32_t fmask = (uint32_t)c1.z << c1.y, fglane = ((uint32_t)c1.z + 1u) << c1.y;
+        const bool trk = (gc.y != 0) & (gc.z >= 0);
+        const uint32_t Tr = T > 1u ? T : 1u;
+        const uint32_t cnext_sa = pin_u32(MS_SA(cnext) + 4u * (uint32_t)lane);   // this lane's column of the second-life keys
         // ---- dormant candidates. A PTS term whose limit is about to move (few domains left at the global minimum) was scanned with
         //      a look-ahead (ms.relax): nodes in cells up to MULTI_RELAX_R over the limit are in the lists too. They cannot win while
         //      their cell is over the limit (dormant: key 0 in ck[], like a dead candidate) and wake up when a minimum move lifts the
@@ -600,84 +632,97 @@ __global__ void __launch_bounds__(LEAN_THREADS, 1) ccsim_wave_multi_kernel(const
         }
         if (cta == 0 && lane == 0) ms.ph[6] += clock64() - ms.tc0;      // replay set-up
         for (;;) {
+          RPROF(long long rp_t0 = clock64(), rp_mm = 0;)
           if (need_rebuild) {       // (one call site, off the round's critical path; see "dormant candidates")
             need_rebuild = false;
             __syncwarp();           // the counter cells / limits written by the term lanes, before every lane reads them
+            // (every load of a pass is issued before its first use, and none sits behind a branch: the loads overlap)
             uint32_t badm = 0u;
             #pragma unroll 1
             for (int q = 0; q < n_gt; q++) {
               const int4 tg = *reinterpret_cast<const int4 *>(&ms.gt_commit[q][0]);   // {cnt_off, inc, pts_idx, n_present}
               const int4 tc = *reinterpret_cast<const int4 *>(&ms.gt_c1[q][0]);       // {lim (kept current by lane q), shift, mask, n_domains}
+              int32_t cv[MULTI_CPT];
               #pragma unroll
               for (int j = 0; j < MULTI_CPT; j++) {
-                const int32_t v = (int32_t)((cd[j] >> tc.y) & (uint32_t)tc.z) - 1;
-                if (v >= 0 && lds_s32(cnt_sa + 4u * (uint32_t)(tg.x + v)) > tc.x) badm |= 1u << j;
+                const int32_t v = (int32_t)((cd[j] >> tc.y) & (uint32_t)tc.z) - 1;   // (-1: no domain; cell 0 is read and ignored)
+                cv[j] = lds_s32(cnt_sa + 4u * (uint32_t)(tg.x + max(v, 0)));
               }
+              #pragma unroll
+              for (int j = 0; j < MULTI_CPT; j++) {
+                const bool has = ((cd[j] >> tc.y) & (uint32_t)tc.z) != 0u;
+                badm |= (uint32_t)(has & (cv[j] > tc.x)) << j;
+              }
+            }
+            uint32_t k0[MULTI_CPT], k1[MULTI_CPT];
+            #pragma unroll
+            for (int j = 0; j < MULTI_CPT; j++) {   // (j * 32 + lane < MULTI_CAP: in bounds; slots >= C are ignored below)
+              k0[j] = (uint32_t)lds_s32(MS_SA(ckey) + 4u * (uint32_t)(j * 32 + lane));
+              k1[j] = (uint32_t)lds_s32(MS_SA(cnext) + 4u * (uint32_t)(j * 32 + lane));
             }
             #pragma unroll
             for (int j = 0; j < MULTI_CPT; j++) {
-              const int idx = j * 32 + lane;
-              uint32_t base = 0u;
-              if (idx < C && !((badm >> j) & 1u)) {
-                const uint32_t k0 = (uint32_t)lds_s32(MS_SA(ckey) + 4u * (uint32_t)idx);
-                if (!((second >> j) & 1u)) base = k0;
-                else if (!single_use) { const uint32_t ns = (uint32_t)lds_s32(MS_SA(cnext) + 4u * (uint32_t)idx); base = ns ? ((ns << MULTI_IDX_BITS) | (k0 & MULTI_IDX_MASK)) : 0u; }
-              }
-              ck[j] = base;
+              const uint32_t life2 = (single_use || k1[j] == 0u) ? 0u : ((k1[j] << MULTI_IDX_BITS) | (k0[j] & MULTI_IDX_MASK));
+              const uint32_t base = ((second >> j) & 1u) ? life2 : k0[j];
+              ck[j] = (j * 32 + lane < C && !((badm >> j) & 1u)) ? base : 0u;
             }
+            RPROF(const long long rp_t1 = clock64(); RP_ADD(RP_REBUILD, rp_t1 - rp_t0, 1); rp_t0 = rp_t1;)
           }
-          rounds++;
+          // ---- the round: only its dependent chain — arg-max (REDUX) -> owner's payload (REDUX) -> counter cells (LDS/STS) -> filled
+          //      cells and "a minimum moved" (REDUX) -> kill. No branch is divergent on the common path: every lane runs the same code
+          //      and predication selects; the work that does not depend on the arg-max (the lane's best slot, its payload, its
+          //      next-life key) overlaps the REDUX. ----
           uint32_t m = ck[0];
           #pragma unroll
           for (int j = 1; j < MULTI_CPT; j++) m = max(m, ck[j]);
-          const uint32_t g = __reduce_max_sync(0xffffffffu, m);
-          if (g == 0u || g < T) { ran_dry = true; break; }      // nothing left, or an unseen node could rank above g
+          const uint32_t g = __reduce_max_sync(0xffffffffu, m);     // (issued first: what follows up to the test of g fills its latency)
+          // this lane's best slot: its payload, with the slot index in bits 27..29 and "this slot has won before" in bit 31 (keys are
+          // unique, so when m != 0 exactly one slot matches; when m == 0 the lane is not the owner and the value is not used)
+          uint32_t pm = 0u;
+          #pragma unroll
+          for (int j = 0; j < MULTI_CPT; j++)
+            pm |= (ck[j] == m) ? (cd[j] | ((uint32_t)j << MULTI_PAY_BITS) | (((second >> j) & 1u) << 31)) : 0u;
+          const uint32_t ns = (uint32_t)lds_s32(cnext_sa + 128u * ((pm >> MULTI_PAY_BITS) & 7u));   // (read ahead: used after the next REDUX)
+          if (g < Tr) { ran_dry = true; RP_ADD(RP_ROUND, clock64() - rp_t0, 1); break; }      // nothing left (g == 0), or an unseen node could rank above g
           // ---- commit pod k+acc (assume -> AssumePod -> NodeInfo.update(+1): schedule_one.go:967-984, types.go:409-427) ----
           // the owner lane contributes the winner's payload (keys are unique: exactly one lane and slot match)
-          uint32_t dsel = 0u;
-          #pragma unroll
-          for (int j = 0; j < MULTI_CPT; j++) dsel = (ck[j] == g) ? cd[j] : dsel;
-          const uint32_t pay = __reduce_or_sync(0xffffffffu, dsel);
+          const uint32_t pay = __reduce_or_sync(0xffffffffu, m == g ? pm : 0u);
+          // the key the winning slot has after the win: its second life, or 0 (single-use template, second win, or the node takes
+          // no further clone)
+          const uint32_t nk = (single_use | (ns == 0u) | (pm >> 31)) ? 0u : ((ns << MULTI_IDX_BITS) | (m & MULTI_IDX_MASK));
           // the winner comes back once with the key it has after this clone (if it still fits); when a node wins for the second
-          // time in a wave its third key is unknown: the wave ends after that commit
-          bool sec = false;
-          if (single_use) {           // a clone blocks its own node (hostname anti-affinity): the winner just leaves
-            #pragma unroll
-            for (int j = 0; j < MULTI_CPT; j++) { const bool w = ck[j] == g; ck[j] = w ? 0u : ck[j]; second |= (uint32_t)w << j; }   // (bit j: this slot has won — a rebuild leaves it out)
-          } else {
-            #pragma unroll
-            for (int j = 0; j < MULTI_CPT; j++)
-              if (ck[j] == g) {
-                sec = (second >> j) & 1u;
-                const uint32_t ns = sec ? 0u : (uint32_t)lds_s32(MS_SA(cnext) + 4u * (uint32_t)(j * 32 + lane));
-                ck[j] = ns ? ((ns << MULTI_IDX_BITS) | (g & MULTI_IDX_MASK)) : 0u;
-                second |= 1u << j;
-              }
-          }
+          // time in a wave its third key is unknown: the wave ends after that commit (bit 31 of pay). A single-use clone blocks
+          // its own node (hostname anti-affinity): the winner just leaves. Bit j of `second`: slot j has won.
+          #pragma unroll
+          for (int j = 0; j < MULTI_CPT; j++) ck[j] = (ck[j] == g) ? nk : ck[j];
+          second |= (uint32_t)(m == g) << ((pm >> MULTI_PAY_BITS) & 7u);
           // Only what the next round depends on happens here: the counter cells of the winner's domains (lane q = term q; the
           // host guarantees one term per incremented replicated counter), whether a cell went over its limit, whether a PTS
           // minimum moved. The winner's row (NodeInfo.update, node-local counters) is brought up to date by its own thread after the wave.
-          bool minchg = false;
-          uint32_t fullf = 0u;
-          if (lane < n_gt) {
-            const int32_t v = (int32_t)((pay >> c1.y) & (uint32_t)c1.z) - 1;
-            if (v >= 0) {
-              const uint32_t ca = cnt_sa + 4u * (uint32_t)(gc.x + v);
-              const int32_t old = lds_s32(ca), nv = old + gc.y;
-              sts_s32(ca, nv);
-              if (nv > c1.x) fullf = ((uint32_t)(v + 1) | ((uint32_t)c1.z + 1u)) << c1.y;   // candidates in this cell are dead from now on (+ the field's guard bit)
-              if (gc.y && gc.z >= 0 && v < gc.w && old == my_min) { my_num--; minchg = my_num <= 0; }   // the global minimum of this constraint moves: limits change, rescan
-            }
-          }
+          // (lanes >= n_gt have a zero field mask: no domain, nothing written)
+          const uint32_t fpay = pay & fmask;                     // the winner's field of this lane's term, in place
+          const bool has = fpay != 0u;
+          const uint32_t ca = cnt_sa + 4u * (uint32_t)(gc.x + max((int32_t)(fpay >> c1.y) - 1, 0));
+          const int32_t old = lds_s32(ca), nv = old + gc.y;
+          if (has) sts_s32(ca, nv);
+          // candidates in a cell that went over its limit are dead from now on: its field, with the field's guard bit
+          const uint32_t fullf = (has & (nv > c1.x)) ? (fpay | fglane) : 0u;
+          const bool atmin = has & trk & ((int32_t)(fpay >> c1.y) - 1 < gc.w) & (old == my_min);   // a domain leaves the global minimum ...
+          my_num -= (int32_t)atmin;
+          const bool minchg = atmin & (my_num <= 0);                                                  // ... the last one: the minimum moves
           if (lane == 0) sts_s32(MS_SA(acc_node) + 4u * (uint32_t)acc, ckey_index(g));
           acc++;
+          // one OR-reduction carries the filled cells (the fields of different terms are disjoint bit ranges) and, in bit 31, that
+          // some term's minimum moved
+          const uint32_t F = __reduce_or_sync(0xffffffffu, fullf | ((uint32_t)minchg << 31));
           // A PTS minimum moved (filtering.go:56-69: minMatchNum): recount it and move the term's limit. The wave goes on unless
           // the move changes some node's feasibility: that takes a domain whose count lies in (old limit, new limit] — nodes there
           // were rejected by the scan (or killed earlier in this wave) and pass now. Without such a domain every verdict so far
           // stands (the 8-region constraint of C4 moves its minimum every 8 placements and never binds).
           bool rescan = false, woke = false;
-          const unsigned mc = __ballot_sync(0xffffffffu, minchg);
+          const unsigned mc = (F >> 31) ? __ballot_sync(0xffffffffu, minchg) : 0u;
           for (unsigned nm = mc; nm; nm &= nm - 1) {
+            RPROF(const long long rp_m0 = clock64();)
             const int q = __ffs(nm) - 1;
             const int32_t off = __shfl_sync(0xffffffffu, gc.x, q), npres = __shfl_sync(0xffffffffu, gc.w, q), ndom = __shfl_sync(0xffffffffu, c1.w, q);
             const int32_t lim_old = __shfl_sync(0xffffffffu, c1.x, q), loff = __shfl_sync(0xffffffffu, lim_off, q);
@@ -699,28 +744,30 @@ __global__ void __launch_bounds__(LEAN_THREADS, 1) ccsim_wave_multi_kernel(const
             if (rq) { rescan |= (lim_new >= __shfl_sync(0xffffffffu, unpub_min, q)) | (p.debug_flags & 1); woke = true; }
             else rescan |= __any_sync(0xffffffffu, hit) | (p.debug_flags & 1);
             if (lane == q) { my_min = mn; my_num = num; c1.x = lim_new; lim_moved = true; sts_s32(MS_SA(gt_c1) + 16u * (uint32_t)q, lim_new); }
+            RPROF(__syncwarp(); const long long rp_m1 = clock64(); RP_ADD(RP_MINMOVE + q, rp_m1 - rp_m0, 1); rp_mm += rp_m1 - rp_m0;)
           }
           need_rebuild = woke & !rescan;
           // (no statistics, special registers or kernel parameters are touched inside the round loop: one S2R on this dependent
           //  chain costs as much as ten ALU instructions)
-          bool stopb = __any_sync(0xffffffffu, sec) | rescan;
-          if (stopb | (acc >= acc_limit)) { ended_by_rescan = rescan; break; }
+          if ((pay >> 31) | rescan | (acc >= acc_limit)) { ended_by_rescan = rescan; RP_ADD(RP_ROUND, clock64() - rp_t0 - rp_mm, 1); break; }
           // only the candidates sitting in a counter cell that this commit pushed over its limit die (monotone: for the rest of
-          // the wave); the fields of different terms are disjoint bit ranges, so one OR-reduction carries all filled cells, each
-          // with its field's guard bit (the rebuild at the top of the next round sets every candidate as counters and limits stand
-          // by then — `fullf` was taken against the limits before the move)
-          const uint32_t F = woke ? 0u : __reduce_or_sync(0xffffffffu, fullf);
-          if (F) {
+          // the wave) (the rebuild at the top of the next round sets every candidate as counters and limits stand by then —
+          // `fullf` was taken against the limits before the move)
+          const uint32_t Fc = woke ? 0u : (F & ((1u << MULTI_PAY_BITS) - 1u));
+          if (Fc) {
             // One SWAR test per candidate instead of a compare per term: x = cd ^ (filled cells) is zero in a field exactly where
             // the candidate sits in the filled cell of that term. With every guard bit set, subtracting the fields' lowest bits
             // borrows a guard bit away exactly in the zero fields, and the guard stops the borrow there.
-            const uint32_t fv = F & ~fguard, fg = F & fguard;
+            const uint32_t fv = pin_u32(Fc & ~fguard), fg = Fc & fguard;
             #pragma unroll
             for (int j = 0; j < MULTI_CPT; j++)
               if (~(((cd[j] ^ fv) | fguard) - flsb) & fg) ck[j] = 0u;    // (dead — in a look-ahead wave: dormant, a rebuild may bring it back)
+            RP_ADD(RP_KILL, 0, 1);
           }
+          RP_ADD(RP_ROUND, clock64() - rp_t0 - rp_mm, 1);
         }
-        if (cta == 0 && lane == 0) { ms.st_rounds += rounds; if (ended_by_rescan) ms.ph[7] += 1; }      // (ph[7]: waves ended by a minimum move that changes verdicts)
+        RPROF(if (cta == 0 && lane == 0) ms.rp_t = clock64();)
+        if (cta == 0 && lane == 0) { ms.st_rounds += acc + (int)ran_dry; if (ended_by_rescan) ms.ph[7] += 1; }      // (ph[7]: waves ended by a minimum move that changes verdicts)
         // the winners of this CTA's tile, handed to their threads for the row updates after barrier R (a node may be accepted
         // twice: second life)
         __syncwarp();
@@ -771,6 +818,7 @@ __global__ void __launch_bounds__(LEAN_THREADS, 1) ccsim_wave_multi_kernel(const
       }
     }
     __syncthreads();                                                    // R: the accepted list, counters, limits
+    RPROF(if (cta == 0 && tid == 0 && ms.rp_t) { ms.rp_cyc[RP_AFTER] += clock64() - ms.rp_t; ms.rp_cnt[RP_AFTER]++; ms.rp_t = 0; })
     MPH_MARK(4);
     const int32_t acc = ms.accepted;
     // ClusterCapacityBinder.Bind + postBindHook: pod k+i -> node (plugin.go:34-53; simulator.go:297-312). Every CTA knows the
@@ -838,6 +886,21 @@ __global__ void __launch_bounds__(LEAN_THREADS, 1) ccsim_wave_multi_kernel(const
         printf("multi-commit replay: waves %lld rounds %lld look-ahead waves %d (without a placement: %d) | cycles: replay %lld set-up %lld, per round %.0f\n",
                limit_hit ? wv : wv + 1, ms.st_rounds, ms.st_relaxed, ms.st_empty, ms.ph[4], ms.ph[6],
                (double)(ms.ph[4] - ms.ph[6]) / (double)(ms.st_rounds > 0 ? ms.st_rounds : 1));
+#ifdef MULTI_ROUND_PROFILE
+      {
+        const double w = (double)(limit_hit ? wv : wv + 1), nr = (double)(ms.st_rounds > 0 ? ms.st_rounds : 1);
+        printf("round profile (CTA 0): waves %.0f rounds %lld | replay %.0f cycles/wave, set-up %.0f\n", w, ms.st_rounds, ms.ph[4] / w, ms.ph[6] / w);
+        printf("round profile: common round %lld events, %.0f cycles/round, %.0f cycles/wave\n", ms.rp_cnt[RP_ROUND], ms.rp_cyc[RP_ROUND] / nr, ms.rp_cyc[RP_ROUND] / w);
+        printf("round profile: rebuilds %lld, %.0f cycles each, %.0f cycles/wave\n", ms.rp_cnt[RP_REBUILD],
+               ms.rp_cyc[RP_REBUILD] / (double)(ms.rp_cnt[RP_REBUILD] > 0 ? ms.rp_cnt[RP_REBUILD] : 1), ms.rp_cyc[RP_REBUILD] / w);
+        printf("round profile: after the loop %lld waves, %.0f cycles/wave\n", ms.rp_cnt[RP_AFTER], ms.rp_cyc[RP_AFTER] / w);
+        printf("round profile: rounds with a non-zero kill mask %lld\n", ms.rp_cnt[RP_KILL]);
+        for (int q = 0; q < MULTI_GT; q++)
+          if (ms.rp_cnt[RP_MINMOVE + q])
+            printf("round profile: term %d minimum moves %lld, %.0f cycles each, %.0f cycles/wave\n", q, ms.rp_cnt[RP_MINMOVE + q],
+                   ms.rp_cyc[RP_MINMOVE + q] / (double)ms.rp_cnt[RP_MINMOVE + q], ms.rp_cyc[RP_MINMOVE + q] / w);
+      }
+#endif
     }
   }
 }
