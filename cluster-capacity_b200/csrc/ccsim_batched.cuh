@@ -105,7 +105,6 @@ __global__ void __launch_bounds__(LEAN_THREADS, 1) ccsim_wave_batched_kernel(con
   const long long eq_cpu = ls.eq_cpu, eq_mem = ls.eq_mem;
   const int32_t pods_need = ls.pods_need;
   const ccsim_template &t = ls.tmpl;
-  const int64_t taint_const = (t.score_enable & CCSIM_PL_TAINT_TOLERATION) ? (int64_t)t.w_taint * 100 : 0;   // maxCount == 0 -> every node 100
 
   long long k = 0, waves = 0, extra_evals = 0;
   bool limit_hit = false;   // postBindHook's limit (simulator.go:300-305)
@@ -143,22 +142,9 @@ __global__ void __launch_bounds__(LEAN_THREADS, 1) ccsim_wave_batched_kernel(con
       unsigned long long *myslots = p.slots + ((size_t)(waves & 1) * CCSIM_MAX_GRID + cta) * SLOT_STRIDE;
       const unsigned long long vb = warp_max_u64(lane < LEAN_WARPS ? ls.warp_best[lane][0] : 0ull);
       if (lane == 0) st_slot(&myslots[0], vb | tagbits);
-      const unsigned long long *all = p.slots + (size_t)(waves & 1) * CCSIM_MAX_GRID * SLOT_STRIDE;
-      unsigned long long v[CCSIM_MAX_GRID / 32];
-      unsigned spins = 0;
-      bool pending, dead = false;
-      do {
-        pending = false;
-        #pragma unroll
-        for (int q = 0; q < CCSIM_MAX_GRID / 32; q++) { const int b = lane + 32 * q; v[q] = (b < p.grid) ? ld_slot(&all[(size_t)b * SLOT_STRIDE]) : tagbits; }
-        #pragma unroll
-        for (int q = 0; q < CCSIM_MAX_GRID / 32; q++) pending |= ((uint32_t)(v[q] >> KEY_TAG_SHIFT) != tag);
-        if (++spins > WATCHDOG_SPINS) { dead = true; break; }
-      } while (__any_sync(0xffffffffu, pending));
-      unsigned long long m = 0ull;
-      #pragma unroll
-      for (int q = 0; q < CCSIM_MAX_GRID / 32; q++) { const unsigned long long b = v[q] & KEY_BODY_MASK; m = b > m ? b : m; }
-      m = warp_max_u64(m);
+      unsigned long long v[GATHER_Q];
+      bool dead = poll_tagged(p, waves, tag, 0, lane, v);
+      const unsigned long long m = gather_max(v);
       dead = __any_sync(0xffffffffu, dead);
       if (lane == 0) {
         if (dead) ls.stop = 3;
@@ -260,6 +246,5 @@ __global__ void __launch_bounds__(LEAN_THREADS, 1) ccsim_wave_batched_kernel(con
     o->examined = o->evals;
     for (int c = 0; c < CCSIM_MAX_PTS; c++) o->ptsmin[c] = 0;
     o->aff_total = 0;
-    (void)taint_const;
   }
 }

@@ -471,28 +471,53 @@ __device__ __forceinline__ bool cross_gpu_exchange(const DevParams &p, long long
   return __any_sync(0xffffffffu, dead);
 }
 
-// grid-wide max of one value (< 2^44) per CTA through word `word` of the slot lines (same tagged-word protocol as the keys)
-__device__ __forceinline__ unsigned long long exchange_max(const DevParams &p, long long k, uint32_t tag, int word,
-                                                           unsigned long long mine, int lane, int cta, bool &dead) {
+// ---- tagged-word gather: the grid-wide half of an intra-GPU exchange --------------------------------------------------
+// Each CTA publishes one word, tagged with the wave, in word `word` of its slot line of parity k & 1; warp 0 of every CTA then
+// waits here until the word of every CTA carries `tag`. All of a lane's loads are in flight together. On return v[q] holds the
+// body of CTA lane + 32 q's word (0 past the grid); the result is true when the watchdog expired first. Every lane leaves the
+// loop in the same iteration, but the compiler cannot see that: gather_tagged votes the flag, poll_tagged leaves the vote to
+// a caller that schedules it after its own reduction.
+#define GATHER_Q (CCSIM_MAX_GRID / 32)
+__device__ __forceinline__ bool poll_tagged(const DevParams &p, long long k, uint32_t tag, int word, int lane,
+                                            unsigned long long (&v)[GATHER_Q]) {
   const unsigned long long tagbits = (unsigned long long)tag << KEY_TAG_SHIFT;
-  if (lane == 0) st_slot(p.slots + ((size_t)(k & 1) * CCSIM_MAX_GRID + cta) * SLOT_STRIDE + word, (mine & KEY_BODY_MASK) | tagbits);
   const unsigned long long *all = p.slots + (size_t)(k & 1) * CCSIM_MAX_GRID * SLOT_STRIDE + word;
-  unsigned long long v[CCSIM_MAX_GRID / 32];
   unsigned spins = 0;
-  bool pending;
+  bool pending, dead = false;
   do {
     pending = false;
     #pragma unroll
-    for (int q = 0; q < CCSIM_MAX_GRID / 32; q++) { const int b = lane + 32 * q; v[q] = (b < p.grid) ? ld_slot(&all[(size_t)b * SLOT_STRIDE]) : tagbits; }
+    for (int q = 0; q < GATHER_Q; q++) { const int b = lane + 32 * q; v[q] = (b < p.grid) ? ld_slot(&all[(size_t)b * SLOT_STRIDE]) : tagbits; }
     #pragma unroll
-    for (int q = 0; q < CCSIM_MAX_GRID / 32; q++) pending |= ((uint32_t)(v[q] >> KEY_TAG_SHIFT) != tag);
+    for (int q = 0; q < GATHER_Q; q++) pending |= ((uint32_t)(v[q] >> KEY_TAG_SHIFT) != tag);
     if (++spins > WATCHDOG_SPINS) { dead = true; break; }
   } while (__any_sync(0xffffffffu, pending));
+  #pragma unroll
+  for (int q = 0; q < GATHER_Q; q++) v[q] &= KEY_BODY_MASK;
+  return dead;
+}
+__device__ __forceinline__ bool gather_tagged(const DevParams &p, long long k, uint32_t tag, int word, int lane,
+                                              unsigned long long (&v)[GATHER_Q]) {
+  return __any_sync(0xffffffffu, poll_tagged(p, k, tag, word, lane, v));
+}
+// the largest gathered body (keys: the winner; 0 = no CTA had one)
+__device__ __forceinline__ unsigned long long gather_max(const unsigned long long (&v)[GATHER_Q]) {
   unsigned long long m = 0ull;
   #pragma unroll
-  for (int q = 0; q < CCSIM_MAX_GRID / 32; q++) { const unsigned long long b = v[q] & KEY_BODY_MASK; m = b > m ? b : m; }
-  dead = __any_sync(0xffffffffu, dead);
+  for (int q = 0; q < GATHER_Q; q++) m = v[q] > m ? v[q] : m;
   return warp_max_u64(m);
+}
+// the sum of the gathered bodies of the CTAs below `cta`, and of all of them
+__device__ __forceinline__ void gather_prefix_total(const unsigned long long (&v)[GATHER_Q], int lane, int cta,
+                                                    unsigned long long &prefix, unsigned long long &total) {
+  unsigned long long pre = 0, tot = 0;
+  #pragma unroll
+  for (int q = 0; q < GATHER_Q; q++) {
+    tot += v[q];
+    if (lane + 32 * q < cta) pre += v[q];
+  }
+  for (int o = 16; o > 0; o >>= 1) { pre += __shfl_xor_sync(0xffffffffu, pre, o); tot += __shfl_xor_sync(0xffffffffu, tot, o); }
+  prefix = pre; total = tot;
 }
 
 // Several grid-wide maxima at once: lane q < NV publishes vals[q] (< 2^44, 0 = "nothing") in word word0+q of this CTA's
@@ -525,6 +550,18 @@ __device__ __forceinline__ void exchange_max_n(const DevParams &p, long long k, 
     vals[w] = warp_max_u64(m);
   }
   dead = __any_sync(0xffffffffu, dead);
+}
+
+// grid-wide prefix and total of one value per CTA (< 2^44 in total) through word `word` of the slot lines: the sum over the
+// CTAs below this one, and over all of them. Returns true, on every lane, when the watchdog expired.
+__device__ __forceinline__ bool exchange_prefix_total(const DevParams &p, long long k, uint32_t tag, int word, unsigned long long mine,
+                                                      int lane, int cta, unsigned long long &prefix, unsigned long long &total) {
+  const unsigned long long tagbits = (unsigned long long)tag << KEY_TAG_SHIFT;
+  if (lane == 0) st_slot(p.slots + ((size_t)(k & 1) * CCSIM_MAX_GRID + cta) * SLOT_STRIDE + word, (mine & KEY_BODY_MASK) | tagbits);
+  unsigned long long v[GATHER_Q];
+  const bool dead = poll_tagged(p, k, tag, word, lane, v);
+  gather_prefix_total(v, lane, cta, prefix, total);
+  return __any_sync(0xffffffffu, dead);
 }
 
 // grid-wide sum of one count per CTA (< 2^44 in total), with release/acquire fences around it: global stores made by the
@@ -605,4 +642,48 @@ __device__ __forceinline__ int32_t node_affinity_raw(const DevParams &p, const c
 __device__ __forceinline__ int64_t taint_norm(int raw, int maxraw) {
   if (maxraw == 0) return 100;
   return 100 - (100 * (int64_t)raw / maxraw);
+}
+
+// prioritizeNodes + selectHost over the winners of the normalisation classes (schedule_one.go:776-941): class c holds the
+// feasible nodes with c untolerated PreferNoSchedule taints, whose TaintToleration NormalizeScore depends only on c and on the
+// highest class present. Returns the winner's key with its total score (0: no feasible node).
+__device__ __forceinline__ unsigned long long select_host_over_classes(const unsigned long long *cbest, int ncls, const ccsim_template &t) {
+  unsigned long long wkey = cbest[0];
+  if (ncls > 1 || (t.score_enable & CCSIM_PL_TAINT_TOLERATION)) {
+    int maxraw = 0;
+    for (int c = 0; c < ncls; c++) if (cbest[c] != 0ull) maxraw = c;
+    wkey = 0ull;
+    for (int c = 0; c < ncls; c++) {
+      if (cbest[c] == 0ull) continue;
+      int64_t total = key_score(cbest[c]);
+      if (t.score_enable & CCSIM_PL_TAINT_TOLERATION) total += (int64_t)t.w_taint * taint_norm(c, maxraw);
+      const unsigned long long kk = pack_key(total, key_index(cbest[c]));
+      wkey = kk > wkey ? kk : wkey;
+    }
+  }
+  return wkey;
+}
+
+// PodTopologySpread's global minimum (filtering.go:56-69) as a recount: the minimum of cnt[0..n_present) and how many domains
+// hold it, over all NT (== blockDim.x) threads of the block. scratch: NT / 32 ints of shared memory. Every thread gets the minimum; the
+// multiplicity is valid in thread 0.
+template <int NT>
+__device__ __forceinline__ int32_t block_min_count(const int32_t *cnt, int32_t n_present, int32_t *scratch, int32_t &num) {
+  int32_t m = INT32_MAX;
+  for (int d = threadIdx.x; d < n_present; d += blockDim.x) m = min(m, cnt[d]);
+  m = __reduce_min_sync(0xffffffffu, m);
+  if ((threadIdx.x & 31) == 0) scratch[threadIdx.x >> 5] = m;
+  __syncthreads();
+  m = INT32_MAX;
+  for (int w = 0; w < NT / 32; w++) m = min(m, scratch[w]);
+  __syncthreads();
+  int32_t s = 0;
+  for (int d = threadIdx.x; d < n_present; d += blockDim.x) s += (cnt[d] == m);
+  s = __reduce_add_sync(0xffffffffu, s);
+  if ((threadIdx.x & 31) == 0) scratch[threadIdx.x >> 5] = s;
+  __syncthreads();
+  num = 0;
+  if (threadIdx.x == 0)
+    for (int w = 0; w < NT / 32; w++) num += scratch[w];
+  return m;
 }

@@ -730,11 +730,6 @@ struct ccsim_handle {
   int sm_count = 0;
   size_t l2_bytes = 0;
   size_t smem_optin = 0;
-  int last_resident = 0;
-  int last_lean = 0;
-  int last_batched = 0;
-  int last_multi = 0;
-  int last_stream = 0;
   std::vector<void *> stream_allocs;                    // padded streaming columns + per-template score memo (ccsim_stream.cuh)
   uint64_t taint_or0 = 0;                               // OR over the nodes of taint word 0
   std::vector<std::pair<void *, size_t>> block_cache;   // freed device blocks kept for reuse (exact size match)
@@ -1129,6 +1124,19 @@ static void fill_params(ccsim_handle *h, DevParams &p, int64_t max_pods) {
   p.taint_list_off = h->d_taint_off; p.taint_list = h->d_taint_list;
 }
 
+// A template that needs one of the uncommon predicates the lean and streaming kernels leave out (filter_extras: ephemeral storage,
+// extended resources, nodeAffinity terms, nodeName, PreFilter node sets, hostPorts against clones already placed).
+static bool needs_extras(const ccsim_handle *h, const ccsim_template &T) {
+  const bool nzfit = (T.filter_enable & CCSIM_PL_FIT) && !(T.flags & CCSIM_TF_FIT_ALL_ZERO);
+  if (nzfit && T.req_eph > 0) return true;
+  if (nzfit) for (int k = 0; k < h->meta.n_scalars; k++) if (T.req_scalar[k] != 0) return true;
+  if ((T.filter_enable & CCSIM_PL_NODE_AFFINITY) && (T.flags & CCSIM_TF_HAS_AFFINITY_TERMS)) return true;
+  if ((T.filter_enable & CCSIM_PL_NODE_NAME) && T.nodename_idx >= 0) return true;
+  if (T.flags & CCSIM_TF_PREFILTER_NODES) return true;
+  if ((T.filter_enable & CCSIM_PL_NODE_PORTS) && (T.flags & CCSIM_TF_HAS_HOST_PORTS) && h->w_placed) return true;
+  return false;
+}
+
 // Everything a Run does before the wave kernel starts: output / streaming buffers, restoring the working columns, choosing the
 // engine, uploading the parameters. Kept apart from the launch (ccsim_prepare) for hosts that drive several ranks from one
 // process: every rank must be past its allocations before any rank's persistent kernel starts waiting for its peers.
@@ -1208,9 +1216,8 @@ static int run_prepare(ccsim_handle *h, int64_t max_pods) {
   const size_t per_node = 8 * (9 + (h->meta.static_words > 0 ? 1 : 0)) + 4 * (4 + h->meta.n_topo_cols + n_local);
   const size_t smem_res = cnt_bytes + per_node * (size_t)p.chunk_pad;
   const size_t smem_str = cnt_bytes;
-  const bool resident = smem_res + sizeof(WaveShared) + 1024 <= h->smem_optin && !getenv("CCSIM_FORCE_STREAMING");
+  const bool resident = smem_res + sizeof(WaveShared) + 1024 <= h->smem_optin;
   p.tile_resident = resident ? 1 : 0;
-  h->last_resident = p.tile_resident;
   size_t smem = resident ? smem_res : smem_str;
   const void *kern = resident ? (const void *)ccsim_wave_kernel<true> : (const void *)ccsim_wave_kernel<false>;
   int block = BLOCK_THREADS;
@@ -1228,7 +1235,7 @@ static int run_prepare(ccsim_handle *h, int64_t max_pods) {
     p.sample_k = kf;
   }
   LeanParams lp; memset(&lp, 0, sizeof(lp));
-  // the lean kernel (768 threads) takes every eligible workload; CCSIM_FORCE_GENERIC overrides.
+  // the lean kernel (768 threads) takes every eligible workload
   // normalised soft scorers / ImageLocality columns run in the generic kernel only (multi-phase waves)
   bool has_pref = false, has_soft = false;
   for (auto &T : h->h_templates) {
@@ -1241,16 +1248,10 @@ static int run_prepare(ccsim_handle *h, int64_t max_pods) {
   if (has_soft && (h->cfg.world > 1 || h->n_templates > 1))
     return fail(h, CCSIM_EUNSUPPORTED, "normalised soft scorers (preferred nodeAffinity, ScheduleAnyway spreading, pod-affinity scoring): single template, single GPU only");
   has_pref = has_pref || has_soft;
-  bool lean = resident && !has_pref && h->n_templates == 1 && h->meta.taint_words == 1 && h->meta.static_words <= 1 && !getenv("CCSIM_FORCE_GENERIC");
+  bool lean = resident && !has_pref && h->n_templates == 1 && h->meta.taint_words == 1 && h->meta.static_words <= 1;
   if (lean) {
     const ccsim_template &T = h->h_templates[0];
-    const bool nzfit = (T.filter_enable & CCSIM_PL_FIT) && !(T.flags & CCSIM_TF_FIT_ALL_ZERO);
-    if (nzfit && T.req_eph > 0) lean = false;
-    if (nzfit) for (int k = 0; k < h->meta.n_scalars; k++) if (T.req_scalar[k] != 0) lean = false;
-    if ((T.filter_enable & CCSIM_PL_NODE_AFFINITY) && (T.flags & CCSIM_TF_HAS_AFFINITY_TERMS)) lean = false;
-    if ((T.filter_enable & CCSIM_PL_NODE_NAME) && T.nodename_idx >= 0) lean = false;
-    if (T.flags & CCSIM_TF_PREFILTER_NODES) lean = false;
-    if ((T.filter_enable & CCSIM_PL_NODE_PORTS) && (T.flags & CCSIM_TF_HAS_HOST_PORTS) && h->w_placed) lean = false;
+    if (needs_extras(h, T)) lean = false;
     if (T.n_pts + T.n_aff + T.n_anti > LEAN_MAX_TERMS) lean = false;
     int ns = 0;
     for (int j = 0; j < h->n_counters && lean; j++) {
@@ -1271,20 +1272,17 @@ static int run_prepare(ccsim_handle *h, int64_t max_pods) {
       int units = (10 + ns + 3) / 4;
       if ((units & 1) == 0) units++;
       lp.stride_u = units;
-      const int want1024 = (n + LEAN_THREADS - 1) / LEAN_THREADS;
-      (void)want1024;
       lp.rec_bytes_total = (uint32_t)((size_t)units * 16 * p.chunk_pad);
       const size_t smem_lean = cnt_bytes + lp.rec_bytes_total + (size_t)p.chunk_pad * (6 * 8 + 2 * 4 + (faithful ? 8 : 0));
       if (smem_lean + sizeof(LeanShared) + 1024 > h->smem_optin) lean = false;
       else { smem = smem_lean; kern = faithful ? (const void *)ccsim_wave_lean_kernel<true> : (const void *)ccsim_wave_lean_kernel<false>; block = LEAN_THREADS; }
     }
   }
-  h->last_lean = lean ? 1 : 0;
   if (faithful && (!lean || h->cfg.world > 1))
     return fail(h, CCSIM_EUNSUPPORTED, "reference sampling mode needs the lean resident kernel on a single GPU (one template, <=1 taint/static word, no extras)");
   // batched tie-run engine (ccsim_batched.cuh): one template, node-local predicates and scorers only
   bool batched = lean && !faithful && h->n_counters == 0 && h->max_prefer_pop == 0 && h->cfg.world == 1 &&
-                 h->cfg.engine != CCSIM_ENGINE_SEQUENTIAL && !getenv("CCSIM_FORCE_SEQUENTIAL");
+                 h->cfg.engine != CCSIM_ENGINE_SEQUENTIAL;
   if (batched) {
     const size_t smem_b = smem + (size_t)p.chunk_pad * 12;
     if (smem_b + sizeof(LeanShared) + sizeof(BatchShared) + 1024 > h->smem_optin) batched = false;
@@ -1292,11 +1290,10 @@ static int run_prepare(ccsim_handle *h, int64_t max_pods) {
   }
   if (h->cfg.engine == CCSIM_ENGINE_BATCHED && !batched)
     return fail(h, CCSIM_EUNSUPPORTED, "batched engine needs one template with node-local predicates only, no PreferNoSchedule taints, a resident tile and a single GPU");
-  h->last_batched = batched ? 1 : 0;
   // multi-commit waves (ccsim_multi.cuh): one template coupled through per-domain counters, one node per thread
   MultiParams mp; memset(&mp, 0, sizeof(mp));
   bool multi = lean && !faithful && !batched && h->n_counters > 0 && h->max_prefer_pop == 0 &&
-               h->cfg.engine == CCSIM_ENGINE_AUTO && !getenv("CCSIM_FORCE_SEQUENTIAL") && h->h_templates[0].n_aff == 0 &&
+               h->cfg.engine == CCSIM_ENGINE_AUTO && h->h_templates[0].n_aff == 0 &&
                p.chunk <= LEAN_THREADS && h->n_global < (1 << MULTI_IDX_BITS) && grid * MULTI_M <= MULTI_EPT * LEAN_THREADS;
   if (multi) {
     for (int j = 0; j < h->n_counters; j++) if (h->counters[j].inc < 0) multi = false;   // feasibility must be monotone within a wave
@@ -1329,24 +1326,15 @@ static int run_prepare(ccsim_handle *h, int64_t max_pods) {
     if (smem_m + sizeof(LeanShared) + sizeof(MultiShared) + 1024 > h->smem_optin) multi = false;
     if (multi) { kern = h->cfg.world > 1 ? (const void *)ccsim_wave_multi_kernel<true> : (const void *)ccsim_wave_multi_kernel<false>; smem = smem_m; }
   }
-  h->last_multi = multi ? 1 : 0;
   // streaming engine (ccsim_stream.cuh): node-local templates when the tile is not resident, or several templates; the node
   // tiles go through shared memory with bulk-async copies (TMA) and the score is memoised per (template, node)
   StreamParams sp; memset(&sp, 0, sizeof(sp));
   int stream_mode = 0;
   bool stream = !lean && !has_pref && h->n_counters == 0 && h->max_prefer_pop == 0 && !faithful &&
-                h->meta.taint_words == 1 && h->meta.static_words <= 1 && !getenv("CCSIM_FORCE_GENERIC");
+                h->meta.taint_words == 1 && h->meta.static_words <= 1;
   if (stream)
-    for (const ccsim_template &T : h->h_templates) {
-      const bool nzfit = (T.filter_enable & CCSIM_PL_FIT) && !(T.flags & CCSIM_TF_FIT_ALL_ZERO);
-      if (nzfit && T.req_eph > 0) stream = false;
-      if (nzfit) for (int k = 0; k < h->meta.n_scalars; k++) if (T.req_scalar[k] != 0) stream = false;
-      if ((T.filter_enable & CCSIM_PL_NODE_AFFINITY) && (T.flags & CCSIM_TF_HAS_AFFINITY_TERMS)) stream = false;
-      if ((T.filter_enable & CCSIM_PL_NODE_NAME) && T.nodename_idx >= 0) stream = false;
-      if (T.flags & CCSIM_TF_PREFILTER_NODES) stream = false;
-      if ((T.filter_enable & CCSIM_PL_NODE_PORTS) && (T.flags & CCSIM_TF_HAS_HOST_PORTS) && h->w_placed) stream = false;
-      if (T.n_pts || T.n_aff || T.n_anti) stream = false;
-    }
+    for (const ccsim_template &T : h->h_templates)
+      if (needs_extras(h, T) || T.n_pts || T.n_aff || T.n_anti) stream = false;
   if (stream) {
     free_pool(h, h->stream_allocs);
     bool masks = false;
@@ -1388,20 +1376,10 @@ static int run_prepare(ccsim_handle *h, int64_t max_pods) {
     smem = stream_mode == 2 ? smem_resf : (size_t)STREAM_STAGES * STREAM_TILE * (masks ? 40 : 24) + 128;
     block = STREAM_BLOCK;
   }
-  h->last_stream = stream ? 1 : 0;
   p.self = h->d_params;
   CK(cudaMemcpyAsync(h->d_params, &p, sizeof(DevParams), cudaMemcpyHostToDevice, s));
   int occ = 0;
-  if (stream && stream_mode == 1) CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, ccsim_wave_stream_kernel<1>, block, smem));
-  else if (stream && stream_mode == 2) CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, ccsim_wave_stream_kernel<2>, block, smem));
-  else if (stream) CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, ccsim_wave_stream_kernel<0>, block, smem));
-  else if (multi && h->cfg.world > 1) CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, ccsim_wave_multi_kernel<true>, block, smem));
-  else if (multi) CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, ccsim_wave_multi_kernel<false>, block, smem));
-  else if (batched) CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, ccsim_wave_batched_kernel, block, smem));
-  else if (lean && faithful) CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, ccsim_wave_lean_kernel<true>, block, smem));
-  else if (lean) CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, ccsim_wave_lean_kernel<false>, block, smem));
-  else if (resident) CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, ccsim_wave_kernel<true>, block, smem));
-  else CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, ccsim_wave_kernel<false>, block, smem));
+  CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, block, smem));
   if (occ < 1 || occ * h->sm_count < grid) return fail(h, CCSIM_ECUDA, "persistent grid %d does not fit (occupancy %d x %d SMs)", grid, occ, h->sm_count);
   pl.p = p; pl.lp = lp; pl.mp = mp; pl.sp = sp; pl.kern = kern; pl.grid = grid; pl.block = block; pl.smem = smem;
   pl.stream = stream; pl.multi = multi; pl.batched = batched; pl.lean = lean; pl.resident = resident;
@@ -1431,7 +1409,7 @@ extern "C" int ccsim_run(ccsim_handle *h, int64_t max_pods, ccsim_result *out) {
   DevParams &p = pl.p; LeanParams &lp = pl.lp; MultiParams &mp = pl.mp; StreamParams &sp = pl.sp;
   const void *kern = pl.kern; const int grid = pl.grid, block = pl.block; const size_t smem = pl.smem;
   const bool stream = pl.stream, multi = pl.multi, batched = pl.batched, lean = pl.lean, resident = pl.resident;
-  (void)resident;
+  (void)resident;      // read by the CCSIM_PHASE_TIMERS report only
   void *args[] = { (void *)&p, stream ? (void *)&sp : (void *)&lp, (void *)&mp };
   CK(cudaEventRecord(h->ev0, s));
   // Cooperative launch = the driver guarantees that the whole persistent grid is co-resident (the kernels never use grid.sync()).

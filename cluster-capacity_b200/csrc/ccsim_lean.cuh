@@ -65,10 +65,6 @@ struct __align__(16) LeanShared {
   unsigned long long warp_kth[LEAN_WARPS];
 };
 
-#ifndef WATCHDOG_SPINS
-#define WATCHDOG_SPINS (1u << 24)
-#endif
-
 __shared__ LeanShared ls;
 
 // one thread: fold the template into the lean constants (see build_filter_consts for the generic kernel)
@@ -144,65 +140,14 @@ __device__ void lean_build_consts(const DevParams &p, const LeanParams &lp) {
 __device__ void lean_pts_recount(const DevParams &p, const int32_t *smem_cnt, int c) {
   const ccsim_pts &pc = ls.tmpl.pts[c];
   const DevCounter &dc = p.counters[pc.counter];
-  const int32_t *cnt = smem_cnt + dc.smem_off;
-  int32_t m = INT32_MAX;
-  for (int d = threadIdx.x; d < dc.n_present; d += blockDim.x) m = min(m, cnt[d]);
-  m = __reduce_min_sync(0xffffffffu, m);
-  if ((threadIdx.x & 31) == 0) ls.scratch[threadIdx.x >> 5] = m;
-  __syncthreads();
-  m = INT32_MAX;
-  for (int w = 0; w < LEAN_WARPS; w++) m = min(m, ls.scratch[w]);
-  __syncthreads();
-  int32_t num = 0;
-  for (int d = threadIdx.x; d < dc.n_present; d += blockDim.x) num += (cnt[d] == m);
-  num = __reduce_add_sync(0xffffffffu, num);
-  if ((threadIdx.x & 31) == 0) ls.scratch[threadIdx.x >> 5] = num;
-  __syncthreads();
+  int32_t num;
+  const int32_t m = block_min_count<LEAN_THREADS>(smem_cnt + dc.smem_off, dc.n_present, ls.scratch, num);
   if (threadIdx.x == 0) {
-    int32_t s = 0;
-    for (int w = 0; w < LEAN_WARPS; w++) s += ls.scratch[w];
     ls.ptsmin[c] = pc.min_zero ? 0 : m;
-    ls.ptsnum[c] = s;
+    ls.ptsnum[c] = num;
     ls.dirty = 1;
   }
   __syncthreads();
-}
-
-// tagged exchange of two 22-bit counts per CTA through word `word` of the slot line; returns for each of the two
-// counts the sum over lower CTAs and the total over all CTAs
-__device__ __forceinline__ bool exchange_pair(const DevParams &p, long long k, uint32_t tag, int word, unsigned long long a, unsigned long long b,
-                                              int lane, int cta, unsigned long long &preA, unsigned long long &totA,
-                                              unsigned long long &preB, unsigned long long &totB) {
-  const unsigned long long tagbits = (unsigned long long)tag << KEY_TAG_SHIFT;
-  unsigned long long *myslot = p.slots + ((size_t)(k & 1) * CCSIM_MAX_GRID + cta) * SLOT_STRIDE + word;
-  if (lane == 0) st_slot(myslot, ((a << 22) | b) | tagbits);
-  const unsigned long long *all = p.slots + (size_t)(k & 1) * CCSIM_MAX_GRID * SLOT_STRIDE + word;
-  unsigned long long v[CCSIM_MAX_GRID / 32];
-  unsigned spins = 0;
-  bool pending, dead = false;
-  do {
-    pending = false;
-    #pragma unroll
-    for (int q = 0; q < CCSIM_MAX_GRID / 32; q++) { const int bb = lane + 32 * q; v[q] = (bb < p.grid) ? ld_slot(&all[(size_t)bb * SLOT_STRIDE]) : tagbits; }
-    #pragma unroll
-    for (int q = 0; q < CCSIM_MAX_GRID / 32; q++) pending |= ((uint32_t)(v[q] >> KEY_TAG_SHIFT) != tag);
-    if (++spins > WATCHDOG_SPINS) { dead = true; break; }
-  } while (__any_sync(0xffffffffu, pending));
-  unsigned long long pa = 0, ta = 0, pb = 0, tb = 0;
-  #pragma unroll
-  for (int q = 0; q < CCSIM_MAX_GRID / 32; q++) {
-    const int bb = lane + 32 * q;
-    const unsigned long long x = (bb < p.grid) ? (v[q] & KEY_BODY_MASK) : 0ull;
-    const unsigned long long xa = x >> 22, xb = x & ((1ull << 22) - 1);
-    ta += xa; tb += xb;
-    if (bb < cta) { pa += xa; pb += xb; }
-  }
-  for (int o = 16; o > 0; o >>= 1) {
-    pa += __shfl_xor_sync(0xffffffffu, pa, o); ta += __shfl_xor_sync(0xffffffffu, ta, o);
-    pb += __shfl_xor_sync(0xffffffffu, pb, o); tb += __shfl_xor_sync(0xffffffffu, tb, o);
-  }
-  preA = pa; totA = ta; preB = pb; totB = tb;
-  return __any_sync(0xffffffffu, dead);
 }
 
 // FAITHFUL: the reference's default sampling (adaptive numFeasibleNodesToFind + rotating start index,
@@ -364,8 +309,12 @@ __global__ void __launch_bounds__(LEAN_THREADS, 1) ccsim_wave_lean_kernel(const 
       const int32_t cB = jb >= cnt_nodes ? ctot : pre[jb];
       const int32_t cA = ctot - cB;
       if (warp == 0) {   // exchange 1: (cA, cB) of every tile -> feasible-rank offsets of this tile's two parts
-        unsigned long long preA, totA, preB, totB;
-        bool dead = exchange_pair(p, k, tag, CCSIM_MAX_CLASSES + 1, (unsigned long long)cA, (unsigned long long)cB, lane, cta, preA, totA, preB, totB);
+        // both counts travel in one word as two 22-bit fields; their sums over the grid stay below 2^22 too (a resident lean tile
+        // holds a few thousand nodes at most, the grid at most CCSIM_MAX_GRID tiles), so the packed sums split without a carry
+        unsigned long long pre, tot;
+        const bool dead = exchange_prefix_total(p, k, tag, CCSIM_MAX_CLASSES + 1, ((unsigned long long)cA << 22) | (unsigned long long)cB, lane, cta, pre, tot);
+        const unsigned long long F = (1ull << 22) - 1;
+        const unsigned long long preA = pre >> 22, totA = tot >> 22, preB = pre & F, totB = tot & F;
         if (lane == 0) { ls.f_preA = (long long)preA; ls.f_preB = (long long)(totA + preB); ls.f_total = (long long)(totA + totB); if (dead) ls.stop = 3; }
       }
       __syncthreads();
@@ -415,63 +364,22 @@ __global__ void __launch_bounds__(LEAN_THREADS, 1) ccsim_wave_lean_kernel(const 
         if (lane == 0) st_slot(&myslots[CCSIM_MAX_CLASSES], kv | tagbits);
       }
       PH_MARK(2);
-      const unsigned long long *all = p.slots + (size_t)(k & 1) * CCSIM_MAX_GRID * SLOT_STRIDE;
       unsigned long long cbest[CCSIM_MAX_CLASSES];
       bool dead = false;
       unsigned long long kth_all = 0ull;
       if (FAITHFUL) {
-        unsigned long long v[CCSIM_MAX_GRID / 32];
-        unsigned spins = 0;
-        bool pending;
-        do {
-          pending = false;
-          #pragma unroll
-          for (int q = 0; q < CCSIM_MAX_GRID / 32; q++) { const int b = lane + 32 * q; v[q] = (b < p.grid) ? ld_slot(&all[(size_t)b * SLOT_STRIDE + CCSIM_MAX_CLASSES]) : tagbits; }
-          #pragma unroll
-          for (int q = 0; q < CCSIM_MAX_GRID / 32; q++) pending |= ((uint32_t)(v[q] >> KEY_TAG_SHIFT) != tag);
-          if (++spins > WATCHDOG_SPINS) { dead = true; break; }
-        } while (__any_sync(0xffffffffu, pending));
-        unsigned long long m = 0ull;
-        #pragma unroll
-        for (int q = 0; q < CCSIM_MAX_GRID / 32; q++) { const unsigned long long b = v[q] & KEY_BODY_MASK; m = b > m ? b : m; }
-        kth_all = warp_max_u64(m);
+        unsigned long long v[GATHER_Q];
+        dead = gather_tagged(p, k, tag, CCSIM_MAX_CLASSES, lane, v);
+        kth_all = gather_max(v);
       }
       for (int c = 0; c < ncls; c++) {
-        unsigned long long v[CCSIM_MAX_GRID / 32];
-        unsigned spins = 0;
-        bool pending;
-        do {
-          pending = false;
-          #pragma unroll
-          for (int q = 0; q < CCSIM_MAX_GRID / 32; q++) {
-            const int b = lane + 32 * q;
-            v[q] = (b < p.grid) ? ld_slot(&all[(size_t)b * SLOT_STRIDE + c]) : tagbits;
-          }
-          #pragma unroll
-          for (int q = 0; q < CCSIM_MAX_GRID / 32; q++) pending |= ((uint32_t)(v[q] >> KEY_TAG_SHIFT) != tag);
-          if (++spins > WATCHDOG_SPINS) { dead = true; break; }
-        } while (__any_sync(0xffffffffu, pending));
-        unsigned long long m = 0ull;
-        #pragma unroll
-        for (int q = 0; q < CCSIM_MAX_GRID / 32; q++) { const unsigned long long b = v[q] & KEY_BODY_MASK; m = b > m ? b : m; }
-        cbest[c] = warp_max_u64(m);
+        unsigned long long v[GATHER_Q];
+        dead |= gather_tagged(p, k, tag, c, lane, v);
+        cbest[c] = gather_max(v);
       }
-      dead = __any_sync(0xffffffffu, dead);
       if (p.world > 1 && !dead) dead = cross_gpu_exchange(p, k, tag, ncls, cbest, lane, cta);
       PH_MARK(3);
-      unsigned long long wkey = cbest[0];
-      if (ncls > 1 || (t.score_enable & CCSIM_PL_TAINT_TOLERATION)) {
-        int maxraw = 0;
-        for (int c = 0; c < ncls; c++) if (cbest[c] != 0ull) maxraw = c;
-        wkey = 0ull;
-        for (int c = 0; c < ncls; c++) {
-          if (cbest[c] == 0ull) continue;
-          int64_t total = key_score(cbest[c]);
-          if (t.score_enable & CCSIM_PL_TAINT_TOLERATION) total += (int64_t)t.w_taint * taint_norm(c, maxraw);
-          const unsigned long long kk = pack_key(total, key_index(cbest[c]));
-          wkey = kk > wkey ? kk : wkey;
-        }
-      }
+      const unsigned long long wkey = select_host_over_classes(cbest, ncls, t);
       if (lane == 0) {
         if (dead) { ls.stop = 3; ls.winner = -1; }
         else if (wkey == 0ull) { ls.stop = 1; ls.winner = -1; }

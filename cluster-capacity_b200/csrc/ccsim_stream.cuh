@@ -343,23 +343,9 @@ __global__ void __launch_bounds__(STREAM_BLOCK, 1) ccsim_wave_stream_kernel(cons
       bool dead = false;
       unsigned long long wkey = 0ull;
       {
-        const unsigned long long *all = p.slots + (size_t)(k & 1) * CCSIM_MAX_GRID * SLOT_STRIDE;
-        unsigned long long v[CCSIM_MAX_GRID / 32];
-        unsigned spins = 0;
-        bool pending;
-        do {
-          pending = false;
-          #pragma unroll
-          for (int q = 0; q < CCSIM_MAX_GRID / 32; q++) { const int b = lane + 32 * q; v[q] = (b < p.grid) ? ld_slot(&all[(size_t)b * SLOT_STRIDE]) : tagbits; }
-          #pragma unroll
-          for (int q = 0; q < CCSIM_MAX_GRID / 32; q++) pending |= ((uint32_t)(v[q] >> KEY_TAG_SHIFT) != tag);
-          if (++spins > WATCHDOG_SPINS) { dead = true; break; }
-        } while (__any_sync(0xffffffffu, pending));
-        unsigned long long m = 0ull;
-        #pragma unroll
-        for (int q = 0; q < CCSIM_MAX_GRID / 32; q++) { const unsigned long long b = v[q] & KEY_BODY_MASK; m = b > m ? b : m; }
-        dead = __any_sync(0xffffffffu, dead);
-        wkey = warp_max_u64(m);
+        unsigned long long v[GATHER_Q];
+        dead = gather_tagged(p, k, tag, 0, lane, v);
+        wkey = gather_max(v);
       }
       if (p.world > 1 && !dead) { unsigned long long cb[1] = {wkey}; dead = cross_gpu_exchange(p, k, tag, 1, cb, lane, cta); wkey = cb[0]; }   // node shards: winners of all ranks
       if (lane == 0) {

@@ -6,8 +6,8 @@ abi = importlib.import_module("cluster-capacity_b200._abi")
 synth = importlib.import_module("cluster-capacity_b200.synth")
 engine = importlib.import_module("cluster-capacity_b200.engine")
 
-def probe(name, snap, tmpl, ctr, limit, bytes_per_eval):
-    with engine.Engine(device=0) as eng:
+def probe(name, snap, tmpl, ctr, limit, bytes_per_eval, engine_kind=abi.ENGINE_AUTO):
+    with engine.Engine(device=0, engine=engine_kind) as eng:
         t0 = time.time(); eng.load_nodes(snap); eng.set_templates(tmpl, ctr); t1 = time.time()
         r = eng.run(limit)
         r = eng.run(limit)
@@ -33,7 +33,5 @@ if __name__ == "__main__":
         snap, tmpl, ctr = synth.c4()
         tmpl[0].n_anti = 0
         probe("C4 spread-only", snap, tmpl, ctr[:3], 20000, 92)
-        os.environ["CCSIM_FORCE_SEQUENTIAL"] = "1"
-        probe("C4 spread-only, sequential", snap, tmpl, ctr[:3], 20000, 92)
-        del os.environ["CCSIM_FORCE_SEQUENTIAL"]
+        probe("C4 spread-only, sequential", snap, tmpl, ctr[:3], 20000, 92, abi.ENGINE_SEQUENTIAL)
     if "c5" in which: probe("C5 1M x 64 templates", *synth.c5(), 6400, 72)
