@@ -326,6 +326,17 @@ __device__ __noinline__ bool filter_extras(const DevParams *pp, int32_t ti, uint
   return ok;
 }
 
+// untolerated PreferNoSchedule taints of node i in taint words 1.. (word 0's are counted inline): the rest of its TaintToleration
+// raw score, i.e. of its normalisation class
+__device__ __noinline__ int prefer_count_hi(const DevParams *pp, int32_t ti, int32_t i) {
+  const DevParams &p = *pp;
+  const ccsim_template &t = p.templates[ti];
+  if (!(t.score_enable & CCSIM_PL_TAINT_TOLERATION)) return 0;
+  int c = 0;
+  for (int w = 1; w < p.taint_words; w++) c += __popcll(p.taint_mask[(size_t)w * p.n + i] & p.taint_prefer[w] & ~t.tol_prefer[w]);
+  return c;
+}
+
 // register copy of the FilterConsts fields every node needs (hoisted out of the node loop)
 struct HotConsts {
   unsigned long long taint_bad0, prefer0, sel0, forbid0;
@@ -386,6 +397,7 @@ __device__ __forceinline__ bool filter_node(const DevParams &p, const HotConsts 
     ok &= !((dom >= 0) && (fc.anti[a].cnt[dom < 0 ? 0 : dom] > 0));
   }
   if (hc.extras && ok) ok = filter_extras(p.self, fc.tmpl_index, hc.extras, i);
+  if ((hc.extras & CCSIM_X_TAINT_WORDS) && ok) raw += prefer_count_hi(p.self, fc.tmpl_index, i);
   return ok;
 }
 

@@ -415,7 +415,7 @@ __global__ void __launch_bounds__(BLOCK_THREADS, 1) ccsim_wave_kernel(const DevP
         const unsigned long long key = pack_key(total, (uint32_t)(p.node_base + i));
         if (ncls == 1) best[0] = key > best[0] ? key : best[0];
         else {
-          const int cls = __popcll(tl.taint0[i] & hc.prefer0);
+          const int cls = __popcll(tl.taint0[i] & hc.prefer0) + ((hc.extras & CCSIM_X_TAINT_WORDS) ? prefer_count_hi(p.self, fc.tmpl_index, i) : 0);
           #pragma unroll
           for (int c = 0; c < CCSIM_MAX_CLASSES; c++) if (c == cls) best[c] = key > best[c] ? key : best[c];
         }
@@ -723,6 +723,7 @@ struct RunPlan {      // what run_prepare decided, consumed by the launch
   DevParams p; LeanParams lp; MultiParams mp; StreamParams sp;
   const void *kern = nullptr; int grid = 0, block = 0; size_t smem = 0;
   bool stream = false, multi = false, batched = false, lean = false, resident = false;
+  const char *kernel_name = "";   // ccsim_kernel_name: outlives the launch, which clears `valid`
 };
 
 struct ccsim_handle {
@@ -1137,6 +1138,19 @@ static bool needs_extras(const ccsim_handle *h, const ccsim_template &T) {
   return false;
 }
 
+// ccsim_kernel_name of a wave-kernel instantiation
+static const char *kernel_name_of(const void *kern) {
+  const struct { const void *k; const char *name; } names[] = {
+    {(const void *)ccsim_wave_kernel<true>, "wave<true>"}, {(const void *)ccsim_wave_kernel<false>, "wave<false>"},
+    {(const void *)ccsim_wave_lean_kernel<false>, "lean<false>"}, {(const void *)ccsim_wave_lean_kernel<true>, "lean<true>"},
+    {(const void *)ccsim_wave_batched_kernel, "batched"},
+    {(const void *)ccsim_wave_multi_kernel<false>, "multi<false>"}, {(const void *)ccsim_wave_multi_kernel<true>, "multi<true>"},
+    {(const void *)ccsim_wave_stream_kernel<0>, "stream<0>"}, {(const void *)ccsim_wave_stream_kernel<1>, "stream<1>"},
+    {(const void *)ccsim_wave_stream_kernel<2>, "stream<2>"}};
+  for (const auto &e : names) if (e.k == kern) return e.name;
+  return "?";
+}
+
 // Everything a Run does before the wave kernel starts: output / streaming buffers, restoring the working columns, choosing the
 // engine, uploading the parameters. Kept apart from the launch (ccsim_prepare) for hosts that drive several ranks from one
 // process: every rank must be past its allocations before any rank's persistent kernel starts waiting for its peers.
@@ -1145,7 +1159,7 @@ static int run_prepare(ccsim_handle *h, int64_t max_pods) {
   if (h->cfg.world > 1 && !h->peers_ready) return fail(h, CCSIM_ESTATE, "sharded run: ccsim_peer_import must come first");
   CK(cudaSetDevice(h->cfg.device));
   RunPlan &pl = h->plan;
-  pl.valid = false; pl.empty = false; pl.max_pods = max_pods;
+  pl.valid = false; pl.empty = false; pl.max_pods = max_pods; pl.kernel_name = "";
   const int32_t n = h->n;
   // output capacity: no run can place more than sum(max(0, alloc_pods - npods)) pods (fit.go:567-576)
   int64_t cap = h->pod_bound + 1;
@@ -1383,6 +1397,7 @@ static int run_prepare(ccsim_handle *h, int64_t max_pods) {
   if (occ < 1 || occ * h->sm_count < grid) return fail(h, CCSIM_ECUDA, "persistent grid %d does not fit (occupancy %d x %d SMs)", grid, occ, h->sm_count);
   pl.p = p; pl.lp = lp; pl.mp = mp; pl.sp = sp; pl.kern = kern; pl.grid = grid; pl.block = block; pl.smem = smem;
   pl.stream = stream; pl.multi = multi; pl.batched = batched; pl.lean = lean; pl.resident = resident;
+  pl.kernel_name = kernel_name_of(kern);
   pl.valid = true;
   return CCSIM_OK;
 }
@@ -1499,6 +1514,8 @@ extern "C" int ccsim_device_info(ccsim_handle *h, int32_t *sm_count, int32_t *gr
 }
 
 extern "C" int64_t ccsim_kernel_launches(const ccsim_handle *h) { return h ? h->launches : 0; }
+
+extern "C" const char *ccsim_kernel_name(const ccsim_handle *h) { return h ? h->plan.kernel_name : ""; }
 
 extern "C" int ccsim_run_stats(const ccsim_handle *h, int64_t out[16]) {
   if (!h || !out) return CCSIM_EINVAL;

@@ -310,7 +310,9 @@ __global__ void __launch_bounds__(LEAN_THREADS, 1) ccsim_wave_lean_kernel(const 
       const int32_t cA = ctot - cB;
       if (warp == 0) {   // exchange 1: (cA, cB) of every tile -> feasible-rank offsets of this tile's two parts
         // both counts travel in one word as two 22-bit fields; their sums over the grid stay below 2^22 too (a resident lean tile
-        // holds a few thousand nodes at most, the grid at most CCSIM_MAX_GRID tiles), so the packed sums split without a carry
+        // holds a few thousand nodes at most, the grid at most CCSIM_MAX_GRID tiles), so the packed sums split without a carry.
+        // tests/test_gpu_kernel_edges.py::test_sampling_largest_lean_tile runs the largest cluster this kernel takes (267 168 nodes
+        // on an H100) and checks that it is below 2^22 nodes
         unsigned long long pre, tot;
         const bool dead = exchange_prefix_total(p, k, tag, CCSIM_MAX_CLASSES + 1, ((unsigned long long)cA << 22) | (unsigned long long)cB, lane, cta, pre, tot);
         const unsigned long long F = (1ull << 22) - 1;

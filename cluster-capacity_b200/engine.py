@@ -16,7 +16,8 @@ _lib = None
 
 EXPORTS = ["ccsim_create", "ccsim_destroy", "ccsim_last_error", "ccsim_abi_version", "ccsim_load_nodes",
            "ccsim_set_templates", "ccsim_run", "ccsim_prepare", "ccsim_node_counts", "ccsim_peer_export", "ccsim_peer_import",
-           "ccsim_device_info", "ccsim_kernel_launches", "ccsim_flush_l2", "ccsim_run_stats", "ccsim_peer_local", "ccsim_peer_import_local"]
+           "ccsim_device_info", "ccsim_kernel_launches", "ccsim_kernel_name", "ccsim_flush_l2", "ccsim_run_stats", "ccsim_peer_local",
+           "ccsim_peer_import_local"]
 
 
 class EngineError(RuntimeError):
@@ -50,6 +51,8 @@ def lib():
         L.ccsim_device_info.argtypes = [C.c_void_p, abi.P32, abi.P32, abi.P32, abi.P64]
         L.ccsim_kernel_launches.restype = C.c_int64
         L.ccsim_kernel_launches.argtypes = [C.c_void_p]
+        L.ccsim_kernel_name.restype = C.c_char_p
+        L.ccsim_kernel_name.argtypes = [C.c_void_p]
         L.ccsim_flush_l2.restype = C.c_int
         L.ccsim_flush_l2.argtypes = [C.c_void_p]
         L.ccsim_peer_local.restype = C.c_int
@@ -165,11 +168,17 @@ class Engine:
         """Latency anatomy of the last run (see ccsim_run_stats in include/ccsim.h)."""
         v = np.zeros(16, np.int64)
         self._check(lib().ccsim_run_stats(self._h, v.ctypes.data_as(abi.P64)), "ccsim_run_stats")
-        return {"engine": self.ENGINE_NAMES[int(v[0])], "waves": int(v[1]), "placed": int(v[2]), "candidates": int(v[3]), "bar_raised_waves": int(v[4]),
-                "grid": int(v[5]), "block": int(v[6]), "smem_bytes": int(v[7]), "phase_cycles": [int(x) for x in v[8:16]]}
+        return {"engine": self.ENGINE_NAMES[int(v[0])], "kernel": self.kernel_name(), "waves": int(v[1]), "placed": int(v[2]),
+                "candidates": int(v[3]), "bar_raised_waves": int(v[4]), "grid": int(v[5]), "block": int(v[6]), "smem_bytes": int(v[7]),
+                "phase_cycles": [int(x) for x in v[8:16]]}
 
     def kernel_launches(self):
         return int(lib().ccsim_kernel_launches(self._h))
+
+    def kernel_name(self):
+        """The wave-kernel instantiation the last prepare() / run() chose, e.g. "lean<true>" or "stream<0>" (see ccsim_kernel_name);
+        "" before any, and for an empty cluster."""
+        return lib().ccsim_kernel_name(self._h).decode()
 
     def flush_l2(self):
         self._check(lib().ccsim_flush_l2(self._h), "ccsim_flush_l2")

@@ -316,6 +316,12 @@ int  ccsim_peer_import_local(ccsim_handle *h, int32_t world, void *const *ptrs /
 /* introspection for tests / bench */
 int  ccsim_device_info(ccsim_handle *h, int32_t *sm_count, int32_t *grid, int32_t *block, int64_t *l2_bytes);
 int64_t ccsim_kernel_launches(const ccsim_handle *h);  /* kernels launched by this handle so far */
+/* the wave-kernel instantiation the last ccsim_prepare (or the prepare inside ccsim_run) chose: "wave<true>" / "wave<false>"
+ * (generic, tile resident / streamed from global memory), "lean<false>" / "lean<true>" (lean, reference sampling), "batched",
+ * "multi<false>" / "multi<true>" (multi-commit, sharded), "stream<0>" / "stream<1>" / "stream<2>" (TMA streaming: every column
+ * streamed / with mask columns / resident free columns). "" before any prepare, after a failed one and for an empty cluster.
+ * Valid after ccsim_prepare alone: no kernel needs to run. The string is static. */
+const char *ccsim_kernel_name(const ccsim_handle *h);
 int  ccsim_flush_l2(ccsim_handle *h);                  /* writes a buffer larger than L2 (bench hygiene) */
 /* latency anatomy of the last run (bench.py's roofline block): [0] engine (0 generic, 1 lean sequential, 2 tie-run batching,
  * 3 multi-commit, 4 streaming) [1] waves [2] placed [3] multi-commit: candidates replayed, summed over waves [4] multi-commit: waves that

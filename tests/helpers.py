@@ -50,6 +50,41 @@ def run_stats(eng):
     return eng.run_stats()
 
 
+def kernel_name(eng):
+    """The wave-kernel instantiation the last prepare() / run() of `eng` chose, e.g. "lean<true>" (Engine.kernel_name)."""
+    return eng.kernel_name()
+
+
+def prepared_kernel(snap, tmpl, ctr, max_pods=0, **engine_kw):
+    """The kernel a workload runs on, from ccsim_prepare alone: nothing is launched."""
+    engine = importlib.import_module("cluster-capacity_b200.engine")
+    with engine.Engine(device=0, **engine_kw) as eng:
+        eng.load_nodes(snap)
+        eng.set_templates(tmpl, ctr)
+        eng.prepare(max_pods)
+        return kernel_name(eng)
+
+
+def largest_n(make, kernel, lo, hi, max_pods=0, **engine_kw):
+    """The largest N in [lo, hi) for which the workload make(N) = (snapshot, templates, counters) still runs on `kernel`, by
+    bisection over prepare() alone. Where one kernel ends depends on sizeof of the shared-memory structs and on the device's
+    opt-in limit, so the tests find it instead of restating it. Requires `kernel` at lo and another kernel (or a refusal) at hi."""
+    def on(n):
+        try:
+            return prepared_kernel(*make(n), max_pods=max_pods, **engine_kw) == kernel
+        except RuntimeError:          # EngineError: the configuration refuses the workload
+            return False
+    assert on(lo), (kernel, lo)
+    assert not on(hi), (kernel, hi)
+    while hi - lo > 1:
+        mid = (lo + hi) // 2
+        if on(mid):
+            lo = mid
+        else:
+            hi = mid
+    return lo
+
+
 def device_sm_count(device=0):
     engine = importlib.import_module("cluster-capacity_b200.engine")
     with engine.Engine(device=device) as eng:
@@ -107,6 +142,37 @@ def sparse_eligibility_case(n, max_skew, every=40, zones=8):
     t.n_pts = 1
     t.pts[0].counter, t.pts[0].max_skew, t.pts[0].self_match, t.pts[0].min_zero = 0, max_skew, 1, 0
     t.n_anti, t.anti_counter[0] = 1, 1
+    return snap, [t], ctr
+
+
+def soft_cluster(seed, n=3000, system_default=False):
+    """Normalised soft scorers on one template: ScheduleAnyway spreading over a zone column (inclusion policies) and the hostname,
+    pod (anti-)affinity score weights per rack and per node, an ImageLocality column and PreferNoSchedule classes. Every wave runs
+    the generic kernel's three-pass pipeline."""
+    rng = np.random.default_rng(seed)
+    zone = rng.integers(0, 20, n).astype(np.int32)
+    zone[rng.random(n) < 0.07] = -1                        # nodes without the zone label
+    rack = rng.integers(0, 200, n).astype(np.int32)
+    bit = lambda a, b: a.astype(np.uint64) << np.uint64(b)
+    static = bit(zone < 0, 0) | bit(rng.random(n) < 0.9, 1) | bit(rng.random(n) < 0.8, 2)
+    taint = bit(rng.random(n) < 0.25, 0)
+    snap = abi.Snapshot(n, rng.choice([2000, 4000, 8000], n), np.full(n, 16 << 30), rng.choice([6, 10, 14], n),
+                        static_mask=static.reshape(1, n), topo=[zone, rack], taint_mask=taint.reshape(1, n), taint_prefer=[1],
+                        taint_lists=[[0] if int(x) else [] for x in taint])
+    ctr = [abi.make_counter(0, rng.integers(0, 40, 20), inc=1, elig_bit=2),           # soft zone constraint, inclusion policies
+           abi.make_counter(-1, rng.integers(0, 3, n), inc=1),                        # soft hostname constraint
+           abi.make_counter(1, rng.integers(-50, 50, 200), inc=-3),                   # pod (anti-)affinity weights per rack
+           abi.make_counter(-1, rng.integers(-5, 20, n), inc=7)]                      # ... and per node
+    t = abi.default_template(300, 256 << 20)
+    t.n_spts = 2
+    t.spts_ignored_bit = -1 if system_default else 0
+    t.spts[0].counter, t.spts[0].max_skew, t.spts[0].hostname, t.spts[0].has_key_bit = 0, 5, 0, -1
+    t.spts[1].counter, t.spts[1].max_skew, t.spts[1].hostname, t.spts[1].has_key_bit = 1, 3, 1, 1
+    t.n_ipa_score = 2
+    t.ipa_score_counter[0], t.ipa_score_counter[1] = 2, 3
+    img = np.where(rng.random(n) < 0.3, rng.integers(1, 101, n), 0).astype(np.uint8)
+    t._keep_img = img
+    t.image_score = img.ctypes.data_as(abi.C.POINTER(abi.C.c_uint8))
     return snap, [t], ctr
 
 

@@ -28,13 +28,15 @@ def gpu_run(snap, tmpl, ctr=(), max_pods=0, engine_kind=abi.ENGINE_SEQUENTIAL, s
     return res, counts, first
 
 
-def check(snap, tmpl, ctr=(), max_pods=0, threads=4, auto_engine=None):
+def check(snap, tmpl, ctr=(), max_pods=0, threads=4, auto_engine=None, kernel=None):
     """Sequential engine (one winner per wave: evals/waves equal the reference-equivalent count) AND the default engine
-    (AUTO: batched tie-run waves when the template is node-local) against the oracle. `auto_engine`: the kernel AUTO must run."""
+    (AUTO: batched tie-run waves when the template is node-local) against the oracle. `auto_engine`: the engine AUTO must run;
+    `kernel`: its kernel instantiation (Engine.kernel_name)."""
     want = oracle.run(snap, tmpl, ctr, max_pods=max_pods, threads=threads)
     stats = {}
     auto, acounts, _ = gpu_run(snap, tmpl, ctr, max_pods, abi.ENGINE_AUTO, stats)
     assert auto_engine is None or stats["engine"] == auto_engine, stats
+    assert kernel is None or stats["kernel"] == kernel, stats
     assert auto.placed == want.placed and auto.stop_code == want.stop_code
     assert np.array_equal(auto.pod_node, want.pod_node), "AUTO engine: placement sequence differs from the oracle"
     assert np.array_equal(auto.reason_hist, want.reason_hist)
@@ -98,12 +100,12 @@ def test_c4_spread_and_anti_affinity(built):
 
 def test_c4_large_domain_set_uses_global_replicas(built):
     # 20000 racks > the 16384-int shared-memory counter area: per-CTA replicas in global memory
-    check(*synth.c4(n=30000, n_existing=30000, zones=16, racks=20000, regions=4), max_pods=300)
+    check(*synth.c4(n=30000, n_existing=30000, zones=16, racks=20000, regions=4), max_pods=300, kernel="wave<true>")
 
 
 def test_c5_multi_template_round_robin(built):
     snap, tmpl, ctr = synth.c5(n=3000, n_templates=7)
-    check(snap, tmpl, ctr, max_pods=4000)
+    check(snap, tmpl, ctr, max_pods=4000, kernel="stream<2>")
 
 
 def test_colocation_affinity(built):
@@ -126,7 +128,7 @@ def test_scalar_resources_and_ephemeral(built):
                         scalars=[(rng.integers(0, 9, n), rng.integers(0, 3, n))])
     t = abi.default_template(500, 1 * GiB, eph=7 * GiB)
     t.req_scalar[0] = 2
-    got = check(snap, [t])
+    got = check(snap, [t], kernel="wave<true>")
     assert got.reason_hist[abi.R_SCALAR0] > 0
 
 
@@ -145,7 +147,7 @@ def test_host_ports_one_clone_per_node(built):
     t.flags |= abi.TF_HAS_HOST_PORTS
     t.port_static_mask[0] = 1
     t.port_tmpl_conflict = 1
-    got = check(snap, [t])
+    got = check(snap, [t], kernel="wave<true>")
     assert got.placed == int((static == 0).sum())
     assert got.reason_hist[abi.R_NODE_PORTS] == n
 
@@ -227,49 +229,21 @@ def test_preferred_node_affinity_two_phase(built):
     for k, (bit, w) in enumerate([(0, 60), (1, 25), (2, 9)]):
         t.pref_weight[k] = w
         t.pref_mask[k][0] = 1 << bit
-    check(snap, [t], max_pods=6000)
-
-
-def _soft_cluster(seed, n=3000, system_default=False):
-    rng = np.random.default_rng(seed)
-    zone = rng.integers(0, 20, n).astype(np.int32)
-    zone[rng.random(n) < 0.07] = -1                        # nodes without the zone label
-    rack = rng.integers(0, 200, n).astype(np.int32)
-    bit = lambda a, b: a.astype(np.uint64) << np.uint64(b)
-    static = bit(zone < 0, 0) | bit(rng.random(n) < 0.9, 1) | bit(rng.random(n) < 0.8, 2)
-    taint = bit(rng.random(n) < 0.25, 0)
-    snap = abi.Snapshot(n, rng.choice([2000, 4000, 8000], n), np.full(n, 16 * GiB), rng.choice([6, 10, 14], n),
-                        static_mask=static.reshape(1, n), topo=[zone, rack], taint_mask=taint.reshape(1, n), taint_prefer=[1],
-                        taint_lists=[[0] if int(x) else [] for x in taint])
-    ctr = [abi.make_counter(0, rng.integers(0, 40, 20), inc=1, elig_bit=2),           # soft zone constraint, inclusion policies
-           abi.make_counter(-1, rng.integers(0, 3, n), inc=1),                        # soft hostname constraint
-           abi.make_counter(1, rng.integers(-50, 50, 200), inc=-3),                   # pod (anti-)affinity weights per rack
-           abi.make_counter(-1, rng.integers(-5, 20, n), inc=7)]                      # ... and per node
-    t = abi.default_template(300, 256 * MiB)
-    t.n_spts = 2
-    t.spts_ignored_bit = -1 if system_default else 0
-    t.spts[0].counter, t.spts[0].max_skew, t.spts[0].hostname, t.spts[0].has_key_bit = 0, 5, 0, -1
-    t.spts[1].counter, t.spts[1].max_skew, t.spts[1].hostname, t.spts[1].has_key_bit = 1, 3, 1, 1
-    t.n_ipa_score = 2
-    t.ipa_score_counter[0], t.ipa_score_counter[1] = 2, 3
-    img = np.where(rng.random(n) < 0.3, rng.integers(1, 101, n), 0).astype(np.uint8)
-    t._keep_img = img
-    t.image_score = img.ctypes.data_as(abi.C.POINTER(abi.C.c_uint8))
-    return snap, [t], ctr
+    check(snap, [t], max_pods=6000, kernel="wave<true>")
 
 
 @pytest.mark.parametrize("system_default", [False, True])
 def test_soft_scorers_three_phase(built, system_default):
     """PodTopologySpread score (log weights from the feasible set, min/max normalisation), InterPodAffinity score (float
     normalisation), ImageLocality column and PreferNoSchedule classes together: every wave runs the three-pass pipeline."""
-    snap, tmpl, ctr = _soft_cluster(5 if system_default else 4, system_default=system_default)
-    got = check(snap, tmpl, ctr, max_pods=5000)
+    snap, tmpl, ctr = helpers.soft_cluster(5 if system_default else 4, system_default=system_default)
+    got = check(snap, tmpl, ctr, max_pods=5000, kernel="wave<true>")
     assert got.placed > 1000
 
 
 def test_soft_scorers_until_full(built):
-    snap, tmpl, ctr = _soft_cluster(6, n=700)
-    got = check(snap, tmpl, ctr)
+    snap, tmpl, ctr = helpers.soft_cluster(6, n=700)
+    got = check(snap, tmpl, ctr, kernel="wave<true>")
     assert got.stop_code == abi.STOP_UNSCHEDULABLE
 
 
@@ -285,7 +259,7 @@ def test_image_locality_only_multi_template(built):
         t._keep_img = img
         t.image_score = img.ctypes.data_as(abi.C.POINTER(abi.C.c_uint8))
         tm.append(t)
-    check(snap, tm, max_pods=3000)
+    check(snap, tm, max_pods=3000, kernel="wave<true>")
 
 
 @pytest.mark.parametrize("limit", [1, 2, 7, 64, 1001, 0])
@@ -321,5 +295,5 @@ def test_multi_commit_zone_anti_affinity_and_missing_keys(built):
     t.anti_counter[0] = 0
     t.n_pts = 1
     t.pts[0].counter, t.pts[0].max_skew, t.pts[0].self_match, t.pts[0].min_zero = 1, 3, 1, 0
-    got = check(snap, [t], ctr, auto_engine="multi-commit")
+    got = check(snap, [t], ctr, auto_engine="multi-commit", kernel="multi<false>")
     assert got.stop_code == abi.STOP_UNSCHEDULABLE and got.placed > 200   # nodes without the zone label are not bound by the anti-affinity term
