@@ -33,17 +33,19 @@
 //                and polls its local copy — an all-gather of world x grid lines fused into the persistent kernel.
 // Replay: ONE warp, no barrier inside: <= 8 candidates per lane in registers; a round is arg-max (REDUX) -> commit (lane q =
 //   counter term q: cell += inc, over-limit test, PTS-minimum tracking, all from registers) -> kill the candidates sitting in
-//   a cell that just filled (SWAR field test against the OR-reduced filled cells). Measured on C4 (one H100 80GB HBM3, 400 W
-//   power limit, CCSIM_DEBUG_FLAGS=8: replay cycles minus set-up over rounds, so minimum moves, wake-ups and the hand-off after
-//   the loop are included): ~890 cycles per reference cycle, ~1 310 before the round was cut down to its dependent chain
-//   (three REDUX, one LDS/STS) — against ~2000 for a block-wide round (two barriers over 24 warps). The other 23 warps wait at
-//   the barrier that ends the wave. -DMULTI_ROUND_PROFILE splits those cycles (scripts/round_profile.sh).
+//   a cell that just filled (SWAR field test against the OR-reduced filled cells). Measured on C4 (one H100 80GB HBM3,
+//   CCSIM_DEBUG_FLAGS=8: replay cycles minus set-up over rounds, so minimum moves, wake-ups and the hand-off after the loop are
+//   included): ~827 cycles per reference cycle with one-pass minimum moves (700 W power limit); ~890 before them and ~1 310 before
+//   the round was cut down to its dependent chain (three REDUX, one LDS/STS; 400 W power limit) — against ~2000 for a block-wide
+//   round (two barriers over 24 warps). The other 23 warps wait at the barrier that ends the wave. -DMULTI_ROUND_PROFILE splits
+//   those cycles (scripts/round_profile.sh). Work around the round stays on this warp: moved onto the whole block (the set-up
+//   between G1 and G2, the look-ahead decision after R) it measured slower on C4, whose terms have 8 and 64 domains.
 //   Row updates of the winners are done by each node's own thread after that barrier (a thread owns its node).
 // Look-ahead waves: a PodTopologySpread minimum move that REOPENS closed domains would end the wave (the reopened nodes were
 //   rejected by the scan and are in nobody's list). When a term's limit is about to move, the scan publishes the nodes of its
-//   closed cells too; they sit in the replay as dormant candidates (key 0) and are rebuilt from the wave's candidate arrays when
-//   the move comes — see "dormant candidates" in the replay. C4: 3654 -> 2260 waves (scripts/wave_sim.py models the wave structure
-//   on the CPU and was used to choose the rule).
+//   closed cells too; they sit in the replay as dormant candidates (key 0: set-up reads the look-ahead terms' cells) and are
+//   rebuilt from the wave's candidate arrays when the move comes — see "dormant candidates" in the replay. C4: 3654 -> 2260 waves
+//   (scripts/wave_sim.py models the wave structure on the CPU and was used to choose the rule).
 #pragma once
 #include "ccsim_lean.cuh"
 
@@ -69,15 +71,19 @@ static_assert(MULTI_M == SLOT_STRIDE, "the keys of a CTA's list fill exactly one
 static_assert(4 + 2 * MULTI_CAP <= CCSIM_MAX_GRID * SLOT_STRIDE, "node shards: a rank's summary fits its region of the line buffer");
 
 // Round profile (profiling builds only: -DMULTI_ROUND_PROFILE; the hooks expand to nothing otherwise, and the shipped library's
-// SASS is the same with and without them). CTA 0's replay warp adds up, over the run, the cycles of: the common round (arg-max ->
-// commit -> kill), the minimum-move handling of each term, the rebuilds, and what follows the loop (the hand-off of the winners to
-// their threads, the look-ahead decision, barrier R); and the events: rounds, minimum moves per term, rebuilds, rounds that kill.
-// The kernel prints the table when the run ends (scripts/round_profile.sh).
+// SASS is the same with and without them). CTA 0's replay warp adds up, over the run, the cycles of: the set-up's candidate load,
+// the common round (arg-max -> commit -> kill), the minimum-move handling of each term, the wake-up rebuilds, and what follows the
+// loop (in total, and its parts: the hand-off of the winners to their threads, the look-ahead decision; the rest is barrier R); and
+// the events: rounds, minimum moves per term, rebuilds, rounds that kill. The kernel prints the table when the run ends
+// (scripts/round_profile.sh).
 #define RP_ROUND 0
 #define RP_REBUILD 1
 #define RP_AFTER 2
 #define RP_KILL 3                 /* (event count only) */
-#define RP_MINMOVE 4              /* + term q */
+#define RP_LOAD 4                 /* set-up: the candidates and the term constants into registers */
+#define RP_HANDOFF 5              /* after the loop: winners -> ms.mult */
+#define RP_DECIDE 6               /* after the loop: the next wave's look-ahead decision */
+#define RP_MINMOVE 7              /* + term q */
 #define RP_N (RP_MINMOVE + MULTI_GT)
 #ifdef MULTI_ROUND_PROFILE
 #define RPROF(...) __VA_ARGS__
@@ -587,6 +593,7 @@ __global__ void __launch_bounds__(LEAN_THREADS, 1) ccsim_wave_multi_kernel(const
         #pragma unroll
         for (int q = 0; q < MULTI_GT; q++)
           if (q < n_gt) { flsb |= 1u << ms.gt_c1[q][1]; fguard |= ((uint32_t)ms.gt_c1[q][2] + 1u) << ms.gt_c1[q][1]; }
+        RPROF(__syncwarp(); RP_ADD(RP_LOAD, clock64() - ms.tc0, 1);)
         const int32_t lim_off = c1.x - my_min;       // PTS: maxSkew - selfMatch (the limit follows the global minimum)
         bool lim_moved = false;
         const bool single_use = ms.single_use != 0;
@@ -608,23 +615,33 @@ __global__ void __launch_bounds__(LEAN_THREADS, 1) ccsim_wave_multi_kernel(const
         //      limit over their cell — the wave then goes on instead of ending for a rescan. It still has to end when the limit
         //      reaches a cell that was NOT published: `unpub_min` = the smallest count above limit + look-ahead at the start of the
         //      wave (such cells are closed, so their counts stand for the whole wave).
-        //      The round loop itself is unchanged: a candidate whose cell fills is zeroed as before. Waking is a REBUILD (rare: at the
-        //      start of a look-ahead wave and after a minimum move of a look-ahead term): every slot's key is read again from the
-        //      wave's candidate arrays — first-life key, or second-life key when bit j of `second` says the slot has won already
-        //      (single-use templates: gone) — and zeroed when one of its cells is over the limit as counters and limits stand now. ----
+        //      The dormant candidates of a look-ahead wave are found at set-up by reading the look-ahead terms' cells only: the scan
+        //      held every other term to its limit, and no commit has happened since. The round loop itself is unchanged: a candidate
+        //      whose cell fills is zeroed as before. Waking is a REBUILD (after a minimum move of a look-ahead term): every slot's key
+        //      is read again from the wave's candidate arrays — first-life key, or second-life key when bit j of `second` says the
+        //      slot has won already (single-use templates: gone) — and zeroed when one of its cells is over the limit as counters and
+        //      limits stand now. ----
         int32_t rlx = 0, unpub_min = INT32_MAX;
         if (lane < n_gt) rlx = lds_s32(MS_SA(relax) + 4u * (uint32_t)lds_s32(MS_SA(gt_term) + 4u * (uint32_t)lane));
         any_relax = __any_sync(0xffffffffu, rlx > 0);
-        bool need_rebuild = any_relax;
+        bool need_rebuild = false;
         if (any_relax) {
           for (unsigned nm = __ballot_sync(0xffffffffu, rlx > 0); nm; nm &= nm - 1) {
             const int q = __ffs(nm) - 1;
-            const int32_t off = __shfl_sync(0xffffffffu, gc.x, q), ndom = __shfl_sync(0xffffffffu, c1.w, q);
+            const int32_t off = __shfl_sync(0xffffffffu, gc.x, q), ndom = __shfl_sync(0xffffffffu, c1.w, q), lim = __shfl_sync(0xffffffffu, c1.x, q);
+            const uint32_t sh = (uint32_t)__shfl_sync(0xffffffffu, c1.y, q), mk = (uint32_t)__shfl_sync(0xffffffffu, c1.z, q);
             const int32_t publim = __shfl_sync(0xffffffffu, c1.x + rlx, q);
             const uint32_t ca = cnt_sa + 4u * (uint32_t)off;
             int32_t m = INT32_MAX;
             #pragma unroll 1
             for (int d = lane; d < ndom; d += 32) { const int32_t c = lds_s32(ca + 4u * d); if (c > publim) m = min(m, c); }
+            // this term's dormant candidates
+            #pragma unroll
+            for (int j = 0; j < MULTI_CPT; j++) {
+              const uint32_t f = (cd[j] >> sh) & mk;           // dom + 1 (0: no domain; cell 0 is read and ignored)
+              const int32_t c = lds_s32(ca + 4u * (uint32_t)max((int32_t)f - 1, 0));
+              if ((f != 0u) & (c > lim)) ck[j] = 0u;
+            }
             m = __reduce_min_sync(0xffffffffu, m);
             if (lane == q) unpub_min = m;
           }
@@ -727,22 +744,27 @@ __global__ void __launch_bounds__(LEAN_THREADS, 1) ccsim_wave_multi_kernel(const
             const int32_t off = __shfl_sync(0xffffffffu, gc.x, q), npres = __shfl_sync(0xffffffffu, gc.w, q), ndom = __shfl_sync(0xffffffffu, c1.w, q);
             const int32_t lim_old = __shfl_sync(0xffffffffu, c1.x, q), loff = __shfl_sync(0xffffffffu, lim_off, q);
             const uint32_t ca = cnt_sa + 4u * (uint32_t)off;
-            int32_t mn = INT32_MAX;
+            // one pass over the cells (one per lane for a term of <= 32 domains): this lane's minimum over the present domains and
+            // how many sit at it, and its lowest count over the old limit — the move changes verdicts iff that one is <= the new limit
+            int32_t mn = INT32_MAX, num = 0, up = INT32_MAX;
             #pragma unroll 1
-            for (int d = lane; d < npres; d += 32) mn = min(mn, lds_s32(ca + 4u * d));
+            for (int d = lane; d < ndom; d += 32) {
+              const int32_t c = lds_s32(ca + 4u * d);
+              if (c > lim_old) up = min(up, c);
+              if (d < npres) { num = c < mn ? 0 : num; mn = min(mn, c); num += c == mn; }
+            }
+            const int32_t lmn = mn;
             mn = __reduce_min_sync(0xffffffffu, mn);
+            up = __reduce_min_sync(0xffffffffu, up);
+            num = __reduce_add_sync(0xffffffffu, lmn == mn ? num : 0);
             const long long liml = (long long)loff + (long long)mn;
             const int32_t lim_new = liml > INT32_MAX ? INT32_MAX : (liml < INT32_MIN ? INT32_MIN : (int32_t)liml);
-            int32_t num = 0;
-            bool hit = false;
-            #pragma unroll 1
-            for (int d = lane; d < ndom; d += 32) { const int32_t c = lds_s32(ca + 4u * d); num += (d < npres) & (c == mn); hit |= (c > lim_old) & (c <= lim_new); }
-            num = __reduce_add_sync(0xffffffffu, num);
+            const bool hit = up <= lim_new;
             // a term scanned with look-ahead published the nodes of its closed cells: the move only matters when the new limit
             // reaches a cell that was not published; the cells in (old limit, new limit] wake their candidates up instead
             const bool rq = __shfl_sync(0xffffffffu, rlx, q) > 0;
             if (rq) { rescan |= (lim_new >= __shfl_sync(0xffffffffu, unpub_min, q)) | (p.debug_flags & 1); woke = true; }
-            else rescan |= __any_sync(0xffffffffu, hit) | (p.debug_flags & 1);
+            else rescan |= hit | (p.debug_flags & 1);
             if (lane == q) { my_min = mn; my_num = num; c1.x = lim_new; lim_moved = true; sts_s32(MS_SA(gt_c1) + 16u * (uint32_t)q, lim_new); }
             RPROF(__syncwarp(); const long long rp_m1 = clock64(); RP_ADD(RP_MINMOVE + q, rp_m1 - rp_m0, 1); rp_mm += rp_m1 - rp_m0;)
           }
@@ -775,6 +797,7 @@ __global__ void __launch_bounds__(LEAN_THREADS, 1) ccsim_wave_multi_kernel(const
           const int32_t jw = lds_s32(MS_SA(acc_node) + 4u * (uint32_t)i) - (p.node_base + lo);
           if (jw >= 0 && jw < cnt_nodes) atomicAdd(&ms.mult[jw], 1);
         }
+        RPROF(__syncwarp(); const long long rp_h1 = clock64(); RP_ADD(RP_HANDOFF, rp_h1 - ms.rp_t, 1);)
         // ---- the next wave's look-ahead, per PTS term on a replicated counter: its limit is about to move (<= MULTI_RELAX_K present
         //      domains left at the minimum) and the closed domains are not the majority (their nodes would crowd the live ones out of
         //      the tiles' top-M lists). A look-ahead wave that could not place anything is repeated strictly. Every CTA of every rank
@@ -796,6 +819,7 @@ __global__ void __launch_bounds__(LEAN_THREADS, 1) ccsim_wave_multi_kernel(const
           if (p.debug_flags & 32u) nrl = (lane < n_gt && gc.z >= 0 && gc.y > 0 && c1.x < INT32_MAX - 2 * MULTI_RELAX_R && !strict_next) ? MULTI_RELAX_R : 0;   // tests: look-ahead on every PTS term, every wave
           if (lane < n_gt) sts_s32(MS_SA(relax) + 4u * (uint32_t)lds_s32(MS_SA(gt_term) + 4u * (uint32_t)lane), nrl);
           if (cta == 0 && lane == 0 && acc == 0 && any_relax) ms.st_empty++;
+          RPROF(__syncwarp(); RP_ADD(RP_DECIDE, clock64() - rp_h1, 1);)
         }
         // the limits that moved go back to the Filter constants of the next scan
         if (lim_moved) { ls.terms[ms.gt_term[lane]].lim = c1.x; ms.gt_c1[lane][0] = c1.x; }
@@ -891,9 +915,11 @@ __global__ void __launch_bounds__(LEAN_THREADS, 1) ccsim_wave_multi_kernel(const
         const double w = (double)(limit_hit ? wv : wv + 1), nr = (double)(ms.st_rounds > 0 ? ms.st_rounds : 1);
         printf("round profile (CTA 0): waves %.0f rounds %lld | replay %.0f cycles/wave, set-up %.0f\n", w, ms.st_rounds, ms.ph[4] / w, ms.ph[6] / w);
         printf("round profile: common round %lld events, %.0f cycles/round, %.0f cycles/wave\n", ms.rp_cnt[RP_ROUND], ms.rp_cyc[RP_ROUND] / nr, ms.rp_cyc[RP_ROUND] / w);
-        printf("round profile: rebuilds %lld, %.0f cycles each, %.0f cycles/wave\n", ms.rp_cnt[RP_REBUILD],
+        printf("round profile: wake-up rebuilds %lld, %.0f cycles each, %.0f cycles/wave\n", ms.rp_cnt[RP_REBUILD],
                ms.rp_cyc[RP_REBUILD] / (double)(ms.rp_cnt[RP_REBUILD] > 0 ? ms.rp_cnt[RP_REBUILD] : 1), ms.rp_cyc[RP_REBUILD] / w);
-        printf("round profile: after the loop %lld waves, %.0f cycles/wave\n", ms.rp_cnt[RP_AFTER], ms.rp_cyc[RP_AFTER] / w);
+        printf("round profile: set-up: candidate load %.0f cycles/wave\n", ms.rp_cyc[RP_LOAD] / w);
+        printf("round profile: after the loop %lld waves, %.0f cycles/wave (hand-off %.0f, look-ahead decision %.0f)\n", ms.rp_cnt[RP_AFTER],
+               ms.rp_cyc[RP_AFTER] / w, ms.rp_cyc[RP_HANDOFF] / w, ms.rp_cyc[RP_DECIDE] / w);
         printf("round profile: rounds with a non-zero kill mask %lld\n", ms.rp_cnt[RP_KILL]);
         for (int q = 0; q < MULTI_GT; q++)
           if (ms.rp_cnt[RP_MINMOVE + q])
