@@ -68,10 +68,14 @@ def load_scheduler_config(path):
     for d in (plugins.get("multiPoint") or {}).get("disabled") or []:
         out["disabledFilters"].append(d["name"])
         out["disabledScores"].append(d["name"])
-    for point in ("score", "multiPoint"):
+    # getScoreWeights (framework.go:476-497): a Score-point weight wins over a MultiPoint one, and a weight of 0 (or none: an
+    # enabled entry replaces the default one, weight included) means 1. A negative weight is an error.
+    for point in ("multiPoint", "score"):
         for e in (plugins.get(point) or {}).get("enabled") or []:
-            if e.get("weight"):
-                out["weights"][e["name"]] = int(e["weight"])
+            w = int(e.get("weight") or 0)
+            if w < 0:
+                raise SystemExit("Invalid scheduler configuration: score weight of %s is negative: %d" % (e["name"], w))
+            out["weights"][e["name"]] = w or 1
     return out
 
 

@@ -943,6 +943,13 @@ extern "C" int ccsim_load_nodes(ccsim_handle *h, const ccsim_nodes *nd) {
   if (N > 0 && (!nd->alloc_cpu || !nd->alloc_mem || !nd->alloc_eph || !nd->alloc_pods || !nd->req_cpu || !nd->req_mem ||
                 !nd->req_eph || !nd->npods || !nd->nz_cpu || !nd->nz_mem || !nd->taint_mask))
     return fail(h, CCSIM_EINVAL, "null core column");
+  // LeastAllocated's (capacity - requested) * 100 must not wrap: a wrapped score leaves [0, 100] and runs into the key's tag bits
+  for (int32_t i = 0; i < N; i++) {
+    if (nd->alloc_cpu[i] > CCSIM_MAX_SCORED_ALLOCATABLE)
+      return fail(h, CCSIM_EUNSUPPORTED, "node %d: cpu allocatable %lld exceeds %lld", i, (long long)nd->alloc_cpu[i], (long long)CCSIM_MAX_SCORED_ALLOCATABLE);
+    if (nd->alloc_mem[i] > CCSIM_MAX_SCORED_ALLOCATABLE)
+      return fail(h, CCSIM_EUNSUPPORTED, "node %d: memory allocatable %lld exceeds %lld", i, (long long)nd->alloc_mem[i], (long long)CCSIM_MAX_SCORED_ALLOCATABLE);
+  }
   UP(d_alloc_cpu, nd->alloc_cpu, int64_t); UP(d_alloc_mem, nd->alloc_mem, int64_t); UP(d_alloc_eph, nd->alloc_eph, int64_t);
   UP(d_alloc_pods, nd->alloc_pods, int32_t);
   UP(s_req_cpu, nd->req_cpu, int64_t); UP(s_req_mem, nd->req_mem, int64_t); UP(s_req_eph, nd->req_eph, int64_t);
@@ -1043,7 +1050,17 @@ extern "C" int ccsim_set_templates(ccsim_handle *h, int32_t n_templates, const c
   for (int j = 0; j < n_counters; j++) if (counters[j].elig_bit >= 64 * nd.static_words) return fail(h, CCSIM_EINVAL, "counter %d: elig_bit", j);
   for (int t = 0; t < n_templates; t++) {
     const ccsim_template &T = templates[t];
-    const long long wsum = (long long)abs(T.w_taint) + abs(T.w_node_affinity) + abs(T.w_fit) + abs(T.w_pts) + abs(T.w_ipa) + abs(T.w_balanced) + abs(T.w_image);
+    // a negative weight can make a total negative, and score + 1 <= 0 sets the key's tag bits; the reference's plugin weights
+    // are never negative (framework.go:487-497) and its resource weights are validated to [1, 100] (validation_pluginargs.go)
+    const int32_t w[7] = {T.w_taint, T.w_node_affinity, T.w_fit, T.w_pts, T.w_ipa, T.w_balanced, T.w_image};
+    const char *wname[7] = {"TaintToleration", "NodeAffinity", "NodeResourcesFit", "PodTopologySpread", "InterPodAffinity",
+                            "NodeResourcesBalancedAllocation", "ImageLocality"};
+    for (int q = 0; q < 7; q++)
+      if (w[q] < 0) return fail(h, CCSIM_EUNSUPPORTED, "template %d: %s score weight %d is negative", t, wname[q], w[q]);
+    if (T.least_w_cpu < 1 || T.least_w_cpu > 100 || T.least_w_mem < 1 || T.least_w_mem > 100)
+      return fail(h, CCSIM_EUNSUPPORTED, "template %d: NodeResourcesFit resource weights cpu %d / memory %d outside [1, 100]", t, T.least_w_cpu, T.least_w_mem);
+    long long wsum = 0;
+    for (int q = 0; q < 7; q++) wsum += w[q];
     if (wsum * 100 >= 4095) return fail(h, CCSIM_EUNSUPPORTED, "template %d: sum of score weights %lld too large for the packed key", t, wsum);
   }
   if (h->max_prefer_pop + 1 > CCSIM_MAX_CLASSES)

@@ -64,7 +64,11 @@ struct SchedConfig {
     const Json &w = j.at("weights");
     if (w.is_object())
       for (auto &kv : w.obj) {
-        int v = (int)kv.second.i64(1);
+        // getScoreWeights (framework.go:487-497): an explicit 0 means the default of 1; weights are never negative
+        const long long raw = kv.second.i64(1);
+        if (raw < 0) throw std::runtime_error("score weight of " + kv.first + " is negative: " + std::to_string(raw));
+        if (raw > INT32_MAX) throw std::runtime_error("score weight of " + kv.first + " is too large: " + std::to_string(raw));
+        const int v = raw == 0 ? 1 : (int)raw;
         if (kv.first == "TaintToleration") c.w_taint = v; else if (kv.first == "NodeAffinity") c.w_node_affinity = v;
         else if (kv.first == "NodeResourcesFit") c.w_fit = v; else if (kv.first == "PodTopologySpread") c.w_pts = v;
         else if (kv.first == "InterPodAffinity") c.w_ipa = v; else if (kv.first == "NodeResourcesBalancedAllocation") c.w_balanced = v;
@@ -462,6 +466,14 @@ class Encoder {
         e.npods[i] += 1;
       }
     });
+    for (int i = 0; i < n; i++) {   // the engine refuses these too, by index; here the node is named
+      if (e.alloc_cpu[i] > CCSIM_MAX_SCORED_ALLOCATABLE)
+        throw Unsupported("node \"" + e.names[i] + "\": cpu allocatable " + std::to_string(e.alloc_cpu[i]) + "m exceeds " +
+                          std::to_string(CCSIM_MAX_SCORED_ALLOCATABLE) + "m (LeastAllocated's int64 score arithmetic)");
+      if (e.alloc_mem[i] > CCSIM_MAX_SCORED_ALLOCATABLE)
+        throw Unsupported("node \"" + e.names[i] + "\": memory allocatable " + std::to_string(e.alloc_mem[i]) + " exceeds " +
+                          std::to_string(CCSIM_MAX_SCORED_ALLOCATABLE) + " (LeastAllocated's int64 score arithmetic)");
+    }
     tick("node columns");
     // ---- taints: dictionary in first-seen order ----
     std::map<Taint, int> tid;

@@ -280,7 +280,12 @@ void ccsim_destroy(ccsim_handle *h);
 const char *ccsim_last_error(const ccsim_handle *h);  /* h may be NULL: last create error */
 int  ccsim_abi_version(void);
 
-/* snapshot upload (H2D inside the call) */
+/* Largest cpu (milli) / memory allocatable a node may have: LeastAllocated computes (capacity - requested) * 100 in int64
+ * (least_allocated.go:52-61), which wraps above this. ccsim_load_nodes refuses larger values with CCSIM_EUNSUPPORTED. */
+#define CCSIM_MAX_SCORED_ALLOCATABLE (INT64_MAX / 100)
+
+/* snapshot upload (H2D inside the call). ccsim_set_templates refuses negative plugin weights and LeastAllocated resource
+ * weights outside [1, 100] (validation_pluginargs.go), and weight sums whose scores do not fit the packed key. */
 int  ccsim_load_nodes(ccsim_handle *h, const ccsim_nodes *nodes);
 int  ccsim_set_templates(ccsim_handle *h, int32_t n_templates, const ccsim_template *templates,
                          int32_t n_counters, const ccsim_counter *counters);

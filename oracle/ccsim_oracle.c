@@ -26,6 +26,7 @@
 #include <string.h>
 #include <limits.h>
 #include <math.h>
+#include <assert.h>
 #ifdef _OPENMP
 #include <omp.h>
 #endif
@@ -399,6 +400,17 @@ int ccsim_oracle_run_ex(const ccsim_nodes *nd, int32_t n_templates, const ccsim_
     for (int t = 0; t < n_templates; t++)
       for (int c = 0; c < tmpl[t].n_pts; c++)
         if (tmpl[t].pts[c].counter == j && ctr[j].topo_col < 0) return CCSIM_EUNSUPPORTED;
+  /* Preconditions the engine checks too (ccsim_load_nodes / ccsim_set_templates): LeastAllocated's (capacity - requested) * 100
+     must not wrap, and no plugin weight is negative (so every feasible node's total is >= 0 > best's initial -1). Resource
+     weights in [1, 100]: NodeResourcesFitArgs validation (PL:../apis/config/validation/validation_pluginargs.go). */
+  for (int32_t i = 0; i < n; i++)
+    if (nd->alloc_cpu[i] > CCSIM_MAX_SCORED_ALLOCATABLE || nd->alloc_mem[i] > CCSIM_MAX_SCORED_ALLOCATABLE) return CCSIM_EUNSUPPORTED;
+  for (int t = 0; t < n_templates; t++) {
+    const ccsim_template *T = &tmpl[t];
+    if (T->w_taint < 0 || T->w_node_affinity < 0 || T->w_fit < 0 || T->w_pts < 0 || T->w_ipa < 0 || T->w_balanced < 0 || T->w_image < 0 ||
+        T->least_w_cpu < 1 || T->least_w_cpu > 100 || T->least_w_mem < 1 || T->least_w_mem > 100)
+      return CCSIM_EUNSUPPORTED;
+  }
 #ifdef _OPENMP
   if (threads > 0) omp_set_num_threads(threads);
 #else
@@ -585,6 +597,7 @@ int ccsim_oracle_run_ex(const ccsim_nodes *nd, int32_t n_templates, const ccsim_
       if (total > best) { best = total; besti = i; }
     }
     if (mode != 0) start = (int32_t)(((int64_t)start + examined) % n); /* KS:schedule_one.go:538-539 */
+    assert(besti >= 0);   /* feasible > 0 and every total >= 0 (the weight preconditions above) */
 
     /* assume -> Cache.AssumePod -> NodeInfo.AddPod -> update(+1): KS:framework/types.go:409-427 */
     const int32_t w = besti;
