@@ -59,16 +59,12 @@ __device__ __forceinline__ bool exchange_totals(const DevParams &p, long long k_
   return __any_sync(0xffffffffu, dead);
 }
 
+
 __global__ void __launch_bounds__(LEAN_THREADS, 1) ccsim_wave_batched_kernel(const DevParams p, const LeanParams lp) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
-  const uint32_t cnt_bytes = ((uint32_t)p.smem_cnt_ints * 4u + 15u) & ~15u;
-  uint4 *rec = reinterpret_cast<uint4 *>(smem_raw + cnt_bytes);
   const size_t cp = (size_t)p.chunk_pad;
-  long long *c_acpu = reinterpret_cast<long long *>(smem_raw + cnt_bytes + lp.rec_bytes_total);
-  long long *c_amem = c_acpu + cp, *c_rcpu = c_amem + cp, *c_rmem = c_rcpu + cp, *c_zcpu = c_rmem + cp, *c_zmem = c_zcpu + cp;
-  int32_t *c_apods = reinterpret_cast<int32_t *>(c_zmem + cp);
-  int32_t *c_npods = c_apods + cp;
-  int32_t *run = c_npods + cp;        // run length of each node in this wave (0: not tied at S*)
+  const LeanTile t = lean_tile(smem_raw, lp, cp);
+  int32_t *run = reinterpret_cast<int32_t *>(t.own);   // run length of each node in this wave (0: not tied at S*)
   int32_t *fscore = run + cp;         // memo score after the full run (-1: node ended the run infeasible)
   int32_t *off = fscore + cp;         // exclusive prefix of run[] in node order
 
@@ -76,35 +72,15 @@ __global__ void __launch_bounds__(LEAN_THREADS, 1) ccsim_wave_batched_kernel(con
   const int cta = blockIdx.x;
   const int32_t lo = min(p.n, cta * p.chunk), hi = min(p.n, lo + p.chunk);
   const int32_t cnt_nodes = hi - lo;
+  uint4 *rec = t.rec;
   const int su = lp.stride_u;
 
-  for (int32_t j = tid; j < cnt_nodes; j += LEAN_THREADS) {
-    const int32_t i = lo + j;
-    const long long ac = p.alloc_cpu[i], am = p.alloc_mem[i], rc = p.req_cpu[i], rm = p.req_mem[i];
-    const int32_t ap = p.alloc_pods[i], np = p.npods[i];
-    unsigned long long *r8 = reinterpret_cast<unsigned long long *>(rec + (size_t)j * su);
-    int32_t *r4 = reinterpret_cast<int32_t *>(r8);
-    r8[0] = p.taint_mask[i];
-    r8[1] = p.static_words > 0 ? p.static_mask[i] : 0ull;
-    r8[2] = (unsigned long long)(ac - rc);
-    r8[3] = (unsigned long long)(am - rm);
-    r4[8] = ap - np;
-    r4[9] = -1;
-    c_acpu[j] = ac; c_amem[j] = am; c_rcpu[j] = rc; c_rmem[j] = rm;
-    c_zcpu[j] = p.nz_cpu[i]; c_zmem[j] = p.nz_mem[i];
-    c_apods[j] = ap; c_npods[j] = np;
-  }
-  for (int k = tid; k < (int)(sizeof(ccsim_template) / 8); k += LEAN_THREADS)
-    reinterpret_cast<unsigned long long *>(&ls.tmpl)[k] = reinterpret_cast<const unsigned long long *>(&p.templates[0])[k];
-  if (tid == 0) { ls.aff_total = 0; ls.winner = -1; ls.stop = 0; ls.dirty = 1; }
-  __syncthreads();
+  lean_stage(p, lp, t, lo, cnt_nodes);
   if (tid == 0) { lean_build_consts(p, lp); ls.dirty = 0; }
   __syncthreads();
 
-  const unsigned long long taint_bad0 = ls.taint_bad0, sel0 = ls.sel0, forbid0 = ls.forbid0;
-  const long long eq_cpu = ls.eq_cpu, eq_mem = ls.eq_mem;
-  const int32_t pods_need = ls.pods_need;
-  const ccsim_template &t = ls.tmpl;
+  const LeanFit fit = lean_fit();
+  const ccsim_template &tm = ls.tmpl;
 
   long long k = 0, waves = 0, extra_evals = 0;
   bool limit_hit = false;   // postBindHook's limit (simulator.go:300-305)
@@ -117,23 +93,15 @@ __global__ void __launch_bounds__(LEAN_THREADS, 1) ccsim_wave_batched_kernel(con
     unsigned long long best = 0ull;
     for (int32_t j = tid; j < cnt_nodes; j += LEAN_THREADS) {
       const uint4 *r = rec + (size_t)j * su;
-      const uint4 u0 = r[0], u1 = r[1], u2 = r[2];
-      const unsigned long long taint0 = ((unsigned long long)u0.y << 32) | u0.x;
-      const unsigned long long static0 = ((unsigned long long)u0.w << 32) | u0.z;
-      const long long free_cpu = (long long)(((unsigned long long)u1.y << 32) | u1.x);
-      const long long free_mem = (long long)(((unsigned long long)u1.w << 32) | u1.z);
-      int32_t sc = (int32_t)u2.y;
-      bool ok = ((taint0 & taint_bad0) | (~static0 & sel0) | (static0 & forbid0)) == 0ull;
-      ok &= (free_cpu >= eq_cpu) & (free_mem >= eq_mem) & ((int32_t)u2.x >= pods_need);
+      const LeanRow w = lean_row(r);
+      int32_t sc = w.score;
+      const bool ok = lean_fits(w, fit);
       run[j] = 0;
       if (ok) {
-        if (sc < 0) {
-          sc = score_node(c_acpu[j], c_amem[j], c_zcpu[j] + t.least_cpu, c_zmem[j] + t.least_mem, c_rcpu[j] + t.bal_cpu, c_rmem[j] + t.bal_mem, ls.sw);
-          reinterpret_cast<int32_t *>(rec + (size_t)j * su)[9] = sc;
-        }
+        if (sc < 0) sc = lean_rescore(t, lp, j);
         const unsigned long long key = pack_key(sc, (uint32_t)(p.node_base + lo + j));
         best = key > best ? key : best;
-      } else if (sc >= 0) reinterpret_cast<int32_t *>(rec + (size_t)j * su)[9] = -2 - sc;   // remember: infeasible (memo kept as -2-score)
+      } else if (sc >= 0) reinterpret_cast<int32_t *>(rec + (size_t)j * su)[LR_SCORE] = -2 - sc;   // remember: infeasible (memo kept as -2-score)
     }
     { const unsigned long long v = warp_max_u64(best); if (lane == 0) ls.warp_best[warp][0] = v; }
     __syncthreads();                                                    // S1
@@ -159,19 +127,19 @@ __global__ void __launch_bounds__(LEAN_THREADS, 1) ccsim_wave_batched_kernel(con
     const int32_t sstar = ls.winner;
     // ---- runs of the tied nodes: place while feasible and score >= S* ----
     for (int32_t j = tid; j < cnt_nodes; j += LEAN_THREADS) {
-      const int32_t sc = reinterpret_cast<const int32_t *>(rec + (size_t)j * su)[9];
+      const int32_t sc = reinterpret_cast<const int32_t *>(rec + (size_t)j * su)[LR_SCORE];
       if (sc != sstar) continue;                                      // infeasible nodes carry a negative memo
-      long long rc = c_rcpu[j], rm = c_rmem[j], zc = c_zcpu[j], zm = c_zmem[j];
-      const long long ac = c_acpu[j], am = c_amem[j];
-      int32_t np = c_npods[j];
-      const int32_t ap = c_apods[j];
+      long long rc = t.rcpu[j], rm = t.rmem[j], zc = t.zcpu[j], zm = t.zmem[j];
+      const long long ac = t.acpu[j], am = t.amem[j];
+      int32_t np = t.npods[j];
+      const int32_t ap = t.apods[j];
       int32_t r = 0, cur = sstar;
       bool feasible = true;
       do {
-        r++; rc += t.req_cpu; rm += t.req_mem; zc += t.nz_cpu; zm += t.nz_mem; np++;
-        feasible = (ac - rc >= eq_cpu) & (am - rm >= eq_mem) & (ap - np >= pods_need);
+        r++; rc += tm.req_cpu; rm += tm.req_mem; zc += tm.nz_cpu; zm += tm.nz_mem; np++;
+        feasible = (ac - rc >= fit.eq_cpu) & (am - rm >= fit.eq_mem) & (ap - np >= fit.pods_need);
         if (!feasible) break;
-        cur = score_node(ac, am, zc + t.least_cpu, zm + t.least_mem, rc + t.bal_cpu, rm + t.bal_mem, ls.sw);
+        cur = score_node(ac, am, zc + tm.least_cpu, zm + tm.least_mem, rc + tm.bal_cpu, rm + tm.bal_mem, ls.sw);
       } while (cur >= sstar);
       run[j] = r;
       fscore[j] = feasible ? cur : -1;
@@ -211,18 +179,9 @@ __global__ void __launch_bounds__(LEAN_THREADS, 1) ccsim_wave_batched_kernel(con
       long long allowed = remaining - goff;
       allowed = allowed < 0 ? 0 : (allowed > r ? r : allowed);
       if (allowed == 0) continue;
+      lean_commit_row<false>(p, lp, t, j, (int32_t)allowed, (allowed == r) ? fscore[j] : -1);   // (no counters in this kernel)
       const int32_t w = lo + j;
-      const long long rc = c_rcpu[j] + allowed * t.req_cpu, rm = c_rmem[j] + allowed * t.req_mem;
-      const long long zc = c_zcpu[j] + allowed * t.nz_cpu, zm = c_zmem[j] + allowed * t.nz_mem;
-      const int32_t np = c_npods[j] + (int32_t)allowed;
-      c_rcpu[j] = rc; c_rmem[j] = rm; c_zcpu[j] = zc; c_zmem[j] = zm; c_npods[j] = np;
-      unsigned long long *r8 = reinterpret_cast<unsigned long long *>(rec + (size_t)j * su);
-      int32_t *r4 = reinterpret_cast<int32_t *>(r8);
-      r8[2] = (unsigned long long)(c_acpu[j] - rc);
-      r8[3] = (unsigned long long)(c_amem[j] - rm);
-      r4[8] = c_apods[j] - np;
-      r4[9] = (allowed == r) ? fscore[j] : -1;
-      p.req_cpu[w] = rc; p.req_mem[w] = rm; p.nz_cpu[w] = zc; p.nz_mem[w] = zm; p.npods[w] = np;
+      p.req_cpu[w] = t.rcpu[j]; p.req_mem[w] = t.rmem[j]; p.nz_cpu[w] = t.zcpu[j]; p.nz_mem[w] = t.zmem[j]; p.npods[w] = t.npods[j];   // write through
       const int32_t g = p.node_base + w;
       for (long long q = 0; q < allowed; q++) { const long long kk = k + goff + q; if (kk < p.pod_cap) p.pod_node[kk] = g; }
     }
@@ -236,6 +195,8 @@ __global__ void __launch_bounds__(LEAN_THREADS, 1) ccsim_wave_batched_kernel(con
     tag = (p.epoch << 12) | wtag;
   }
 
+  // (this kernel writes its commits through instead of using lean_finish: a write-back after the loop, or lean_finish's result
+  //  fields, cost it 8 B more stack, 12 B more spill stores and 20 B more spill loads)
   if (cta == 0 && tid == 0) {
     DevOut *o = p.out;
     o->placed = k;

@@ -1300,11 +1300,8 @@ static int run_prepare(ccsim_handle *h, int64_t max_pods) {
     }
     if (lean) {
       lp.n_slots = ns;
-      int units = (10 + ns + 3) / 4;
-      if ((units & 1) == 0) units++;
-      lp.stride_u = units;
-      lp.rec_bytes_total = (uint32_t)((size_t)units * 16 * p.chunk_pad);
-      const size_t smem_lean = cnt_bytes + lp.rec_bytes_total + (size_t)p.chunk_pad * (6 * 8 + 2 * 4 + (faithful ? 8 : 0));
+      lean_layout(lp, h->smem_cnt_ints, p.chunk_pad);
+      const size_t smem_lean = lean_smem_bytes(lp, p.chunk_pad, faithful ? 8 : 0);     // + the sampling pass's feasibility and rank
       if (smem_lean + sizeof(LeanShared) + 1024 > h->smem_optin) lean = false;
       else { smem = smem_lean; kern = faithful ? (const void *)ccsim_wave_lean_kernel<true> : (const void *)ccsim_wave_lean_kernel<false>; block = LEAN_THREADS; }
     }
@@ -1315,7 +1312,7 @@ static int run_prepare(ccsim_handle *h, int64_t max_pods) {
   bool batched = lean && !faithful && h->n_counters == 0 && h->max_prefer_pop == 0 && h->cfg.world == 1 &&
                  h->cfg.engine != CCSIM_ENGINE_SEQUENTIAL;
   if (batched) {
-    const size_t smem_b = smem + (size_t)p.chunk_pad * 12;
+    const size_t smem_b = lean_smem_bytes(lp, p.chunk_pad, 12);     // + run length, score after the run, run offset
     if (smem_b + sizeof(LeanShared) + sizeof(BatchShared) + 1024 > h->smem_optin) batched = false;
     else { smem = smem_b; kern = (const void *)ccsim_wave_batched_kernel; }
   }
@@ -1353,7 +1350,9 @@ static int run_prepare(ccsim_handle *h, int64_t max_pods) {
       if (shift + bits + 1 > MULTI_PAY_BITS) { multi = false; break; }
       mp.pay_shift[sl] = shift; mp.pay_mask[sl] = (1u << bits) - 1u; shift += bits + 1;   // + a zero guard bit (the replay's SWAR kill test)
     }
-    const size_t smem_m = smem + (size_t)p.chunk_pad * 8 + 16;     // + the per-node payload column
+    // + the per-node payload column, and 16 bytes that nothing reads: kept so that the kernel's shared-memory size, which
+    //   run_stats() reports, stays what it has been
+    const size_t smem_m = lean_smem_bytes(lp, p.chunk_pad, 8) + 16;
     if (smem_m + sizeof(LeanShared) + sizeof(MultiShared) + 1024 > h->smem_optin) multi = false;
     if (multi) { kern = h->cfg.world > 1 ? (const void *)ccsim_wave_multi_kernel<true> : (const void *)ccsim_wave_multi_kernel<false>; smem = smem_m; }
   }

@@ -24,6 +24,12 @@
 #define LT_ANTI 1
 #define LT_AFF 2
 
+// int32 indices into a node's hot record, after [taint0 | static0] [free_cpu | free_mem] (ints 0..7)
+#define LR_FREE_PODS 8
+#define LR_SCORE 9          /* memoised node-local score, < 0: stale */
+#define LR_SLOT0 10         /* extra slot s (domain id or node-local count) is int LR_SLOT0 + s */
+#define LEAN_COLD_BYTES (6 * 8 + 2 * 4)   /* cold SoA columns per node: alloc/req/nz cpu and mem (int64), alloc_pods, npods (int32) */
+
 // One per-domain term of the Filter pass, 16 bytes (one LDS.128). PodTopologySpread and anti-affinity share one form:
 //   reject  <=>  (node has the topology key) ? count(domain) > lim : miss_rejects
 // (PTS: lim = maxSkew - selfMatch + globalMin, missing key rejects; anti-affinity: lim = 0, missing key passes).
@@ -31,7 +37,7 @@
 struct __align__(16) LeanTerm {
   int16_t kind;      // LT_*
   int16_t miss_rejects;
-  int32_t slot;      // record int index (10 + s) holding the node's domain id, or the node-local count itself
+  int32_t slot;      // record int index (LR_SLOT0 + s) holding the node's domain id, or the node-local count itself
   int32_t cnt_off;   // offset of the counter in the shared replicated-counter area, -1: node-local (the slot IS the count)
   int32_t lim;
 };
@@ -42,10 +48,68 @@ struct LeanParams {
   int32_t slot_topo[LEAN_MAX_SLOTS];     // slot s mirrors topology column slot_topo[s] (>=0) ...
   int32_t slot_counter[LEAN_MAX_SLOTS];  // ... or node-local counter slot_counter[s] (>=0)
   int32_t counter_slot[CCSIM_MAX_COUNTERS]; // counter j -> slot holding its domain id (topo) or its count (node-local)
-  uint32_t rec_bytes_total; // stride * chunk_pad
-  uint32_t cold_off;        // byte offset of the cold SoA columns (alloc/req/nz) in dynamic shared memory
-  uint32_t cnt_off_bytes;   // byte offset of the replicated counters (0)
+  uint32_t rec_off, cold_off, own_off;   // byte offsets in dynamic shared memory (lean_layout)
 };
+
+// The tile of the lean, tie-run and multi-commit kernels in dynamic shared memory, one definition for the host (the kernel's
+// shared-memory size, lean_smem_bytes) and the kernels (their pointers, lean_tile):
+//   [replicated counters, padded to 16 B] [hot records: stride_u x 16 B per node] [cold columns: LEAN_COLD_BYTES per node]
+//   [the kernel's own per-node columns]
+inline void lean_layout(LeanParams &lp, int32_t cnt_ints, int32_t chunk_pad) {
+  int units = (LR_SLOT0 + lp.n_slots + 3) / 4;
+  if ((units & 1) == 0) units++;
+  lp.stride_u = units;
+  lp.rec_off = ((uint32_t)cnt_ints * 4u + 15u) & ~15u;
+  lp.cold_off = lp.rec_off + (uint32_t)units * 16u * (uint32_t)chunk_pad;
+  lp.own_off = lp.cold_off + (uint32_t)LEAN_COLD_BYTES * (uint32_t)chunk_pad;
+}
+inline size_t lean_smem_bytes(const LeanParams &lp, int32_t chunk_pad, size_t own_bytes_per_node) {
+  return (size_t)lp.own_off + own_bytes_per_node * (size_t)chunk_pad;
+}
+
+struct LeanTile {
+  int32_t *cnt;                                     // replicated counter cells
+  uint4 *rec;                                       // hot records
+  long long *acpu, *amem, *rcpu, *rmem, *zcpu, *zmem;
+  int32_t *apods, *npods;
+  unsigned char *own;                               // the kernel's own columns
+  int32_t su;                                       // record stride in 16-byte units
+};
+
+__device__ __forceinline__ LeanTile lean_tile(unsigned char *smem, const LeanParams &lp, size_t cp) {
+  LeanTile t;
+  t.cnt = reinterpret_cast<int32_t *>(smem);
+  t.rec = reinterpret_cast<uint4 *>(smem + lp.rec_off);
+  t.acpu = reinterpret_cast<long long *>(smem + lp.cold_off);
+  t.amem = t.acpu + cp; t.rcpu = t.amem + cp; t.rmem = t.rcpu + cp; t.zcpu = t.rmem + cp; t.zmem = t.zcpu + cp;
+  t.apods = reinterpret_cast<int32_t *>(t.zmem + cp);
+  t.npods = t.apods + cp;
+  t.own = smem + lp.own_off;
+  t.su = lp.stride_u;
+  return t;
+}
+
+__device__ __forceinline__ int32_t *lean_rec4(const LeanTile &t, const LeanParams &lp, int32_t j) {
+  return reinterpret_cast<int32_t *>(t.rec + (size_t)j * t.su);
+}
+
+// a hot record unpacked
+struct LeanRow {
+  unsigned long long taint0, static0;
+  long long free_cpu, free_mem;
+  int32_t free_pods, score;
+};
+__device__ __forceinline__ LeanRow lean_row(const uint4 *r) {
+  const uint4 u0 = r[0], u1 = r[1], u2 = r[2];
+  LeanRow w;
+  w.taint0 = ((unsigned long long)u0.y << 32) | u0.x;
+  w.static0 = ((unsigned long long)u0.w << 32) | u0.z;
+  w.free_cpu = (long long)(((unsigned long long)u1.y << 32) | u1.x);
+  w.free_mem = (long long)(((unsigned long long)u1.w << 32) | u1.z);
+  w.free_pods = (int32_t)u2.x;
+  w.score = (int32_t)u2.y;
+  return w;
+}
 
 struct __align__(16) LeanShared {
   ccsim_template tmpl;
@@ -66,6 +130,66 @@ struct __align__(16) LeanShared {
 };
 
 __shared__ LeanShared ls;
+
+// the node-local part of the Filter pass: NodeUnschedulable, TaintToleration, NodeAffinity(nodeSelector), NodePorts, existing
+// anti-affinity, NodeResourcesFit (the constants are ls's, read by the caller where it wants them in registers)
+struct LeanFit {
+  unsigned long long taint_bad0, sel0, forbid0;
+  long long eq_cpu, eq_mem;
+  int32_t pods_need;
+};
+__device__ __forceinline__ LeanFit lean_fit() {
+  LeanFit f;
+  f.taint_bad0 = ls.taint_bad0; f.sel0 = ls.sel0; f.forbid0 = ls.forbid0;
+  f.eq_cpu = ls.eq_cpu; f.eq_mem = ls.eq_mem; f.pods_need = ls.pods_need;
+  return f;
+}
+__device__ __forceinline__ bool lean_fits(const LeanRow &w, const LeanFit &f) {
+  bool ok = ((w.taint0 & f.taint_bad0) | (~w.static0 & f.sel0) | (w.static0 & f.forbid0)) == 0ull;
+  ok &= (w.free_cpu >= f.eq_cpu) & (w.free_mem >= f.eq_mem) & (w.free_pods >= f.pods_need);
+  return ok;
+}
+
+// the count of a per-domain term for the node of record r4, and whether the node has the term's topology key
+__device__ __forceinline__ int32_t lean_term_count(const int32_t *r4, const int32_t *cnt, const LeanTerm &lt, bool &has) {
+  const int32_t v = r4[lt.slot];                                  // domain id, or the node-local count
+  const bool local = lt.cnt_off < 0;
+  has = local | (v >= 0);
+  return local ? v : cnt[lt.cnt_off + (v < 0 ? 0 : v)];
+}
+
+// a stale score memo: the node was committed since its score was last computed; score it again and memoise
+__device__ __forceinline__ int32_t lean_rescore(const LeanTile &t, const LeanParams &lp, int32_t j) {
+  const ccsim_template &tm = ls.tmpl;
+  const int32_t sc = score_node(t.acpu[j], t.amem[j], t.zcpu[j] + tm.least_cpu, t.zmem[j] + tm.least_mem,
+                                t.rcpu[j] + tm.bal_cpu, t.rmem[j] + tm.bal_mem, ls.sw);
+  lean_rec4(t, lp, j)[LR_SCORE] = sc;
+  return sc;
+}
+
+// assume -> AssumePod -> NodeInfo.update(+1) for `count` clones on tile node j (schedule_one.go:967-984, types.go:409-427): the
+// cold columns, the hot record and (LOCAL_COUNTERS) the node-local counters. `memo`: the node's score after them, or -1 (stale).
+// The lean kernel bumps the node-local counters in its counter lanes instead: a loop on its commit lane made every sequential
+// cycle ~5 % longer (C4 spread-only, ENGINE_SEQUENTIAL, one H100).
+template <bool LOCAL_COUNTERS = true>
+__device__ __forceinline__ void lean_commit_row(const DevParams &p, const LeanParams &lp, const LeanTile &t, int32_t j, int32_t count,
+                                                int32_t memo) {
+  const ccsim_template &tm = ls.tmpl;
+  const long long rc = t.rcpu[j] + count * tm.req_cpu, rm = t.rmem[j] + count * tm.req_mem;
+  const int32_t np = t.npods[j] + count;
+  t.rcpu[j] = rc; t.rmem[j] = rm; t.zcpu[j] += count * tm.nz_cpu; t.zmem[j] += count * tm.nz_mem; t.npods[j] = np;
+  int32_t *r4 = lean_rec4(t, lp, j);
+  unsigned long long *r8 = reinterpret_cast<unsigned long long *>(r4);
+  r8[2] = (unsigned long long)(t.acpu[j] - rc);
+  r8[3] = (unsigned long long)(t.amem[j] - rm);
+  r4[LR_FREE_PODS] = t.apods[j] - np;
+  r4[LR_SCORE] = memo;
+  if (LOCAL_COUNTERS)
+    for (int c = 0; c < p.n_counters; c++) {
+      const CommitInfo &ci = ls.cinfo[c];
+      if (ci.inc && ci.local) r4[LR_SLOT0 + lp.counter_slot[c]] += count * ci.inc;
+    }
+}
 
 // one thread: fold the template into the lean constants (see build_filter_consts for the generic kernel)
 __device__ void lean_build_consts(const DevParams &p, const LeanParams &lp) {
@@ -94,7 +218,7 @@ __device__ void lean_build_consts(const DevParams &p, const LeanParams &lp) {
       LeanTerm &lt = ls.terms[nt++];
       const int j = t.pts[c].counter;
       lt.kind = LT_PTS; lt.miss_rejects = 1;
-      lt.slot = 10 + lp.counter_slot[j];
+      lt.slot = LR_SLOT0 + lp.counter_slot[j];
       lt.cnt_off = p.counters[j].topo_col < 0 ? -1 : p.counters[j].smem_off;
       const long long lim = (long long)t.pts[c].max_skew - t.pts[c].self_match + (long long)ls.ptsmin[c];
       lt.lim = lim > INT32_MAX ? INT32_MAX : (lim < INT32_MIN ? INT32_MIN : (int32_t)lim);
@@ -105,7 +229,7 @@ __device__ void lean_build_consts(const DevParams &p, const LeanParams &lp) {
       LeanTerm &lt = ls.terms[nt++];
       const int j = t.anti_counter[a];
       lt.kind = LT_ANTI; lt.miss_rejects = 0; lt.lim = 0;
-      lt.slot = 10 + lp.counter_slot[j];
+      lt.slot = LR_SLOT0 + lp.counter_slot[j];
       lt.cnt_off = p.counters[j].topo_col < 0 ? -1 : p.counters[j].smem_off;
     }
   ls.n_cmp_terms = nt;
@@ -114,7 +238,7 @@ __device__ void lean_build_consts(const DevParams &p, const LeanParams &lp) {
       LeanTerm &lt = ls.terms[nt++];
       const int j = t.aff_counter[a];
       lt.kind = LT_AFF; lt.miss_rejects = 1; lt.lim = 0;
-      lt.slot = 10 + lp.counter_slot[j];
+      lt.slot = LR_SLOT0 + lp.counter_slot[j];
       lt.cnt_off = p.counters[j].topo_col < 0 ? -1 : p.counters[j].smem_off;
       ls.has_aff = 1;
     }
@@ -150,21 +274,84 @@ __device__ void lean_pts_recount(const DevParams &p, const int32_t *smem_cnt, in
   __syncthreads();
 }
 
+// after a wave: recount every PTS minimum whose last domain at the minimum took a clone (all of them when `force`)
+__device__ __forceinline__ void lean_pts_after_wave(const DevParams &p, const int32_t *smem_cnt, bool force) {
+  for (int c = 0; c < ls.tmpl.n_pts; c++)
+    if (!ls.tmpl.pts[c].min_zero && (ls.ptsnum[c] <= 0 || force) && p.counters[ls.tmpl.pts[c].counter].n_present > 0) lean_pts_recount(p, smem_cnt, c);
+}
+
+// Stage the tile (once): hot AoS records and cold SoA columns of tile nodes [0, cnt_nodes) = global [lo, lo + cnt_nodes),
+// template 0, the replicated counter cells, ls's run state (all threads, ends after a barrier).
+__device__ __forceinline__ void lean_stage(const DevParams &p, const LeanParams &lp, const LeanTile &t, int32_t lo, int32_t cnt_nodes) {
+  const int tid = threadIdx.x;
+  for (int32_t j = tid; j < cnt_nodes; j += LEAN_THREADS) {
+    const int32_t i = lo + j;
+    const long long ac = p.alloc_cpu[i], am = p.alloc_mem[i], rc = p.req_cpu[i], rm = p.req_mem[i];
+    const int32_t ap = p.alloc_pods[i], np = p.npods[i];
+    int32_t *r4 = lean_rec4(t, lp, j);
+    unsigned long long *r8 = reinterpret_cast<unsigned long long *>(r4);
+    r8[0] = p.taint_mask[i];
+    r8[1] = p.static_words > 0 ? p.static_mask[i] : 0ull;
+    r8[2] = (unsigned long long)(ac - rc);
+    r8[3] = (unsigned long long)(am - rm);
+    r4[LR_FREE_PODS] = ap - np;
+    r4[LR_SCORE] = -1;
+    for (int s = 0; s < lp.n_slots; s++)
+      r4[LR_SLOT0 + s] = lp.slot_topo[s] >= 0 ? p.topo[lp.slot_topo[s]][i] : p.counters[lp.slot_counter[s]].work[i];
+    t.acpu[j] = ac; t.amem[j] = am; t.rcpu[j] = rc; t.rmem[j] = rm;
+    t.zcpu[j] = p.nz_cpu[i]; t.zmem[j] = p.nz_mem[i];
+    t.apods[j] = ap; t.npods[j] = np;
+  }
+  for (int k = tid; k < (int)(sizeof(ccsim_template) / 8); k += LEAN_THREADS)
+    reinterpret_cast<unsigned long long *>(&ls.tmpl)[k] = reinterpret_cast<const unsigned long long *>(&p.templates[0])[k];
+  for (int j = 0; j < p.n_counters; j++) {
+    const DevCounter &dc = p.counters[j];
+    if (dc.topo_col < 0) continue;
+    for (int d = tid; d < dc.n_domains; d += LEAN_THREADS) t.cnt[dc.smem_off + d] = dc.init[d];
+  }
+  if (tid == 0) { ls.aff_total = p.templates[0].aff_total_init; ls.winner = -1; ls.stop = 0; ls.dirty = 1; ls.examined = 0; ls.examined_total = 0; }
+  __syncthreads();
+}
+
+// After the run: the tile goes back to the global columns once (the mutable columns and the node-local counters: the snapshot
+// after the run, read by the terminal diagnosis), and CTA 0 writes the final replicated counters and the result fields the
+// lean and multi-commit kernels report. Returns p.out to thread 0 of CTA 0, which fills in the kernel's own fields; nullptr elsewhere.
+__device__ __forceinline__ DevOut *lean_finish(const DevParams &p, const LeanParams &lp, const LeanTile &t, int32_t lo, int32_t cnt_nodes,
+                                               long long placed, bool limit_hit) {
+  const int tid = threadIdx.x;
+  for (int32_t j = tid; j < cnt_nodes; j += LEAN_THREADS) {
+    const int32_t i = lo + j;
+    p.req_cpu[i] = t.rcpu[j]; p.req_mem[i] = t.rmem[j]; p.nz_cpu[i] = t.zcpu[j]; p.nz_mem[i] = t.zmem[j]; p.npods[i] = t.npods[j];
+    const int32_t *r4 = lean_rec4(t, lp, j);
+    for (int s = 0; s < lp.n_slots; s++) if (lp.slot_topo[s] < 0) p.counters[lp.slot_counter[s]].work[i] = r4[LR_SLOT0 + s];
+  }
+  if (blockIdx.x != 0) return nullptr;
+  for (int j = 0; j < p.n_counters; j++) {
+    const DevCounter &dc = p.counters[j];
+    if (dc.topo_col < 0) continue;
+    for (int d = tid; d < dc.n_domains; d += LEAN_THREADS) p.final_cnt[p.final_off[j] + d] = t.cnt[dc.smem_off + d];
+  }
+  if (tid != 0) return nullptr;
+  DevOut *o = p.out;
+  o->placed = placed;
+  o->stop_code = limit_hit ? CCSIM_STOP_LIMIT_REACHED : CCSIM_STOP_UNSCHEDULABLE;
+  o->error = (ls.stop == 3) ? 1 : 0;
+  for (int c = 0; c < CCSIM_MAX_PTS; c++) o->ptsmin[c] = c < ls.tmpl.n_pts ? ls.ptsmin[c] : 0;
+  o->aff_total = ls.aff_total;
+  return o;
+}
+
 // FAITHFUL: the reference's default sampling (adaptive numFeasibleNodesToFind + rotating start index,
 // schedule_one.go:538-539,644-723) as a deterministic sequential scan: only the first K feasible nodes in rotated order
 // compete, ties -> first maximum in rotated order, and the start index advances by the number of nodes examined.
 template <bool FAITHFUL>
 __global__ void __launch_bounds__(LEAN_THREADS, 1) ccsim_wave_lean_kernel(const DevParams p, const LeanParams lp) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
-  int32_t *smem_cnt = reinterpret_cast<int32_t *>(smem_raw);
-  const uint32_t cnt_bytes = ((uint32_t)p.smem_cnt_ints * 4u + 15u) & ~15u;
-  uint4 *rec = reinterpret_cast<uint4 *>(smem_raw + cnt_bytes);
   const size_t cp = (size_t)p.chunk_pad;
-  long long *c_acpu = reinterpret_cast<long long *>(smem_raw + cnt_bytes + lp.rec_bytes_total);
-  long long *c_amem = c_acpu + cp, *c_rcpu = c_amem + cp, *c_rmem = c_rcpu + cp, *c_zcpu = c_rmem + cp, *c_zmem = c_zcpu + cp;
-  int32_t *c_apods = reinterpret_cast<int32_t *>(c_zmem + cp);
-  int32_t *c_npods = c_apods + cp;
-  int32_t *feas = c_npods + cp;     // FAITHFUL only: feasibility flag and exclusive feasible-rank of every tile node
+  const LeanTile t = lean_tile(smem_raw, lp, cp);
+  int32_t *smem_cnt = t.cnt;
+  uint4 *rec = t.rec;   // (the rows below are addressed as rec + j * su: through lean_rec4, lean<true> spilled 24 more bytes)
+  int32_t *feas = reinterpret_cast<int32_t *>(t.own);   // FAITHFUL only: feasibility flag and exclusive feasible-rank of every tile node
   int32_t *pre = feas + cp;
 
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -175,34 +362,7 @@ __global__ void __launch_bounds__(LEAN_THREADS, 1) ccsim_wave_lean_kernel(const 
   const int su = lp.stride_u;
   uint32_t start = 0;               // sched.nextStartNodeIndex (FAITHFUL)
 
-  // ---- stage the tile (once): hot AoS records + cold SoA columns ----
-  for (int32_t j = tid; j < cnt_nodes; j += LEAN_THREADS) {
-    const int32_t i = lo + j;
-    const long long ac = p.alloc_cpu[i], am = p.alloc_mem[i], rc = p.req_cpu[i], rm = p.req_mem[i];
-    const int32_t ap = p.alloc_pods[i], np = p.npods[i];
-    unsigned long long *r8 = reinterpret_cast<unsigned long long *>(rec + (size_t)j * su);
-    int32_t *r4 = reinterpret_cast<int32_t *>(r8);
-    r8[0] = p.taint_mask[i];
-    r8[1] = p.static_words > 0 ? p.static_mask[i] : 0ull;
-    r8[2] = (unsigned long long)(ac - rc);
-    r8[3] = (unsigned long long)(am - rm);
-    r4[8] = ap - np;
-    r4[9] = -1;
-    for (int s = 0; s < lp.n_slots; s++)
-      r4[10 + s] = lp.slot_topo[s] >= 0 ? p.topo[lp.slot_topo[s]][i] : p.counters[lp.slot_counter[s]].work[i];
-    c_acpu[j] = ac; c_amem[j] = am; c_rcpu[j] = rc; c_rmem[j] = rm;
-    c_zcpu[j] = p.nz_cpu[i]; c_zmem[j] = p.nz_mem[i];
-    c_apods[j] = ap; c_npods[j] = np;
-  }
-  for (int k = tid; k < (int)(sizeof(ccsim_template) / 8); k += LEAN_THREADS)
-    reinterpret_cast<unsigned long long *>(&ls.tmpl)[k] = reinterpret_cast<const unsigned long long *>(&p.templates[0])[k];
-  for (int j = 0; j < p.n_counters; j++) {
-    const DevCounter &dc = p.counters[j];
-    if (dc.topo_col < 0) continue;
-    for (int d = tid; d < dc.n_domains; d += LEAN_THREADS) smem_cnt[dc.smem_off + d] = dc.init[d];
-  }
-  if (tid == 0) { ls.aff_total = p.templates[0].aff_total_init; ls.winner = -1; ls.stop = 0; ls.dirty = 1; ls.examined = 0; ls.examined_total = 0; }
-  __syncthreads();
+  lean_stage(p, lp, t, lo, cnt_nodes);
   for (int c = 0; c < ls.tmpl.n_pts; c++) lean_pts_recount(p, smem_cnt, c);
 
 #ifdef CCSIM_PHASE_TIMERS
@@ -222,9 +382,9 @@ __global__ void __launch_bounds__(LEAN_THREADS, 1) ccsim_wave_lean_kernel(const 
       if (tid == 0) ls.dirty = 0;
     }
     // ---- fused Filter pass: one predicate-eval per node of the tile ----
-    const unsigned long long taint_bad0 = ls.taint_bad0, prefer0 = ls.prefer0, sel0 = ls.sel0, forbid0 = ls.forbid0;
-    const long long eq_cpu = ls.eq_cpu, eq_mem = ls.eq_mem;
-    const int32_t pods_need = ls.pods_need, n_terms = ls.n_terms, n_cmp = ls.n_cmp_terms;
+    const LeanFit fit = lean_fit();
+    const unsigned long long prefer0 = ls.prefer0;
+    const int32_t n_terms = ls.n_terms, n_cmp = ls.n_cmp_terms;
     unsigned long long best = 0ull;      // single class
     unsigned long long bestc[CCSIM_MAX_CLASSES];
     if (ncls > 1) {
@@ -233,26 +393,17 @@ __global__ void __launch_bounds__(LEAN_THREADS, 1) ccsim_wave_lean_kernel(const 
     }
     for (int32_t j = tid; j < cnt_nodes; j += LEAN_THREADS) {
       const uint4 *r = rec + (size_t)j * su;
-      const uint4 u0 = r[0], u1 = r[1], u2 = r[2];
-      const unsigned long long taint0 = ((unsigned long long)u0.y << 32) | u0.x;
-      const unsigned long long static0 = ((unsigned long long)u0.w << 32) | u0.z;
-      const long long free_cpu = (long long)(((unsigned long long)u1.y << 32) | u1.x);
-      const long long free_mem = (long long)(((unsigned long long)u1.w << 32) | u1.z);
-      const int32_t free_pods = (int32_t)u2.x;
-      int32_t sc = (int32_t)u2.y;
-      // NodeUnschedulable, TaintToleration, NodeAffinity(nodeSelector), NodePorts, existing anti-affinity, NodeResourcesFit
-      bool ok = ((taint0 & taint_bad0) | (~static0 & sel0) | (static0 & forbid0)) == 0ull;
-      ok &= (free_cpu >= eq_cpu) & (free_mem >= eq_mem) & (free_pods >= pods_need);
+      const LeanRow w = lean_row(r);
+      const unsigned long long taint0 = w.taint0;
+      int32_t sc = w.score;
+      bool ok = lean_fits(w, fit);
       // PodTopologySpread + anti-affinity terms: reject <=> has ? count > lim : miss_rejects
       if (n_cmp) {
         const int32_t *r4 = reinterpret_cast<const int32_t *>(r);
         #pragma unroll 4
         for (int q = 0; q < n_cmp; q++) {
           const LeanTerm lt = ls.terms[q];
-          const int32_t v = r4[lt.slot];                                  // domain id, or the node-local count
-          const bool local = lt.cnt_off < 0;
-          const int32_t c = local ? v : smem_cnt[lt.cnt_off + (v < 0 ? 0 : v)];
-          const bool has = local | (v >= 0);
+          bool has; const int32_t c = lean_term_count(r4, smem_cnt, lt, has);
           ok &= has ? (c <= lt.lim) : (lt.miss_rejects == 0);
         }
       }
@@ -261,21 +412,14 @@ __global__ void __launch_bounds__(LEAN_THREADS, 1) ccsim_wave_lean_kernel(const 
         bool aff_exist = true, aff_missing = false;
         for (int q = n_cmp; q < n_terms; q++) {
           const LeanTerm lt = ls.terms[q];
-          const int32_t v = r4[lt.slot];
-          const bool local = lt.cnt_off < 0;
-          const int32_t c = local ? v : smem_cnt[lt.cnt_off + (v < 0 ? 0 : v)];
-          const bool has = local | (v >= 0);
+          bool has; const int32_t c = lean_term_count(r4, smem_cnt, lt, has);
           aff_missing |= !has; aff_exist &= has & (c > 0);
         }
         ok &= !(aff_missing | (!aff_exist & !ls.aff_bypass));
       }
       if (FAITHFUL) feas[j] = ok ? 1 : 0;
       if (ok) {
-        if (sc < 0) {   // stale memo: this node was committed since its score was last computed
-          sc = score_node(c_acpu[j], c_amem[j], c_zcpu[j] + ls.tmpl.least_cpu, c_zmem[j] + ls.tmpl.least_mem,
-                          c_rcpu[j] + ls.tmpl.bal_cpu, c_rmem[j] + ls.tmpl.bal_mem, ls.sw);
-          reinterpret_cast<int32_t *>(rec + (size_t)j * su)[9] = sc;
-        }
+        if (sc < 0) sc = lean_rescore(t, lp, j);
         if (FAITHFUL) continue;     // keys are built after the sampling cut is known
         const unsigned long long key = pack_key(sc, (uint32_t)(p.node_base + lo + j));
         if (ncls == 1) best = key > best ? key : best;
@@ -328,7 +472,7 @@ __global__ void __launch_bounds__(LEAN_THREADS, 1) ccsim_wave_lean_kernel(const 
         const uint32_t gidx = (uint32_t)(p.node_base + lo + j);
         const uint32_t rot = gidx >= start ? gidx - start : gidx + (uint32_t)p.n_global - start;
         if (gr == K - 1) kth = (unsigned long long)rot + 1ull;
-        const int32_t sc = reinterpret_cast<const int32_t *>(rec + (size_t)j * su)[9];
+        const int32_t sc = reinterpret_cast<const int32_t *>(rec + (size_t)j * su)[LR_SCORE];
         const unsigned long long key = pack_key(sc, rot);     // ties -> first in rotated order
         if (ncls == 1) best = key > best ? key : best;
         else {
@@ -354,7 +498,7 @@ __global__ void __launch_bounds__(LEAN_THREADS, 1) ccsim_wave_lean_kernel(const 
     PH_MARK(1);
 
     if (warp == 0) {
-      const ccsim_template &t = ls.tmpl;
+      const ccsim_template &tm = ls.tmpl;
       const unsigned long long tagbits = (unsigned long long)tag << KEY_TAG_SHIFT;
       unsigned long long *myslots = p.slots + ((size_t)(k & 1) * CCSIM_MAX_GRID + cta) * SLOT_STRIDE;
       for (int c = 0; c < ncls; c++) {
@@ -381,7 +525,7 @@ __global__ void __launch_bounds__(LEAN_THREADS, 1) ccsim_wave_lean_kernel(const 
       }
       if (p.world > 1 && !dead) dead = cross_gpu_exchange(p, k, tag, ncls, cbest, lane, cta);
       PH_MARK(3);
-      const unsigned long long wkey = select_host_over_classes(cbest, ncls, t);
+      const unsigned long long wkey = select_host_over_classes(cbest, ncls, tm);
       if (lane == 0) {
         if (dead) { ls.stop = 3; ls.winner = -1; }
         else if (wkey == 0ull) { ls.stop = 1; ls.winner = -1; }
@@ -391,24 +535,14 @@ __global__ void __launch_bounds__(LEAN_THREADS, 1) ccsim_wave_lean_kernel(const 
           if (cta == 0) ls.examined_total += ls.examined;
         }
       }
-      // ---- commit (assume -> AssumePod -> NodeInfo.update(+1): schedule_one.go:967-984, types.go:409-427) ----
+      // ---- commit: the owner's row (lean_commit_row) and every CTA's replicated counters ----
       if (!dead && wkey != 0ull) {
         const int32_t g = FAITHFUL ? (int32_t)(((unsigned long long)start + key_index(wkey)) % (unsigned long long)p.n_global) : (int32_t)key_index(wkey);
         const int32_t w = g - p.node_base;
         const bool mine = (w >= lo && w < hi);
         const int32_t jw = w - lo;
         if (mine && lane == 31) {
-          const long long rc = c_rcpu[jw] + t.req_cpu, rm = c_rmem[jw] + t.req_mem;
-          const long long zc = c_zcpu[jw] + t.nz_cpu, zm = c_zmem[jw] + t.nz_mem;
-          const int32_t np = c_npods[jw] + 1;
-          c_rcpu[jw] = rc; c_rmem[jw] = rm; c_zcpu[jw] = zc; c_zmem[jw] = zm; c_npods[jw] = np;
-          unsigned long long *r8 = reinterpret_cast<unsigned long long *>(rec + (size_t)jw * su);
-          int32_t *r4 = reinterpret_cast<int32_t *>(r8);
-          r8[2] = (unsigned long long)(c_acpu[jw] - rc);
-          r8[3] = (unsigned long long)(c_amem[jw] - rm);
-          r4[8] = c_apods[jw] - np;
-          r4[9] = -1;            // this node's NodeInfo generation changed: its memoised score is stale
-          p.req_cpu[w] = rc; p.req_mem[w] = rm; p.nz_cpu[w] = zc; p.nz_mem[w] = zm; p.npods[w] = np;   // write through
+          lean_commit_row<false>(p, lp, t, jw, 1, -1);      // this node's NodeInfo generation changed: its memoised score is stale
           if (k < p.pod_cap) p.pod_node[k] = g; else ls.stop = 3;
         }
         if (p.world > 1 && !mine && cta == 0 && lane == 31) {   // sharded run: every rank keeps the whole pod -> node sequence
@@ -420,18 +554,13 @@ __global__ void __launch_bounds__(LEAN_THREADS, 1) ccsim_wave_lean_kernel(const 
           const CommitInfo ci = ls.cinfo[j];
           if (ci.inc) {
             if (ci.local) {
-              if (mine) {
-                int32_t *r4 = reinterpret_cast<int32_t *>(rec + (size_t)jw * su);
-                const int32_t nv = r4[10 + lp.counter_slot[j]] + ci.inc;
-                r4[10 + lp.counter_slot[j]] = nv;
-                p.counters[j].work[w] = nv;
-              }
+              if (mine) reinterpret_cast<int32_t *>(rec + (size_t)jw * su)[LR_SLOT0 + lp.counter_slot[j]] += ci.inc;
               if (ci.is_aff) { atomicAdd((unsigned long long *)&ls.aff_total, (unsigned long long)ci.inc); ls.dirty = 1; }
             } else {
               // the winner's domain id: from this CTA's tile if it owns the node, else from the whole-cluster column (L2).
               // (Carrying the ids with the exchanged key instead — as extra words or packed into the key's low bits — lengthens every
               //  CTA's exchange for a lookup only the non-owner CTAs make.)
-              const int32_t dom = mine ? reinterpret_cast<const int32_t *>(rec + (size_t)jw * su)[10 + lp.counter_slot[j]] : ci.gtopo[g];
+              const int32_t dom = mine ? reinterpret_cast<const int32_t *>(rec + (size_t)jw * su)[LR_SLOT0 + lp.counter_slot[j]] : ci.gtopo[g];
               if (dom >= 0) {
                 int32_t *cnt = smem_cnt + p.counters[j].smem_off;
                 const int32_t old = cnt[dom];
@@ -448,32 +577,18 @@ __global__ void __launch_bounds__(LEAN_THREADS, 1) ccsim_wave_lean_kernel(const 
     __syncthreads();                                                    // S2
     PH_MARK(5);
     if (ls.stop) break;
-    for (int c = 0; c < ls.tmpl.n_pts; c++)
-      if (!ls.tmpl.pts[c].min_zero && ls.ptsnum[c] <= 0 && p.counters[ls.tmpl.pts[c].counter].n_present > 0) lean_pts_recount(p, smem_cnt, c);
+    lean_pts_after_wave(p, smem_cnt, false);
     wtag = (wtag == 4095u) ? 1u : wtag + 1u;
     tag = (p.epoch << 12) | wtag;
     if (FAITHFUL) start = (uint32_t)(((unsigned long long)start + (unsigned long long)ls.examined) % (unsigned long long)p.n_global);
   }
 
-  if (cta == 0) {
-    for (int j = 0; j < p.n_counters; j++) {
-      const DevCounter &dc = p.counters[j];
-      if (dc.topo_col < 0) continue;
-      for (int d = tid; d < dc.n_domains; d += LEAN_THREADS) p.final_cnt[p.final_off[j] + d] = smem_cnt[dc.smem_off + d];
-    }
-    if (tid == 0) {
-      DevOut *o = p.out;
-      o->placed = k;
-      o->stop_code = limit_hit ? CCSIM_STOP_LIMIT_REACHED : CCSIM_STOP_UNSCHEDULABLE;
-      o->error = (ls.stop == 3) ? 1 : 0;
-      o->waves = limit_hit ? k : k + 1;
-      o->evals = o->waves * (long long)p.n;
-      o->examined = FAITHFUL ? ls.examined_total : o->evals;
-      for (int c = 0; c < CCSIM_MAX_PTS; c++) o->ptsmin[c] = ls.ptsmin[c];
-      o->aff_total = ls.aff_total;
+  if (DevOut *o = lean_finish(p, lp, t, lo, cnt_nodes, k, limit_hit)) {
+    o->waves = limit_hit ? k : k + 1;
+    o->evals = o->waves * (long long)p.n;
+    o->examined = FAITHFUL ? ls.examined_total : o->evals;
 #ifdef CCSIM_PHASE_TIMERS
-      for (int q = 0; q < 8; q++) o->phase_cycles[q] = ph[q];
+    for (int q = 0; q < 8; q++) o->phase_cycles[q] = ph[q];
 #endif
-    }
   }
 }

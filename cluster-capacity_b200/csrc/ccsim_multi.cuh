@@ -169,6 +169,23 @@ __device__ __forceinline__ void multi_append(bool keep, uint32_t ck, unsigned lo
   }
 }
 
+// More candidates than the replay holds: the bar T is raised to the lowest of MULTI_BINS equal steps between T and the best key
+// that leaves <= MULTI_CAP candidates; every CTA sees the same data and decides alike. The caller counts its candidates into
+// ms.hist with multi_hist_add; multi_raise_bar returns the new T with the candidate arrays emptied (all threads, two barriers).
+__device__ __forceinline__ void multi_hist_add(uint32_t ck, uint32_t T, unsigned long long range) {
+  if (ck != 0u && ck >= T) atomicAdd(&ms.hist[(unsigned)(((unsigned long long)(ck - T) * MULTI_BINS) / range)], 1u);
+}
+__device__ __forceinline__ uint32_t multi_raise_bar(uint32_t T, uint32_t kbest, unsigned long long range, int cta) {
+  int bsel = MULTI_BINS;
+  { unsigned sum = 0; for (int bq = MULTI_BINS - 1; bq >= 0; bq--) { sum += ms.hist[bq]; if (sum > (unsigned)MULTI_CAP) break; bsel = bq; } }
+  T = (bsel >= MULTI_BINS) ? kbest : T + (uint32_t)(((unsigned long long)bsel * range + (MULTI_BINS - 1)) / MULTI_BINS);
+  __syncthreads();
+  if (threadIdx.x == 0) ms.ncand = 0;
+  if (cta == 0 && threadIdx.x == 0) ms.st_overflow++;
+  __syncthreads();
+  return T;
+}
+
 // phase timers live in shared memory (thread 0 of CTA 0 only): registers are what this kernel is short of
 #define MPH_START() do { if (cta == 0 && tid == 0) ms.tc0 = clock64(); } while (0)
 #define MPH_MARK(i) do { if (cta == 0 && tid == 0) { const long long tc1_ = clock64(); ms.ph[i] += tc1_ - ms.tc0; ms.tc0 = tc1_; } } while (0)
@@ -176,64 +193,35 @@ __device__ __forceinline__ void multi_append(bool keep, uint32_t ck, unsigned lo
 template <bool XGPU>
 __global__ void __launch_bounds__(LEAN_THREADS, 1) ccsim_wave_multi_kernel(const DevParams p, const LeanParams lp, const MultiParams mp) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
-  int32_t *smem_cnt = reinterpret_cast<int32_t *>(smem_raw);
-  const uint32_t cnt_bytes = ((uint32_t)p.smem_cnt_ints * 4u + 15u) & ~15u;
-  uint4 *rec = reinterpret_cast<uint4 *>(smem_raw + cnt_bytes);
   const size_t cp = (size_t)p.chunk_pad;
-  long long *c_acpu = reinterpret_cast<long long *>(smem_raw + cnt_bytes + lp.rec_bytes_total);
-  long long *c_amem = c_acpu + cp, *c_rcpu = c_amem + cp, *c_rmem = c_rcpu + cp, *c_zcpu = c_rmem + cp, *c_zmem = c_zcpu + cp;
-  int32_t *c_apods = reinterpret_cast<int32_t *>(c_zmem + cp);
-  int32_t *c_npods = c_apods + cp;
-  unsigned long long *c_pay = reinterpret_cast<unsigned long long *>(c_npods + cp);   // (chunk_pad is a multiple of 4: 8-byte aligned)
+  const LeanTile t = lean_tile(smem_raw, lp, cp);
+  int32_t *smem_cnt = t.cnt;
+  unsigned long long *c_pay = reinterpret_cast<unsigned long long *>(t.own);   // each node's payload (the 16 bytes after it are not read)
 
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int cta = blockIdx.x;
   const int32_t lo = min(p.n, cta * p.chunk), hi = min(p.n, lo + p.chunk);
   const int32_t cnt_nodes = hi - lo;      // <= LEAN_THREADS (host-checked): one node per thread
-  const int su = lp.stride_u;
   const uint32_t cnt_sa = pin_u32(smem_u32(smem_cnt)), ms_sa = pin_u32(smem_u32(&ms));   // shared bases for the replay's explicit-address accesses
 #define MS_SA(field) (ms_sa + (uint32_t)offsetof(MultiShared, field))
   const int nlists = p.grid;                            // lines of this GPU (node shards: every rank launches the same grid, sized from the largest shard)
   const int tot = nlists * MULTI_M;
 
-  // ---- stage the tile (once): hot AoS records + cold SoA columns (same layout as the lean kernel) ----
-  for (int32_t j = tid; j < cnt_nodes; j += LEAN_THREADS) {
-    const int32_t i = lo + j;
-    const long long ac = p.alloc_cpu[i], am = p.alloc_mem[i], rc = p.req_cpu[i], rm = p.req_mem[i];
-    const int32_t ap = p.alloc_pods[i], np = p.npods[i];
-    unsigned long long *r8 = reinterpret_cast<unsigned long long *>(rec + (size_t)j * su);
-    int32_t *r4 = reinterpret_cast<int32_t *>(r8);
-    r8[0] = p.taint_mask[i];
-    r8[1] = p.static_words > 0 ? p.static_mask[i] : 0ull;
-    r8[2] = (unsigned long long)(ac - rc);
-    r8[3] = (unsigned long long)(am - rm);
-    r4[8] = ap - np;
-    r4[9] = -1;
-    for (int s = 0; s < lp.n_slots; s++)
-      r4[10 + s] = lp.slot_topo[s] >= 0 ? p.topo[lp.slot_topo[s]][i] : p.counters[lp.slot_counter[s]].work[i];
-    c_acpu[j] = ac; c_amem[j] = am; c_rcpu[j] = rc; c_rmem[j] = rm;
-    c_zcpu[j] = p.nz_cpu[i]; c_zmem[j] = p.nz_mem[i];
-    c_apods[j] = ap; c_npods[j] = np;
-    // the node's payload for the candidate exchange: domain id + 1 of every topology slot (static: labels do not change)
-    unsigned long long py = 0ull;
-    for (int s = 0; s < lp.n_slots; s++)
-      if (mp.pay_mask[s]) py |= (unsigned long long)((uint32_t)(r4[10 + s] + 1) & mp.pay_mask[s]) << mp.pay_shift[s];
-    c_pay[j] = py;
-  }
-  for (int k = tid; k < (int)(sizeof(ccsim_template) / 8); k += LEAN_THREADS)
-    reinterpret_cast<unsigned long long *>(&ls.tmpl)[k] = reinterpret_cast<const unsigned long long *>(&p.templates[0])[k];
-  for (int j = 0; j < p.n_counters; j++) {
-    const DevCounter &dc = p.counters[j];
-    if (dc.topo_col < 0) continue;
-    for (int d = tid; d < dc.n_domains; d += LEAN_THREADS) smem_cnt[dc.smem_off + d] = dc.init[d];
-  }
-  if (tid == 0) { ls.aff_total = p.templates[0].aff_total_init; ls.winner = -1; ls.stop = 0; ls.dirty = 1; ms.accepted = 0; ms.dead = 0; ms.stopb = 0; ms.n_gt = 0; ms.ncand = 0; ms.delta = 1u << MULTI_IDX_BITS; ms.force_strict = 0; ms.st_relaxed = 0; ms.st_empty = 0;
+  if (tid == 0) { ms.accepted = 0; ms.dead = 0; ms.stopb = 0; ms.n_gt = 0; ms.ncand = 0; ms.delta = 1u << MULTI_IDX_BITS; ms.force_strict = 0; ms.st_relaxed = 0; ms.st_empty = 0;
                   for (int q = 0; q < LEAN_MAX_TERMS; q++) ms.relax[q] = 0;
                   for (int q = 0; q < 8; q++) ms.ph[q] = 0; ms.tc0 = 0; ms.st_cand = 0; ms.st_overflow = 0; ms.st_rounds = 0;
                   RPROF(for (int q = 0; q < RP_N; q++) ms.rp_cyc[q] = ms.rp_cnt[q] = 0; ms.rp_t = 0;) }
   ms.mult[tid] = 0;
-  __syncthreads();
+  lean_stage(p, lp, t, lo, cnt_nodes);
   for (int c = 0; c < ls.tmpl.n_pts; c++) lean_pts_recount(p, smem_cnt, c);
+  // the node's payload for the candidate exchange: domain id + 1 of every topology slot (static: labels do not change)
+  for (int32_t j = tid; j < cnt_nodes; j += LEAN_THREADS) {
+    const int32_t *r4 = lean_rec4(t, lp, j);
+    unsigned long long py = 0ull;
+    for (int s = 0; s < lp.n_slots; s++)
+      if (mp.pay_mask[s]) py |= (unsigned long long)((uint32_t)(r4[LR_SLOT0 + s] + 1) & mp.pay_mask[s]) << mp.pay_shift[s];
+    c_pay[j] = py;
+  }
 
   long long k = 0, wv = 0;
   uint32_t delta = 1u << MULTI_IDX_BITS;     // bar distance below the best key: starts at one score level
@@ -250,7 +238,7 @@ __global__ void __launch_bounds__(LEAN_THREADS, 1) ccsim_wave_multi_kernel(const
         int g = 0;
         for (int q = 0; q < ls.n_cmp_terms; q++)
           if (ls.terms[q].cnt_off >= 0 && g < MULTI_GT) {
-            const int sl = ls.terms[q].slot - 10;
+            const int sl = ls.terms[q].slot - LR_SLOT0;
             ms.gt_c1[g][0] = ls.terms[q].lim; ms.gt_c1[g][1] = (int32_t)mp.pay_shift[sl]; ms.gt_c1[g][2] = (int32_t)mp.pay_mask[sl]; ms.gt_c1[g][3] = 0;
             ms.gt_commit[g][0] = ls.terms[q].cnt_off; ms.gt_commit[g][1] = 0; ms.gt_commit[g][2] = -1; ms.gt_commit[g][3] = 0;
             for (int j = 0; j < p.n_counters; j++)
@@ -265,7 +253,7 @@ __global__ void __launch_bounds__(LEAN_THREADS, 1) ccsim_wave_multi_kernel(const
         for (int q = 0; q < ls.n_cmp_terms; q++)
           if (ls.terms[q].cnt_off < 0 && ls.terms[q].kind == LT_ANTI)
             for (int j = 0; j < p.n_counters; j++)
-              if (p.counters[j].topo_col < 0 && 10 + lp.counter_slot[j] == ls.terms[q].slot && ls.cinfo[j].inc > 0) su1 = 1;
+              if (p.counters[j].topo_col < 0 && LR_SLOT0 + lp.counter_slot[j] == ls.terms[q].slot && ls.cinfo[j].inc > 0) su1 = 1;
         ms.single_use = su1;
       }
       __syncthreads();
@@ -275,33 +263,20 @@ __global__ void __launch_bounds__(LEAN_THREADS, 1) ccsim_wave_multi_kernel(const
     uint32_t key = 0u;
     if (tid < cnt_nodes) {
       const int32_t j = tid;
-      const uint4 *r = rec + (size_t)j * su;
-      const uint4 u0 = r[0], u1 = r[1], u2 = r[2];
-      const unsigned long long taint0 = ((unsigned long long)u0.y << 32) | u0.x;
-      const unsigned long long static0 = ((unsigned long long)u0.w << 32) | u0.z;
-      const long long free_cpu = (long long)(((unsigned long long)u1.y << 32) | u1.x);
-      const long long free_mem = (long long)(((unsigned long long)u1.w << 32) | u1.z);
-      const int32_t free_pods = (int32_t)u2.x;
-      int32_t sc = (int32_t)u2.y;
-      bool ok = ((taint0 & ls.taint_bad0) | (~static0 & ls.sel0) | (static0 & ls.forbid0)) == 0ull;
-      ok &= (free_cpu >= ls.eq_cpu) & (free_mem >= ls.eq_mem) & (free_pods >= ls.pods_need);
+      const int32_t *r4 = lean_rec4(t, lp, j);
+      const LeanRow w = lean_row(reinterpret_cast<const uint4 *>(r4));
+      int32_t sc = w.score;
+      bool ok = lean_fits(w, lean_fit());
       const int32_t n_cmp = ls.n_cmp_terms;
-      const int32_t *r4 = reinterpret_cast<const int32_t *>(r);
       #pragma unroll 4
       for (int q = 0; q < n_cmp; q++) {
         const LeanTerm lt = ls.terms[q];
-        const int32_t v = r4[lt.slot];
-        const bool local = lt.cnt_off < 0;
-        const int32_t c = local ? v : smem_cnt[lt.cnt_off + (v < 0 ? 0 : v)];
-        const bool has = local | (v >= 0);
+        bool has;
+        const int32_t c = lean_term_count(r4, smem_cnt, lt, has);
         ok &= has ? (c <= lt.lim + ms.relax[q]) : (lt.miss_rejects == 0);     // (relax > 0: closed cells close to reopening publish their nodes as dormant candidates)
       }
       if (ok) {
-        if (sc < 0) {
-          sc = score_node(c_acpu[j], c_amem[j], c_zcpu[j] + ls.tmpl.least_cpu, c_zmem[j] + ls.tmpl.least_mem,
-                          c_rcpu[j] + ls.tmpl.bal_cpu, c_rmem[j] + ls.tmpl.bal_mem, ls.sw);
-          reinterpret_cast<int32_t *>(rec + (size_t)j * su)[9] = sc;
-        }
+        if (sc < 0) sc = lean_rescore(t, lp, j);
         key = ckey(sc, (uint32_t)(p.node_base + lo + j));
       }
     }
@@ -349,22 +324,19 @@ __global__ void __launch_bounds__(LEAN_THREADS, 1) ccsim_wave_multi_kernel(const
         // score again, on the row as it would be after this commit (types.go:409-427). Per-domain terms are re-checked by
         // the replay itself. 0 = the node would not take another clone.
         if (!ms.single_use) {    // (a clone that blocks its own node — hostname anti-affinity — never has a second life)
-        const uint4 *r = rec + (size_t)jj * su;
-        const uint4 u1 = r[1], u2 = r[2];
-        const long long free_cpu = (long long)(((unsigned long long)u1.y << 32) | u1.x) - ls.tmpl.req_cpu;
-        const long long free_mem = (long long)(((unsigned long long)u1.w << 32) | u1.z) - ls.tmpl.req_mem;
-        bool ok2 = (free_cpu >= ls.eq_cpu) & (free_mem >= ls.eq_mem) & ((int32_t)u2.x - 1 >= ls.pods_need);
-        const int32_t *r4 = reinterpret_cast<const int32_t *>(r);
+        const int32_t *r4 = lean_rec4(t, lp, jj);
+        const LeanRow w = lean_row(reinterpret_cast<const uint4 *>(r4));
+        bool ok2 = (w.free_cpu - ls.tmpl.req_cpu >= ls.eq_cpu) & (w.free_mem - ls.tmpl.req_mem >= ls.eq_mem) & (w.free_pods - 1 >= ls.pods_need);
         for (int q = 0; q < ls.n_cmp_terms; q++) {
           const LeanTerm lt = ls.terms[q];
           if (lt.cnt_off >= 0) continue;                       // replicated counters: the replay's business
           int inc = 0;
-          for (int j = 0; j < p.n_counters; j++) if (p.counters[j].topo_col < 0 && 10 + lp.counter_slot[j] == lt.slot) inc = ls.cinfo[j].inc;
+          for (int j = 0; j < p.n_counters; j++) if (p.counters[j].topo_col < 0 && LR_SLOT0 + lp.counter_slot[j] == lt.slot) inc = ls.cinfo[j].inc;
           ok2 &= (r4[lt.slot] + inc <= lt.lim);
         }
         if (ok2) {
-          const int32_t sc2 = score_node(c_acpu[jj], c_amem[jj], c_zcpu[jj] + ls.tmpl.nz_cpu + ls.tmpl.least_cpu, c_zmem[jj] + ls.tmpl.nz_mem + ls.tmpl.least_mem,
-                                         c_rcpu[jj] + ls.tmpl.req_cpu + ls.tmpl.bal_cpu, c_rmem[jj] + ls.tmpl.req_mem + ls.tmpl.bal_mem, ls.sw);
+          const int32_t sc2 = score_node(t.acpu[jj], t.amem[jj], t.zcpu[jj] + ls.tmpl.nz_cpu + ls.tmpl.least_cpu, t.zmem[jj] + ls.tmpl.nz_mem + ls.tmpl.least_mem,
+                                         t.rcpu[jj] + ls.tmpl.req_cpu + ls.tmpl.bal_cpu, t.rmem[jj] + ls.tmpl.req_mem + ls.tmpl.bal_mem, ls.sw);
           pay |= (unsigned long long)(uint32_t)(sc2 + 1) << MULTI_NEXT_SHIFT;
         }
         }
@@ -446,24 +418,13 @@ __global__ void __launch_bounds__(LEAN_THREADS, 1) ccsim_wave_multi_kernel(const
       __syncthreads();                                                  // G2
       C = ms.ncand;
       if (C <= MULTI_CAP || pass == 1) break;
-      // More candidates than the replay holds: raise T to the lowest of 64 equal steps between T and the best key that leaves
-      // <= MULTI_CAP candidates; every CTA sees the same data and decides alike.
       if (tid < MULTI_BINS) ms.hist[tid] = 0u;
       __syncthreads();
       const unsigned long long range = (unsigned long long)(kbest - T) + 1ull;
       #pragma unroll
-      for (int u = 0; u < MULTI_EPT; u++) {
-        const uint32_t ck = (uint32_t)ea[u];
-        if (ck != 0u && ck >= T) atomicAdd(&ms.hist[(unsigned)(((unsigned long long)(ck - T) * MULTI_BINS) / range)], 1u);
-      }
+      for (int u = 0; u < MULTI_EPT; u++) multi_hist_add((uint32_t)ea[u], T, range);
       __syncthreads();
-      int bsel = MULTI_BINS;
-      { unsigned sum = 0; for (int bq = MULTI_BINS - 1; bq >= 0; bq--) { sum += ms.hist[bq]; if (sum > (unsigned)MULTI_CAP) break; bsel = bq; } }
-      T = (bsel >= MULTI_BINS) ? kbest : T + (uint32_t)(((unsigned long long)bsel * range + (MULTI_BINS - 1)) / MULTI_BINS);
-      __syncthreads();
-      if (tid == 0) ms.ncand = 0;
-      if (cta == 0 && tid == 0) ms.st_overflow++;
-      __syncthreads();
+      T = multi_raise_bar(T, kbest, range, cta);
     }
     if (XGPU) {
       // ---- gather, level 2 (node shards): every rank now holds ITS candidates keyed >= its bar T_r (<= MULTI_CAP of them, the same in
@@ -545,18 +506,11 @@ __global__ void __launch_bounds__(LEAN_THREADS, 1) ccsim_wave_multi_kernel(const
         if (tid < MULTI_BINS) ms.hist[tid] = 0u;
         __syncthreads();
         const unsigned long long range = (unsigned long long)(kbest - T) + 1ull;
-        if (lkey != 0u && lkey >= T) atomicAdd(&ms.hist[(unsigned)(((unsigned long long)(lkey - T) * MULTI_BINS) / range)], 1u);
+        multi_hist_add(lkey, T, range);
         #pragma unroll
-        for (int u = 0; u < MULTI_XPT; u++)
-          if (rkey[u] != 0u && rkey[u] >= T) atomicAdd(&ms.hist[(unsigned)(((unsigned long long)(rkey[u] - T) * MULTI_BINS) / range)], 1u);
+        for (int u = 0; u < MULTI_XPT; u++) multi_hist_add(rkey[u], T, range);
         __syncthreads();
-        int bsel = MULTI_BINS;
-        { unsigned sum = 0; for (int bq = MULTI_BINS - 1; bq >= 0; bq--) { sum += ms.hist[bq]; if (sum > (unsigned)MULTI_CAP) break; bsel = bq; } }
-        T = (bsel >= MULTI_BINS) ? kbest : T + (uint32_t)(((unsigned long long)bsel * range + (MULTI_BINS - 1)) / MULTI_BINS);
-        __syncthreads();
-        if (tid == 0) ms.ncand = 0;
-        if (cta == 0 && tid == 0) ms.st_overflow++;
-        __syncthreads();
+        T = multi_raise_bar(T, kbest, range, cta);
       }
       dead = dead || ms.dead != 0;
     }
@@ -848,85 +802,50 @@ __global__ void __launch_bounds__(LEAN_THREADS, 1) ccsim_wave_multi_kernel(const
     // ClusterCapacityBinder.Bind + postBindHook: pod k+i -> node (plugin.go:34-53; simulator.go:297-312). Every CTA knows the
     // whole list; CTA 0 (of every rank: each keeps the whole sequence) records it.
     if (cta == 0 && tid < acc && k + tid < p.pod_cap) p.pod_node[k + tid] = ms.acc_node[tid];
-    // ---- assume -> AssumePod -> NodeInfo.update(+1) (schedule_one.go:967-984, types.go:409-427): the replay warp counted this
-    //      thread's node among the winners (ms.mult). Only this thread reads the row before the next S1. ----
+    // ---- the winners' rows: the replay warp counted this thread's node among the winners (ms.mult). Only this thread reads the
+    //      row before the next S1. ----
     if (tid < cnt_nodes && acc) {
       const int mult = ms.mult[tid];
       if (mult) {
         ms.mult[tid] = 0;
-        const ccsim_template &t = ls.tmpl;
-        const int32_t jw = tid;
-        const long long rc = c_rcpu[jw] + mult * t.req_cpu, rm = c_rmem[jw] + mult * t.req_mem;
-        const int32_t np = c_npods[jw] + mult;
-        c_rcpu[jw] = rc; c_rmem[jw] = rm; c_zcpu[jw] += mult * t.nz_cpu; c_zmem[jw] += mult * t.nz_mem; c_npods[jw] = np;
-        unsigned long long *r8 = reinterpret_cast<unsigned long long *>(rec + (size_t)jw * su);
-        int32_t *r4 = reinterpret_cast<int32_t *>(r8);
-        r8[2] = (unsigned long long)(c_acpu[jw] - rc);
-        r8[3] = (unsigned long long)(c_amem[jw] - rm);
-        r4[8] = c_apods[jw] - np;
-        r4[9] = -1;            // this node's NodeInfo generation changed: its memoised score is stale
-        for (int j = 0; j < p.n_counters; j++) {
-          const CommitInfo ci = ls.cinfo[j];
-          if (ci.inc && ci.local) r4[10 + lp.counter_slot[j]] += mult * ci.inc;   // node-local counters (written back when the run ends)
-        }
+        lean_commit_row(p, lp, t, tid, mult, -1);     // this node's NodeInfo generation changed: its memoised score is stale
       }
     }
     MPH_MARK(5);
     k += acc;
     delta = ms.delta;
     if (ls.stop) break;
-    for (int c = 0; c < ls.tmpl.n_pts; c++)
-      if (!ls.tmpl.pts[c].min_zero && (ls.ptsnum[c] <= 0 || (p.debug_flags & 2)) && p.counters[ls.tmpl.pts[c].counter].n_present > 0) lean_pts_recount(p, smem_cnt, c);
+    lean_pts_after_wave(p, smem_cnt, p.debug_flags & 2);
     wtag = (wtag == 4095u) ? 1u : wtag + 1u;
     tag = (p.epoch << 12) | wtag;
   }
 
-  // ---- write the tile back: the global columns are the snapshot-after-run (terminal diagnosis, ccsim_node_counts) ----
-  for (int32_t j = tid; j < cnt_nodes; j += LEAN_THREADS) {
-    const int32_t i = lo + j;
-    p.req_cpu[i] = c_rcpu[j]; p.req_mem[i] = c_rmem[j]; p.nz_cpu[i] = c_zcpu[j]; p.nz_mem[i] = c_zmem[j]; p.npods[i] = c_npods[j];
-    const int32_t *r4 = reinterpret_cast<const int32_t *>(rec + (size_t)j * su);
-    for (int sl = 0; sl < lp.n_slots; sl++) if (lp.slot_topo[sl] < 0) p.counters[lp.slot_counter[sl]].work[i] = r4[10 + sl];
-  }
-  if (cta == 0) {
-    for (int j = 0; j < p.n_counters; j++) {
-      const DevCounter &dc = p.counters[j];
-      if (dc.topo_col < 0) continue;
-      for (int d = tid; d < dc.n_domains; d += LEAN_THREADS) p.final_cnt[p.final_off[j] + d] = smem_cnt[dc.smem_off + d];
-    }
-    if (tid == 0) {
-      DevOut *o = p.out;
-      o->placed = k;
-      o->stop_code = limit_hit ? CCSIM_STOP_LIMIT_REACHED : CCSIM_STOP_UNSCHEDULABLE;
-      o->error = (ls.stop == 3) ? 1 : 0;
-      o->waves = limit_hit ? wv : wv + 1;
-      o->evals = o->waves * (long long)p.n;
-      o->examined = o->evals;
-      for (int c = 0; c < CCSIM_MAX_PTS; c++) o->ptsmin[c] = ls.ptsmin[c];
-      o->aff_total = ls.aff_total;
-      for (int q = 0; q < 8; q++) o->phase_cycles[q] = ms.ph[q];
-      o->stat[0] = ms.st_cand; o->stat[1] = ms.st_overflow; o->stat[2] = ms.st_rounds;
-      if (p.debug_flags & 8u)
-        printf("multi-commit replay: waves %lld rounds %lld look-ahead waves %d (without a placement: %d) | cycles: replay %lld set-up %lld, per round %.0f\n",
-               limit_hit ? wv : wv + 1, ms.st_rounds, ms.st_relaxed, ms.st_empty, ms.ph[4], ms.ph[6],
-               (double)(ms.ph[4] - ms.ph[6]) / (double)(ms.st_rounds > 0 ? ms.st_rounds : 1));
+  if (DevOut *o = lean_finish(p, lp, t, lo, cnt_nodes, k, limit_hit)) {
+    o->waves = limit_hit ? wv : wv + 1;
+    o->evals = o->waves * (long long)p.n;
+    o->examined = o->evals;
+    for (int q = 0; q < 8; q++) o->phase_cycles[q] = ms.ph[q];
+    o->stat[0] = ms.st_cand; o->stat[1] = ms.st_overflow; o->stat[2] = ms.st_rounds;
+    if (p.debug_flags & 8u)
+      printf("multi-commit replay: waves %lld rounds %lld look-ahead waves %d (without a placement: %d) | cycles: replay %lld set-up %lld, per round %.0f\n",
+             limit_hit ? wv : wv + 1, ms.st_rounds, ms.st_relaxed, ms.st_empty, ms.ph[4], ms.ph[6],
+             (double)(ms.ph[4] - ms.ph[6]) / (double)(ms.st_rounds > 0 ? ms.st_rounds : 1));
 #ifdef MULTI_ROUND_PROFILE
-      {
-        const double w = (double)(limit_hit ? wv : wv + 1), nr = (double)(ms.st_rounds > 0 ? ms.st_rounds : 1);
-        printf("round profile (CTA 0): waves %.0f rounds %lld | replay %.0f cycles/wave, set-up %.0f\n", w, ms.st_rounds, ms.ph[4] / w, ms.ph[6] / w);
-        printf("round profile: common round %lld events, %.0f cycles/round, %.0f cycles/wave\n", ms.rp_cnt[RP_ROUND], ms.rp_cyc[RP_ROUND] / nr, ms.rp_cyc[RP_ROUND] / w);
-        printf("round profile: wake-up rebuilds %lld, %.0f cycles each, %.0f cycles/wave\n", ms.rp_cnt[RP_REBUILD],
-               ms.rp_cyc[RP_REBUILD] / (double)(ms.rp_cnt[RP_REBUILD] > 0 ? ms.rp_cnt[RP_REBUILD] : 1), ms.rp_cyc[RP_REBUILD] / w);
-        printf("round profile: set-up: candidate load %.0f cycles/wave\n", ms.rp_cyc[RP_LOAD] / w);
-        printf("round profile: after the loop %lld waves, %.0f cycles/wave (hand-off %.0f, look-ahead decision %.0f)\n", ms.rp_cnt[RP_AFTER],
-               ms.rp_cyc[RP_AFTER] / w, ms.rp_cyc[RP_HANDOFF] / w, ms.rp_cyc[RP_DECIDE] / w);
-        printf("round profile: rounds with a non-zero kill mask %lld\n", ms.rp_cnt[RP_KILL]);
-        for (int q = 0; q < MULTI_GT; q++)
-          if (ms.rp_cnt[RP_MINMOVE + q])
-            printf("round profile: term %d minimum moves %lld, %.0f cycles each, %.0f cycles/wave\n", q, ms.rp_cnt[RP_MINMOVE + q],
-                   ms.rp_cyc[RP_MINMOVE + q] / (double)ms.rp_cnt[RP_MINMOVE + q], ms.rp_cyc[RP_MINMOVE + q] / w);
-      }
-#endif
+    {
+      const double w = (double)(limit_hit ? wv : wv + 1), nr = (double)(ms.st_rounds > 0 ? ms.st_rounds : 1);
+      printf("round profile (CTA 0): waves %.0f rounds %lld | replay %.0f cycles/wave, set-up %.0f\n", w, ms.st_rounds, ms.ph[4] / w, ms.ph[6] / w);
+      printf("round profile: common round %lld events, %.0f cycles/round, %.0f cycles/wave\n", ms.rp_cnt[RP_ROUND], ms.rp_cyc[RP_ROUND] / nr, ms.rp_cyc[RP_ROUND] / w);
+      printf("round profile: wake-up rebuilds %lld, %.0f cycles each, %.0f cycles/wave\n", ms.rp_cnt[RP_REBUILD],
+             ms.rp_cyc[RP_REBUILD] / (double)(ms.rp_cnt[RP_REBUILD] > 0 ? ms.rp_cnt[RP_REBUILD] : 1), ms.rp_cyc[RP_REBUILD] / w);
+      printf("round profile: set-up: candidate load %.0f cycles/wave\n", ms.rp_cyc[RP_LOAD] / w);
+      printf("round profile: after the loop %lld waves, %.0f cycles/wave (hand-off %.0f, look-ahead decision %.0f)\n", ms.rp_cnt[RP_AFTER],
+             ms.rp_cyc[RP_AFTER] / w, ms.rp_cyc[RP_HANDOFF] / w, ms.rp_cyc[RP_DECIDE] / w);
+      printf("round profile: rounds with a non-zero kill mask %lld\n", ms.rp_cnt[RP_KILL]);
+      for (int q = 0; q < MULTI_GT; q++)
+        if (ms.rp_cnt[RP_MINMOVE + q])
+          printf("round profile: term %d minimum moves %lld, %.0f cycles each, %.0f cycles/wave\n", q, ms.rp_cnt[RP_MINMOVE + q],
+                 ms.rp_cyc[RP_MINMOVE + q] / (double)ms.rp_cnt[RP_MINMOVE + q], ms.rp_cyc[RP_MINMOVE + q] / w);
     }
+#endif
   }
 }
