@@ -771,6 +771,12 @@ struct ccsim_handle {
   ccsim_template *d_templates = nullptr;
   DevCounter counters[CCSIM_MAX_COUNTERS];
   int32_t *d_final_cnt = nullptr; int32_t final_off[CCSIM_MAX_COUNTERS] = {}; int32_t final_total = 0;
+  // int32 range of the counters (run_prepare): free pod slots of every node and of every domain of each topology column over the
+  // whole cluster (ccsim_load_nodes), and per counter the most placements after which all its domains are still exact
+  // (ccsim_set_templates), with NodeResourcesFit bounding each domain by its slots (lim_fit) or not (lim_any)
+  std::vector<int32_t> node_slots;
+  std::vector<int64_t> dom_slots[CCSIM_MAX_TOPO_COLS];
+  struct CounterRange { int64_t lim_fit, lim_any; int32_t dom_fit, dom_any, init_fit, init_any; } cnt_range[CCSIM_MAX_COUNTERS];
   int32_t smem_cnt_ints = 0;
   // run state
   int grid = 0;
@@ -1002,6 +1008,16 @@ extern "C" int ccsim_load_nodes(ccsim_handle *h, const ccsim_nodes *nd) {
     if (pc > maxpop) maxpop = pc;
   }
   h->pod_bound = bound; h->max_prefer_pop = maxpop;
+  h->node_slots.assign(N, 0);
+  for (int32_t i = 0; i < N; i++) h->node_slots[i] = std::max<int32_t>(0, nd->alloc_pods[i] - nd->npods[i]);
+  for (int c = 0; c < CCSIM_MAX_TOPO_COLS; c++) h->dom_slots[c].clear();
+  for (int c = 0; c < nd->n_topo_cols; c++)
+    for (int32_t i = 0; i < N; i++) {
+      const int32_t d = nd->topo[c][i];
+      if (d < 0) continue;
+      if ((size_t)d >= h->dom_slots[c].size()) h->dom_slots[c].resize((size_t)d + 1, 0);
+      h->dom_slots[c][d] += h->node_slots[i];
+    }
   h->taint_or0 = 0;
   for (int32_t i = 0; i < N; i++) h->taint_or0 |= nd->taint_mask[i];
   CK(cudaStreamSynchronize(h->stream));
@@ -1094,6 +1110,21 @@ extern "C" int ccsim_set_templates(ccsim_handle *h, int32_t n_templates, const c
     d.topo_col = c.topo_col; d.inc = c.inc; d.n_present = c.n_present; d.is_aff = 0; d.smem_off = -1; d.work = nullptr; d.elig_bit = c.elig_bit; d.pad = 0;
     for (int a = 0; a < templates[0].n_aff; a++) if (templates[0].aff_counter[a] == j) d.is_aff = 1;
     if (c.topo_col >= nd.n_topo_cols) return fail(h, CCSIM_EINVAL, "counter %d: topo_col", j);
+    {
+      // domain d stays exact for m placements into it while |init_d| + m * |inc| <= INT32_MAX, i.e. m <= room_d; it receives at
+      // most min(placements, its free slots) of them while NodeResourcesFit filters, at most `placements` otherwise
+      auto &r = h->cnt_range[j];
+      r.lim_fit = r.lim_any = INT64_MAX; r.dom_fit = r.dom_any = -1; r.init_fit = r.init_any = 0;
+      const int64_t inc = std::llabs((long long)c.inc);
+      const bool local = c.topo_col < 0;
+      for (int32_t d = 0; inc > 0 && d < c.n_domains; d++) {
+        const int64_t room = std::max<int64_t>(0, ((int64_t)INT32_MAX - std::llabs((long long)c.init[d])) / inc);
+        const int64_t slots = local ? (d < (int32_t)h->node_slots.size() ? h->node_slots[d] : 0)
+                                    : ((size_t)d < h->dom_slots[c.topo_col].size() ? h->dom_slots[c.topo_col][d] : 0);
+        if (room < r.lim_any) { r.lim_any = room; r.dom_any = d; r.init_any = c.init[d]; }
+        if (slots > room && room < r.lim_fit) { r.lim_fit = room; r.dom_fit = d; r.init_fit = c.init[d]; }
+      }
+    }
     if (c.topo_col < 0) {
       // node-local: init is a whole-cluster column; keep this shard's slice
       if (c.n_domains != h->n_global) return fail(h, CCSIM_EINVAL, "counter %d: node-local counter needs n_domains == n_nodes", j);
@@ -1186,7 +1217,25 @@ static int run_prepare(ccsim_handle *h, int64_t max_pods) {
     for (const ccsim_template &T : h->h_templates)
       if (!(T.filter_enable & CCSIM_PL_FIT))
         return fail(h, CCSIM_EUNSUPPORTED, "NodeResourcesFit is disabled for a template: the run is unbounded, --max-limit is required");
-  if (max_pods > 0 && (max_pods < cap || [&] { for (const ccsim_template &T : h->h_templates) if (!(T.filter_enable & CCSIM_PL_FIT)) return true; return false; }())) cap = max_pods;
+  const bool fit_off = [&] { for (const ccsim_template &T : h->h_templates) if (!(T.filter_enable & CCSIM_PL_FIT)) return true; return false; }();
+  if (max_pods > 0 && (max_pods < cap || fit_off)) cap = max_pods;
+  // Counters are int32 here and in the oracle; the reference counts in int64 (podtopologyspread/scoring.go,
+  // interpodaffinity/scoring.go). A counter that could leave int32 during the run is refused, never left to wrap: a domain that
+  // receives m placements holds init + m' * inc with m' <= m, so |init| + m * |inc| <= INT32_MAX keeps every value exact, and m is
+  // at most min(placements, the domain's free pod slots) while NodeResourcesFit filters.
+  int64_t placements = h->pod_bound;
+  if (max_pods > 0 && (max_pods < placements || fit_off)) placements = max_pods;
+  for (int j = 0; j < h->n_counters; j++) {
+    const auto &r = h->cnt_range[j];
+    const int64_t lim = fit_off ? r.lim_any : r.lim_fit;
+    const int32_t d = fit_off ? r.dom_any : r.dom_fit;
+    if (placements > lim) {
+      const int32_t tc = h->counters[j].topo_col;
+      const int64_t m = fit_off ? placements : std::min(placements, tc < 0 ? (int64_t)h->node_slots[d] : h->dom_slots[tc][d]);
+      return fail(h, CCSIM_EUNSUPPORTED, "counter %d, domain %d: |initial count| %lld + %lld placements x |increment| %d can leave int32",
+                  j, d, std::llabs((long long)(fit_off ? r.init_any : r.init_fit)), (long long)m, std::abs(h->counters[j].inc));
+    }
+  }
   if (cap > h->pod_cap) {
     if (h->d_pod_node) cudaFreeAsync(h->d_pod_node, h->stream);
     h->d_pod_node = nullptr; h->pod_cap = 0;

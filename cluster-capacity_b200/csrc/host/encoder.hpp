@@ -661,7 +661,7 @@ class Encoder {
       }
       int colidx = (int)e.topo.size();
       e.topo.push_back(col);
-      std::vector<int32_t> init(counts.begin(), counts.end());
+      std::vector<int32_t> init = int32_counts(counts, tc.topology_key);
       const bool self = hard_sel[c].matches(t_.labels);
       // an Everything selector (labelSelector: {}) self-matches (filtering.go:341-344) but is never COUNTED: countPodsMatchSelector
       // returns 0 for selector.Empty() (common.go:144-147), so committed clones do not raise the domain counts either
@@ -686,7 +686,7 @@ class Encoder {
       return out;
     };
     std::vector<AffinityTerm> aff = merged(t_.aff_required), anti = merged(t_.anti_required);
-    auto ipa_counter = [&](const std::string &key, const std::function<int(const Pod &)> &weight, int inc, int32_t &out_idx) {
+    auto ipa_counter = [&](const std::string &key, const std::function<int64_t(const Pod &)> &weight, int inc, int32_t &out_idx) {
       // one counter per topology key; node-local when every node has the key with a unique value
       FlatIndex dom_id; std::vector<int32_t> col(n, -1); std::vector<int64_t> counts;
       std::vector<const std::string *> value(n, nullptr);
@@ -716,12 +716,12 @@ class Encoder {
       tick("  ipa/weights");
       for (int i = 0; i < n; i++) if (col[i] >= 0) counts[col[i]] += per_node[i];
       if (unique && n > 0) {
-        std::vector<int32_t> init(per_node.begin(), per_node.end());
+        std::vector<int32_t> init = int32_counts(per_node, key);
         add_counter(e, -1, init, n, inc);
       } else {
         int colidx = (int)e.topo.size();
         e.topo.push_back(col);
-        std::vector<int32_t> init(counts.begin(), counts.end());
+        std::vector<int32_t> init = int32_counts(counts, key);
         add_counter(e, colidx, init, (int)init.size(), inc);
       }
       out_idx = (int32_t)e.counters.size() - 1;
@@ -835,7 +835,7 @@ class Encoder {
             if (!require_all && missing && explicit_empty) throw Unsupported("a topology label with an empty value next to nodes without the label (PodTopologySpread score)");
             int colidx = (int)e.topo.size();
             e.topo.push_back(col);
-            std::vector<int32_t> init(counts.begin(), counts.end());
+            std::vector<int32_t> init = int32_counts(counts, sc.key);
             add_counter(e, colidx, init, (int)init.size(), inc);
             if (!everyone && inc) e.counters.back().elig_bit = new_bit([&, counted](int i) { return counted[i] != 0; });
           }
@@ -870,8 +870,9 @@ class Encoder {
       else for (int i = 0; i < n; i++) for (auto *p : pods_on_[i]) visit(p);
       if (keys.size() > CCSIM_MAX_IPA) throw Unsupported("more than 8 topology keys in pod (anti-)affinity scoring terms");
       for (size_t k = 0; k < keys.size(); k++) {
-        auto w = [&](const Pod &p) { auto it = per_pod.find(&p); if (it == per_pod.end()) return 0; auto jt = it->second.find(keys[k]); return jt == it->second.end() ? 0 : (int)jt->second; };
-        ipa_counter(keys[k], w, clone.count(keys[k]) ? (int)clone[keys[k]] : 0, T.ipa_score_counter[k]);
+        auto w = [&](const Pod &p) -> int64_t { auto it = per_pod.find(&p); if (it == per_pod.end()) return 0; auto jt = it->second.find(keys[k]); return jt == it->second.end() ? 0 : jt->second; };
+        const int64_t inc = clone.count(keys[k]) ? clone[keys[k]] : 0;
+        ipa_counter(keys[k], w, int32_counts({inc}, keys[k])[0], T.ipa_score_counter[k]);
       }
       T.n_ipa_score = (int32_t)keys.size();
     }
@@ -976,6 +977,15 @@ class Encoder {
       break;
     }
     return sel;
+  }
+
+  // Per-domain counts are summed in int64 like the reference's and held as int32 by the engine: a sum outside int32 is refused,
+  // naming the topology key, instead of being narrowed.
+  static std::vector<int32_t> int32_counts(const std::vector<int64_t> &v, const std::string &key) {
+    for (int64_t x : v)
+      if (x < INT32_MIN || x > INT32_MAX)
+        throw Unsupported("topology key \"" + key + "\": a per-domain count of " + std::to_string(x) + " is outside int32");
+    return std::vector<int32_t>(v.begin(), v.end());
   }
 
   static void add_counter(Encoded &e, int topo_col, const std::vector<int32_t> &init, int n_present, int inc) {

@@ -12,7 +12,9 @@
 //   PodRequests / AggregateContainerRequests  k8s.io/component-helpers/resource/helpers.go:144-251
 #pragma once
 #include <mutex>
+#include <cstdint>
 #include <cstdlib>
+#include <stdexcept>
 #include <new>
 #include <algorithm>
 #include <map>
@@ -276,6 +278,14 @@ struct Pod {
   std::map<std::string, ResourceList> status_resources, status_allocated;   // containerStatuses[*].resources.requests / allocatedResources
   bool resize_infeasible = false;
 
+  // WeightedPodAffinityTerm.weight and PreferredSchedulingTerm.weight are int32 in the API: a value outside int32 does not
+  // decode there, and is refused here instead of being truncated
+  static int term_weight(const Json &w) {
+    const int64_t v = w.i64(0);
+    if (v < INT32_MIN || v > INT32_MAX) throw std::runtime_error("a preferred term's weight " + std::to_string(v) + " is outside int32");
+    return (int)v;
+  }
+
   static std::vector<AffinityTerm> parse_terms(const Json &arr, const std::string &pod_ns, bool weighted) {
     std::vector<AffinityTerm> out;
     if (!arr.is_array()) return out;
@@ -289,7 +299,7 @@ struct Pod {
       if ((!nss.is_array() || nss.arr.empty()) && !nsel.is_object()) t.namespaces.insert(pod_ns);
       else if (nss.is_array()) for (auto &x : nss.arr) t.namespaces.insert(x.str());
       t.ns_selector = Selector::from_label_selector(nsel);
-      if (weighted) t.weight = (int)e0.at("weight").i64(0);
+      if (weighted) t.weight = term_weight(e0.at("weight"));
       out.push_back(t);
     }
     return out;
@@ -377,7 +387,7 @@ struct Pod {
             for (auto &v : e.at("values").arr) r.values.push_back(v.str());
             nt.match_fields.push_back(r);
           }
-        const int w = (int)pt.at("weight").i64(0);
+        const int w = term_weight(pt.at("weight"));
         if (w != 0 && !nt.empty()) p.node_affinity_preferred.push_back({w, nt});
       }
     if (sp.at("tolerations").is_array())

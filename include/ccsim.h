@@ -291,7 +291,9 @@ int  ccsim_set_templates(ccsim_handle *h, int32_t n_templates, const ccsim_templ
                          int32_t n_counters, const ccsim_counter *counters);
 
 /* Run: place pods k = 0,1,2,... (template k % n_templates) until one does not fit or max_pods (>0) are placed.
- * Restores the loaded snapshot first, so it can be called repeatedly. Blocking. */
+ * Restores the loaded snapshot first, so it can be called repeatedly. Blocking. Refuses (CCSIM_EUNSUPPORTED, before any launch) a
+ * counter with a domain whose |init| + m * |inc| could leave int32, m = min(max_pods, the free pod slots of the cluster, those of
+ * the domain's nodes); without the slot bounds when a template disables NodeResourcesFit. */
 int  ccsim_run(ccsim_handle *h, int64_t max_pods, ccsim_result *out);
 /* Optional: everything ccsim_run(h, max_pods) does BEFORE the wave kernel starts (buffers, restoring the snapshot, engine choice),
  * synchronously. A host that drives several ranks from one process calls it on every handle, then starts the ccsim_run calls

@@ -411,6 +411,33 @@ int ccsim_oracle_run_ex(const ccsim_nodes *nd, int32_t n_templates, const ccsim_
         T->least_w_cpu < 1 || T->least_w_cpu > 100 || T->least_w_mem < 1 || T->least_w_mem > 100)
       return CCSIM_EUNSUPPORTED;
   }
+  /* The per-domain counters are int32 (s.cnt), the reference's counts int64 (PL:podtopologyspread/scoring.go:192-224,
+     PL:interpodaffinity/scoring.go:236-256): refuse a counter that could leave int32 within the run, as the engine does
+     (ccsim_prepare). A domain receives at most min(placements, its free pod slots) commits while NodeResourcesFit filters
+     (fit.go:567-576), at most `placements` otherwise; placements = min(max_pods, the cluster's free pod slots). */
+  {
+    int64_t bound = 0;
+    int fit_off = 0;
+    for (int32_t i = 0; i < n; i++) if (nd->alloc_pods[i] > nd->npods[i]) bound += (int64_t)nd->alloc_pods[i] - nd->npods[i];
+    for (int t = 0; t < n_templates; t++) if (!(tmpl[t].filter_enable & CCSIM_PL_FIT)) fit_off = 1;
+    if (max_pods > 0 && (max_pods < bound || fit_off)) bound = max_pods;
+    for (int j = 0; j < n_counters; j++) {
+      const int64_t inc = llabs((long long)ctr[j].inc);
+      if (inc == 0 || ctr[j].n_domains <= 0) continue;
+      int64_t *slots = (int64_t*)calloc((size_t)ctr[j].n_domains, 8);
+      for (int32_t i = 0; i < n; i++) {
+        const int32_t d = ctr[j].topo_col < 0 ? i : nd->topo[ctr[j].topo_col][i];
+        if (d >= 0 && d < ctr[j].n_domains && nd->alloc_pods[i] > nd->npods[i]) slots[d] += (int64_t)nd->alloc_pods[i] - nd->npods[i];
+      }
+      int refuse = 0;
+      for (int32_t d = 0; d < ctr[j].n_domains && !refuse; d++) {
+        const int64_t m = fit_off || slots[d] > bound ? bound : slots[d];
+        if (m > 0 && llabs((long long)ctr[j].init[d]) + m * inc > INT32_MAX) refuse = 1;
+      }
+      free(slots);
+      if (refuse) return CCSIM_EUNSUPPORTED;
+    }
+  }
 #ifdef _OPENMP
   if (threads > 0) omp_set_num_threads(threads);
 #else
