@@ -2,6 +2,7 @@
 import ctypes as C
 import importlib
 import random
+import threading
 
 import numpy as np
 
@@ -95,6 +96,91 @@ def persistent_grid(n, sm_count, world=1):
     """CTAs per rank of the persistent wave kernels: sized from the largest node shard."""
     shard = -(-n // world)
     return max(1, min(sm_count, MAX_GRID, -(-shard // GRID_NODES)))
+
+
+# ---- node-sharded ranks on one device -------------------------------------------------------------------------------
+def sharded_engines(snap, tmpl, ctr, world, kind):
+    """`world` handles of this process on device 0 (rank r = the r-th), loaded and wired to each other by pointer
+    (Engine.connect_local): the same in-kernel exchange as across GPUs, only the stores do not cross NVLink."""
+    engine = importlib.import_module("cluster-capacity_b200.engine")
+    engs = [engine.Engine(device=0, engine=kind, rank=r, world=world) for r in range(world)]
+    try:
+        for e in engs:
+            e.load_nodes(snap)
+            e.set_templates(tmpl, ctr)
+        engine.Engine.connect_local(engs)
+    except Exception:
+        for e in engs:
+            e.close()
+        raise
+    return engs
+
+
+def run_sharded_once(engs, lim):
+    """One run of every rank: all ranks past their allocations (prepare) before any rank's kernel starts waiting for its peers,
+    then the runs side by side, one host thread per rank. Returns the ranks' RunResults."""
+    world = len(engs)
+    res, errs = [None] * world, []
+    for e in engs:
+        e.prepare(lim)
+
+    def work(r):
+        try:
+            res[r] = engs[r].run(lim)
+        except Exception as ex:       # noqa: BLE001
+            errs.append(ex)
+    th = [threading.Thread(target=work, args=(r,)) for r in range(world)]
+    for t in th:
+        t.start()
+    for t in th:
+        t.join(timeout=120)
+    assert not errs, errs
+    assert all(r is not None for r in res), "a rank did not finish"
+    return res
+
+
+def run_sharded(snap, tmpl, ctr, limit, world, kind, runs):
+    """The ranks of a node-sharded run as handles of this process on device 0, one run per entry of `runs` (its max_pods) on the
+    same handles. Returns [(per-rank RunResults, per-rank run_stats)] per run."""
+    engs = sharded_engines(snap, tmpl, ctr, world, kind)
+    out = []
+    for lim in runs:
+        res = run_sharded_once(engs, lim)
+        out.append((res, [e.run_stats() for e in engs]))
+    for e in engs:
+        e.close()
+    return out
+
+
+def sharded_kernels(snap, tmpl, ctr, world, max_pods=0, kind=0):
+    """The kernel each rank of a node-sharded run would launch, from ccsim_prepare alone (ranks of this process on device 0,
+    connected; nothing is launched)."""
+    engs = sharded_engines(snap, tmpl, ctr, world, kind)
+    try:
+        for e in engs:
+            e.prepare(max_pods)
+        return [kernel_name(e) for e in engs]
+    finally:
+        for e in engs:
+            e.close()
+
+
+def largest_sharded_n(make, kernel, lo, hi, world, max_pods=0):
+    """largest_n for a node-sharded run: the largest N in [lo, hi) for which every rank of make(N) still runs `kernel`."""
+    def on(n):
+        try:
+            return set(sharded_kernels(*make(n), world, max_pods=max_pods)) == {kernel}
+        except RuntimeError:          # EngineError: the configuration refuses the workload
+            return False
+    assert on(lo), (kernel, lo)
+    assert not on(hi), (kernel, hi)
+    while hi - lo > 1:
+        mid = (lo + hi) // 2
+        if on(mid):
+            lo = mid
+        else:
+            hi = mid
+    return lo
 
 
 def multi_eligible(snap, tmpl, ctr, sm_count):

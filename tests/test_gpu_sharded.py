@@ -14,8 +14,9 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 pytestmark = pytest.mark.gpu
 
 
-def _worker(rank, world, port, which, q):
+def _worker(rank, world, port, which, q, n=0):
     sys.path.insert(0, ROOT)
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
     os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port))
     dist.init_process_group("gloo", rank=rank, world_size=world)
     synth = importlib.import_module("cluster-capacity_b200.synth")
@@ -31,6 +32,12 @@ def _worker(rank, world, port, which, q):
     elif which == "c5":            # several node-local templates: the streaming (TMA) engine over node shards
         snap, tmpl, ctr = synth.c5(n=300_001, n_templates=9)
         limit = 1500
+    elif which == "ext":          # the generic kernel: extended resource, ephemeral storage and hostPorts, resident tiles
+        snap, tmpl, ctr = importlib.import_module("test_gpu_sharded_edges").generic_ext_ports(200_001)
+        limit = 3000
+    elif which == "generic_streamed":     # the generic kernel with each rank's tile streamed from global memory
+        snap, tmpl, ctr = importlib.import_module("test_gpu_sharded_edges").generic_streamed(n)
+        limit = 300
     elif which == "c4_wide":      # enough nodes per shard for full grids: the multi-commit replay sees 2 x grid candidate lists
         snap, tmpl, ctr = synth.c4(n=120_001, n_existing=200_000, zones=32, racks=1024, regions=8)
         limit = 3000
@@ -68,19 +75,38 @@ def _worker(rank, world, port, which, q):
                 ok &= eng.run_stats()["engine"] == "multi-commit" and (w.placed < 100 or res.waves * 2 < w.waves)
             if which == "c5":
                 ok &= eng.run_stats()["engine"].startswith("streaming")
+            if which in KERNEL:
+                if eng.run_stats()["kernel"] != KERNEL[which]:
+                    why.append("engine %d run %d: kernel %s" % (kind, it, eng.run_stats()["kernel"]))
+                ok &= eng.run_stats()["kernel"] == KERNEL[which]
         eng.close()
     q.put((rank, bool(ok), int(res.placed), why))
     dist.destroy_process_group()
 
 
-@pytest.mark.parametrize("which", ["c3", "c4", "c4_wide", "spread", "c5"])
+KERNEL = {"ext": "wave<true>", "generic_streamed": "wave<false>"}     # the instantiation every rank must run
+
+
+@pytest.mark.parametrize("which", ["c3", "c4", "c4_wide", "spread", "c5", "ext", "generic_streamed"])
 def test_two_gpu_sharded_matches_oracle(built, which):
+    """generic_streamed: the smallest cluster whose shards no longer fit the generic kernel's resident tile, found by bisection over
+    ccsim_prepare with two connected ranks of this process (nothing is launched). Only this test reaches wave<false> over shards:
+    a streamed tile needs a full grid per rank, and two full grids do not fit on one device at once."""
     if torch.cuda.device_count() < 2:
         pytest.skip("needs 2 GPUs")
+    n = 0
+    if which == "generic_streamed":
+        sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
+        import helpers
+        import test_gpu_sharded_edges as edges
+        n = helpers.largest_sharded_n(edges.generic_streamed, "wave<true>", 100_000, 2_000_000, 2, max_pods=300) + 1
+        n += n % 2          # at odd N the last shard is one node shorter and may stay resident: an even N streams on both ranks
+        assert helpers.sharded_kernels(*edges.generic_streamed(n), 2, max_pods=300) == ["wave<false>"] * 2
+        print("\n  first sharded wave<false>: N = %d" % n, end="")
     ctx = mp.get_context("spawn")
     q = ctx.Queue()
     port = 29700 + os.getpid() % 1500
-    procs = [ctx.Process(target=_worker, args=(r, 2, port, which, q)) for r in range(2)]
+    procs = [ctx.Process(target=_worker, args=(r, 2, port, which, q, n)) for r in range(2)]
     for p in procs:
         p.start()
     out = [q.get(timeout=300) for _ in procs]

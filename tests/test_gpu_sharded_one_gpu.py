@@ -4,49 +4,18 @@ streams (small clusters: every rank needs only a few SMs), started from one host
 as across GPUs — candidate lines of every CTA into every rank's buffer (multi-commit), winner words (lean, streaming) — only
 the stores do not cross NVLink. Results must equal the oracle's, like tests/test_gpu_sharded.py on a multi-GPU box."""
 import importlib
-import threading
 
 import numpy as np
 import pytest
 
 import helpers
+from helpers import run_sharded
 
 abi = importlib.import_module("cluster-capacity_b200._abi")
 synth = importlib.import_module("cluster-capacity_b200.synth")
 from oracle import binding as oracle  # noqa: E402
 
 pytestmark = pytest.mark.gpu
-
-
-def run_sharded(snap, tmpl, ctr, limit, world, kind, runs):
-    engine = importlib.import_module("cluster-capacity_b200.engine")
-    engs = [engine.Engine(device=0, engine=kind, rank=r, world=world) for r in range(world)]
-    for e in engs:
-        e.load_nodes(snap)
-        e.set_templates(tmpl, ctr)
-    engine.Engine.connect_local(engs)
-    out = []
-    for lim in runs:
-        res, errs = [None] * world, []
-        for e in engs:              # every rank past its allocations before any rank's kernel starts waiting for its peers
-            e.prepare(lim)
-
-        def work(r):
-            try:
-                res[r] = engs[r].run(lim)
-            except Exception as ex:       # noqa: BLE001
-                errs.append(ex)
-        th = [threading.Thread(target=work, args=(r,)) for r in range(world)]
-        for t in th:
-            t.start()
-        for t in th:
-            t.join(timeout=120)
-        assert not errs, errs
-        assert all(r is not None for r in res), "a rank did not finish"
-        out.append((res, [e.run_stats() for e in engs]))
-    for e in engs:
-        e.close()
-    return out
 
 
 CASES = {

@@ -585,11 +585,10 @@ def test_trajectory_ladder(built, sm_count, inst):
 @pytest.mark.gpu
 def test_multi_sharded_ladder(built, sm_count):
     """The multi-commit ladder over two node shards of this one device (multi<true>)."""
-    import test_gpu_sharded_one_gpu as sh
     for kind in ("one", "trajectory"):
         snap, tmpl, ctr = ladder(kind, "multi<false>")
         want = _check_against_model(snap, tmpl, ctr)
-        (res, stats), = sh.run_sharded(snap, tmpl, ctr, 0, 2, AUTO, [0])
+        (res, stats), = helpers.run_sharded(snap, tmpl, ctr, 0, 2, AUTO, [0])
         print("\n  %s: %s" % (kind, [s["kernel"] for s in stats]), end="")
         assert all(s["kernel"] == "multi<true>" for s in stats), stats
         for r in res:
