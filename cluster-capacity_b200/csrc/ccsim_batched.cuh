@@ -1,6 +1,6 @@
 // ccsim_batched.cuh — batched tie-run waves: many commits per wave, same placement sequence as the sequential loop.
 //
-// Eligibility (host, ccsim_run): ONE template whose enabled predicates and scorers are all node-local (no
+// Eligibility (host, run_prepare): ONE template whose enabled predicates and scorers are all node-local (no
 // PodTopologySpread / InterPodAffinity counters, no hostPort-vs-clone conflicts, TaintToleration's normalised score constant
 // because no feasible-set normalisation class beyond 0 exists) and a shared-memory resident tile.
 // Then every node's total score is a function of its own clone count only, and the reference loop is a k-way merge of N

@@ -128,6 +128,13 @@ __device__ __forceinline__ long long ipa_raw(const DevParams &p, const ccsim_tem
   return sc;
 }
 
+// Dynamic shared memory of ccsim_wave_kernel: the counters, then (RESIDENT) the node tile. Must agree with the kernel's carving: per node
+// 8 B for taint, static (if any), alloc / req / nz / free cpu and memory; 4 B for free_pods, alloc_pods, npods, score, topology, local counters
+static size_t wave_smem_bytes(const DevParams &p, bool resident) {
+  const size_t per_node = 8 * (9 + (p.static_words > 0 ? 1 : 0)) + 4 * (4 + p.n_topo + p.n_local);
+  return (((size_t)p.smem_cnt_ints * 4 + 15) & ~(size_t)15) + (resident ? per_node * (size_t)p.chunk_pad : 0);
+}
+
 // ------------------------------------------------------------------------------------------------------------------
 // The persistent wave kernel (sequential engine: one winner per wave; always a valid execution of the reference loop)
 //   RESIDENT: the CTA's node tile (every column the Filter/Score pass reads) is staged into shared memory once and
@@ -717,14 +724,41 @@ __global__ void ccsim_flush_kernel(unsigned long long *buf, size_t n, unsigned l
 // ------------------------------------------------------------------------------------------------------------------
 // host side of the C-ABI
 // ------------------------------------------------------------------------------------------------------------------
+// Every wave-kernel instantiation run_prepare may pick, in the order of the WK_* indices, and what the host knows about it
+enum EngineCode { ENG_GENERIC, ENG_LEAN, ENG_TIE_RUN, ENG_MULTI, ENG_STREAM };   // ccsim_run_stats[0]
+struct WaveKernel {
+  const void *fn;
+  const char *name;        // ccsim_kernel_name
+  EngineCode engine;
+  int block;
+  size_t static_smem;      // its __shared__ structs
+  size_t fixed_dyn_smem;   // its dynamic shared-memory limit if fixed; 0: what the opt-in limit leaves (take_if_fits)
+};
+static const WaveKernel WAVE_KERNELS[] = {
+  {(const void *)ccsim_wave_kernel<true>, "wave<true>", ENG_GENERIC, BLOCK_THREADS, sizeof(WaveShared), 0},
+  {(const void *)ccsim_wave_kernel<false>, "wave<false>", ENG_GENERIC, BLOCK_THREADS, sizeof(WaveShared), SMEM_CNT_MAX_INTS * sizeof(int32_t) + 16},
+  {(const void *)ccsim_wave_lean_kernel<false>, "lean<false>", ENG_LEAN, LEAN_THREADS, sizeof(LeanShared), 0},
+  {(const void *)ccsim_wave_lean_kernel<true>, "lean<true>", ENG_LEAN, LEAN_THREADS, sizeof(LeanShared), 0},
+  {(const void *)ccsim_wave_batched_kernel, "batched", ENG_TIE_RUN, LEAN_THREADS, sizeof(LeanShared) + sizeof(BatchShared), 0},
+  {(const void *)ccsim_wave_multi_kernel<false>, "multi<false>", ENG_MULTI, LEAN_THREADS, sizeof(LeanShared) + sizeof(MultiShared), 0},
+  {(const void *)ccsim_wave_multi_kernel<true>, "multi<true>", ENG_MULTI, LEAN_THREADS, sizeof(LeanShared) + sizeof(MultiShared), 0},
+  {(const void *)ccsim_wave_stream_kernel<0>, "stream<0>", ENG_STREAM, STREAM_BLOCK, sizeof(StreamShared), stream_smem_bytes(0, 0)},
+  {(const void *)ccsim_wave_stream_kernel<1>, "stream<1>", ENG_STREAM, STREAM_BLOCK, sizeof(StreamShared), stream_smem_bytes(1, 0)},
+  {(const void *)ccsim_wave_stream_kernel<2>, "stream<2>", ENG_STREAM, STREAM_BLOCK, sizeof(StreamShared), 0},
+};
+enum { WK_WAVE, WK_WAVE_STREAMED, WK_LEAN, WK_LEAN_SAMPLING, WK_BATCHED, WK_MULTI, WK_MULTI_SHARDED, WK_STREAM /* + mode */ };
+static_assert(sizeof(WAVE_KERNELS) / sizeof(WAVE_KERNELS[0]) == WK_STREAM + 3, "one WAVE_KERNELS entry per WK_* index");
+
 struct RunPlan {      // what run_prepare decided, consumed by the launch
   bool valid = false, empty = false;
   int64_t max_pods = 0;
   DevParams p; LeanParams lp; MultiParams mp; StreamParams sp;
-  const void *kern = nullptr; int grid = 0, block = 0; size_t smem = 0;
-  bool stream = false, multi = false, batched = false, lean = false, resident = false;
-  const char *kernel_name = "";   // ccsim_kernel_name: outlives the launch, which clears `valid`
+  const WaveKernel *kern = nullptr; size_t smem = 0;   // kern: ccsim_kernel_name, outlives the launch, which clears `valid`
 };
+
+// Template facts of the engine choice (ccsim_set_templates): a template without NodeResourcesFit's Filter (no "Too many pods" bound);
+// normalised soft scorers; the lean and streaming kernels cover every template (no soft scorer, ImageLocality or needs_extras; one taint word, <= 1 static word)
+struct TemplateFacts { bool fit_off, has_soft, lean_filter; };
 
 struct ccsim_handle {
   ccsim_config cfg;
@@ -768,10 +802,11 @@ struct ccsim_handle {
   // templates
   int32_t n_templates = 0, n_counters = 0;
   std::vector<ccsim_template> h_templates;
+  TemplateFacts tf = {};
   ccsim_template *d_templates = nullptr;
   DevCounter counters[CCSIM_MAX_COUNTERS];
   int32_t *d_final_cnt = nullptr; int32_t final_off[CCSIM_MAX_COUNTERS] = {}; int32_t final_total = 0;
-  // int32 range of the counters (run_prepare): free pod slots of every node and of every domain of each topology column over the
+  // int32 range of the counters (check_run_bounds): free pod slots of every node and of every domain of each topology column over the
   // whole cluster (ccsim_load_nodes), and per counter the most placements after which all its domains are still exact
   // (ccsim_set_templates), with NodeResourcesFit bounding each domain by its slots (lim_fit) or not (lim_any)
   std::vector<int32_t> node_slots;
@@ -889,23 +924,9 @@ extern "C" int ccsim_create(const ccsim_config *cfg, ccsim_handle **out) {
   cudaMemset(h->d_xslots, 0, sizeof(unsigned long long) * XSLOTS_TOTAL_WORDS);
   h->x_peer[cfg->rank] = h->d_xslots;
   h->smem_optin = (size_t)prop.sharedMemPerBlockOptin;
-  cudaFuncSetAttribute(ccsim_wave_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                       (int)(h->smem_optin - sizeof(WaveShared) - 1024));
-  cudaFuncSetAttribute(ccsim_wave_lean_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                       (int)(h->smem_optin - sizeof(LeanShared) - 1024));
-  cudaFuncSetAttribute(ccsim_wave_lean_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                       (int)(h->smem_optin - sizeof(LeanShared) - 1024));
-  cudaFuncSetAttribute(ccsim_wave_batched_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                       (int)(h->smem_optin - sizeof(LeanShared) - sizeof(BatchShared) - 1024));
-  cudaFuncSetAttribute(ccsim_wave_multi_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                       (int)(h->smem_optin - sizeof(LeanShared) - sizeof(MultiShared) - 1024));
-  cudaFuncSetAttribute(ccsim_wave_multi_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                       (int)(h->smem_optin - sizeof(LeanShared) - sizeof(MultiShared) - 1024));
-  cudaFuncSetAttribute(ccsim_wave_stream_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(STREAM_STAGES * STREAM_TILE * 24 + 128));
-  cudaFuncSetAttribute(ccsim_wave_stream_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(STREAM_STAGES * STREAM_TILE * 40 + 128));
-  cudaFuncSetAttribute(ccsim_wave_stream_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(h->smem_optin - sizeof(StreamShared) - 1024));
-  cudaFuncSetAttribute(ccsim_wave_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                       (int)(SMEM_CNT_MAX_INTS * sizeof(int32_t) + 16));
+  for (const WaveKernel &k : WAVE_KERNELS)   // a fixed size, or what the opt-in limit leaves (take_if_fits)
+    cudaFuncSetAttribute(k.fn, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                         (int)(k.fixed_dyn_smem ? k.fixed_dyn_smem : h->smem_optin - k.static_smem - 1024));
   *out = h;
   return CCSIM_OK;
 }
@@ -1025,6 +1046,19 @@ extern "C" int ccsim_load_nodes(ccsim_handle *h, const ccsim_nodes *nd) {
   return CCSIM_OK;
 }
 
+// A template that needs one of the uncommon predicates the lean and streaming kernels leave out (filter_extras: ephemeral storage,
+// extended resources, nodeAffinity terms, nodeName, PreFilter node sets, hostPorts against clones already placed).
+static bool needs_extras(const ccsim_handle *h, const ccsim_template &T) {
+  const bool nzfit = (T.filter_enable & CCSIM_PL_FIT) && !(T.flags & CCSIM_TF_FIT_ALL_ZERO);
+  if (nzfit && T.req_eph > 0) return true;
+  if (nzfit) for (int k = 0; k < h->meta.n_scalars; k++) if (T.req_scalar[k] != 0) return true;
+  if ((T.filter_enable & CCSIM_PL_NODE_AFFINITY) && (T.flags & CCSIM_TF_HAS_AFFINITY_TERMS)) return true;
+  if ((T.filter_enable & CCSIM_PL_NODE_NAME) && T.nodename_idx >= 0) return true;
+  if (T.flags & CCSIM_TF_PREFILTER_NODES) return true;
+  if ((T.filter_enable & CCSIM_PL_NODE_PORTS) && (T.flags & CCSIM_TF_HAS_HOST_PORTS) && h->w_placed) return true;
+  return false;
+}
+
 extern "C" int ccsim_set_templates(ccsim_handle *h, int32_t n_templates, const ccsim_template *templates,
                                    int32_t n_counters, const ccsim_counter *counters) {
   if (!h || !templates) return fail(h, CCSIM_EINVAL, "null argument");
@@ -1082,6 +1116,17 @@ extern "C" int ccsim_set_templates(ccsim_handle *h, int32_t n_templates, const c
   if (h->max_prefer_pop + 1 > CCSIM_MAX_CLASSES)
     return fail(h, CCSIM_EUNSUPPORTED, "a node carries %d PreferNoSchedule taints (max %d)", h->max_prefer_pop, CCSIM_MAX_CLASSES - 1);
   h->h_templates.assign(templates, templates + n_templates);
+  TemplateFacts &tf = h->tf;
+  tf = TemplateFacts{false, false, nd.taint_words == 1 && nd.static_words <= 1};
+  for (const ccsim_template &T : h->h_templates) {
+    if (!(T.filter_enable & CCSIM_PL_FIT)) tf.fit_off = true;
+    if (T.n_pref_terms > 0 && (T.score_enable & CCSIM_PL_NODE_AFFINITY)) tf.has_soft = true;
+    if (T.n_spts > 0 && (T.score_enable & CCSIM_PL_POD_TOPOLOGY_SPREAD)) tf.has_soft = true;
+    if (T.n_ipa_score > 0 && (T.score_enable & CCSIM_PL_INTER_POD_AFFINITY)) tf.has_soft = true;
+    if ((T.image_score && (T.score_enable & CCSIM_PL_IMAGE_LOCALITY)) || needs_extras(h, T)) tf.lean_filter = false;
+  }
+  for (int j = 0; j < n_counters; j++) if (counters[j].elig_bit >= 0) tf.has_soft = true;
+  if (tf.has_soft) tf.lean_filter = false;
   int rc;
   {
     // ImageLocality columns: this shard's slice goes to the device, the device copy of the template points at it
@@ -1147,77 +1192,15 @@ extern "C" int ccsim_set_templates(ccsim_handle *h, int32_t n_templates, const c
   return CCSIM_OK;
 }
 
-static void fill_params(ccsim_handle *h, DevParams &p, int64_t max_pods) {
-  memset(&p, 0, sizeof(p));
-  const ccsim_nodes &nd = h->meta;
-  p.n = h->n; p.n_global = h->n_global; p.node_base = h->node_base;
-  p.n_scalars = nd.n_scalars; p.taint_words = nd.taint_words; p.static_words = nd.static_words; p.n_topo = nd.n_topo_cols;
-  p.n_templates = h->n_templates; p.n_counters = h->n_counters;
-  p.n_classes = h->max_prefer_pop + 1;
-  p.rank = h->cfg.rank; p.world = h->cfg.world;
-  p.alloc_cpu = h->d_alloc_cpu; p.alloc_mem = h->d_alloc_mem; p.alloc_eph = h->d_alloc_eph; p.alloc_pods = h->d_alloc_pods;
-  for (int k = 0; k < nd.n_scalars; k++) { p.alloc_scalar[k] = h->d_alloc_scalar[k]; p.req_scalar[k] = h->w_req_scalar[k]; }
-  p.taint_mask = h->d_taint; p.static_mask = h->d_static;
-  for (int k = 0; k < nd.n_topo_cols; k++) { p.topo[k] = h->d_topo[k]; p.topo_full[k] = h->d_topo_full[k]; }
-  for (int r = 0; r < CCSIM_MAX_WORLD; r++) p.xslots_peer[r] = h->x_peer[r];
-  p.req_cpu = h->w_req_cpu; p.req_mem = h->w_req_mem; p.req_eph = h->w_req_eph; p.nz_cpu = h->w_nz_cpu; p.nz_mem = h->w_nz_mem;
-  p.npods = h->w_npods; p.placed_mask = h->w_placed; p.score_cache = h->w_score; p.feas = h->w_feas;
-  for (int c = 0; c < CCSIM_MAX_PTS; c++) p.stamp[c] = h->d_stamp[c];
-  for (int w = 0; w < CCSIM_MAX_TAINT_WORDS; w++) { p.taint_nosched[w] = nd.taint_nosched[w]; p.taint_prefer[w] = nd.taint_prefer[w]; }
-  p.templates = h->d_templates;
-  for (int j = 0; j < h->n_counters; j++) { p.counters[j] = h->counters[j]; p.final_off[j] = h->final_off[j]; }
-  p.final_cnt = h->d_final_cnt;
-  p.slots = h->d_slots;
-  p.pod_node = h->d_pod_node; p.pod_cap = h->pod_cap; p.max_pods = max_pods;
-  p.out = h->d_out;
-  p.taint_list_off = h->d_taint_off; p.taint_list = h->d_taint_list;
-}
-
-// A template that needs one of the uncommon predicates the lean and streaming kernels leave out (filter_extras: ephemeral storage,
-// extended resources, nodeAffinity terms, nodeName, PreFilter node sets, hostPorts against clones already placed).
-static bool needs_extras(const ccsim_handle *h, const ccsim_template &T) {
-  const bool nzfit = (T.filter_enable & CCSIM_PL_FIT) && !(T.flags & CCSIM_TF_FIT_ALL_ZERO);
-  if (nzfit && T.req_eph > 0) return true;
-  if (nzfit) for (int k = 0; k < h->meta.n_scalars; k++) if (T.req_scalar[k] != 0) return true;
-  if ((T.filter_enable & CCSIM_PL_NODE_AFFINITY) && (T.flags & CCSIM_TF_HAS_AFFINITY_TERMS)) return true;
-  if ((T.filter_enable & CCSIM_PL_NODE_NAME) && T.nodename_idx >= 0) return true;
-  if (T.flags & CCSIM_TF_PREFILTER_NODES) return true;
-  if ((T.filter_enable & CCSIM_PL_NODE_PORTS) && (T.flags & CCSIM_TF_HAS_HOST_PORTS) && h->w_placed) return true;
-  return false;
-}
-
-// ccsim_kernel_name of a wave-kernel instantiation
-static const char *kernel_name_of(const void *kern) {
-  const struct { const void *k; const char *name; } names[] = {
-    {(const void *)ccsim_wave_kernel<true>, "wave<true>"}, {(const void *)ccsim_wave_kernel<false>, "wave<false>"},
-    {(const void *)ccsim_wave_lean_kernel<false>, "lean<false>"}, {(const void *)ccsim_wave_lean_kernel<true>, "lean<true>"},
-    {(const void *)ccsim_wave_batched_kernel, "batched"},
-    {(const void *)ccsim_wave_multi_kernel<false>, "multi<false>"}, {(const void *)ccsim_wave_multi_kernel<true>, "multi<true>"},
-    {(const void *)ccsim_wave_stream_kernel<0>, "stream<0>"}, {(const void *)ccsim_wave_stream_kernel<1>, "stream<1>"},
-    {(const void *)ccsim_wave_stream_kernel<2>, "stream<2>"}};
-  for (const auto &e : names) if (e.k == kern) return e.name;
-  return "?";
-}
-
-// Everything a Run does before the wave kernel starts: output / streaming buffers, restoring the working columns, choosing the
-// engine, uploading the parameters. Kept apart from the launch (ccsim_prepare) for hosts that drive several ranks from one
-// process: every rank must be past its allocations before any rank's persistent kernel starts waiting for its peers.
-static int run_prepare(ccsim_handle *h, int64_t max_pods) {
-  if (!h->have_nodes || !h->have_templates) return fail(h, CCSIM_ESTATE, "load_nodes and set_templates must come first");
-  if (h->cfg.world > 1 && !h->peers_ready) return fail(h, CCSIM_ESTATE, "sharded run: ccsim_peer_import must come first");
-  CK(cudaSetDevice(h->cfg.device));
-  RunPlan &pl = h->plan;
-  pl.valid = false; pl.empty = false; pl.max_pods = max_pods; pl.kernel_name = "";
-  const int32_t n = h->n;
-  // output capacity: no run can place more than sum(max(0, alloc_pods - npods)) pods (fit.go:567-576)
-  int64_t cap = h->pod_bound + 1;
+// The refusals a run meets before it touches anything: a run that nothing bounds, and counters that could leave int32. `cap`: the
+// output capacity, since no run can place more than sum(max(0, alloc_pods - npods)) pods (fit.go:567-576), or max_pods.
+static int check_run_bounds(ccsim_handle *h, int64_t max_pods, int64_t &cap) {
+  const bool fit_off = h->tf.fit_off;
   // ("Too many pods" bounds a run only while NodeResourcesFit filters: with the plugin disabled through --default-config an
   //  unlimited run never ends in the reference either)
-  if (max_pods <= 0)
-    for (const ccsim_template &T : h->h_templates)
-      if (!(T.filter_enable & CCSIM_PL_FIT))
-        return fail(h, CCSIM_EUNSUPPORTED, "NodeResourcesFit is disabled for a template: the run is unbounded, --max-limit is required");
-  const bool fit_off = [&] { for (const ccsim_template &T : h->h_templates) if (!(T.filter_enable & CCSIM_PL_FIT)) return true; return false; }();
+  if (max_pods <= 0 && fit_off)
+    return fail(h, CCSIM_EUNSUPPORTED, "NodeResourcesFit is disabled for a template: the run is unbounded, --max-limit is required");
+  cap = h->pod_bound + 1;
   if (max_pods > 0 && (max_pods < cap || fit_off)) cap = max_pods;
   // Counters are int32 here and in the oracle; the reference counts in int64 (podtopologyspread/scoring.go,
   // interpodaffinity/scoring.go). A counter that could leave int32 during the run is refused, never left to wrap: a domain that
@@ -1236,14 +1219,18 @@ static int run_prepare(ccsim_handle *h, int64_t max_pods) {
                   j, d, std::llabs((long long)(fit_off ? r.init_any : r.init_fit)), (long long)m, std::abs(h->counters[j].inc));
     }
   }
+  return CCSIM_OK;
+}
+
+// The pod -> node buffer grown to `cap`; the working columns restored from the snapshot (a Run never changes the snapshot)
+static int restore_run_state(ccsim_handle *h, int64_t cap) {
   if (cap > h->pod_cap) {
     if (h->d_pod_node) cudaFreeAsync(h->d_pod_node, h->stream);
     h->d_pod_node = nullptr; h->pod_cap = 0;
     CK(cudaMallocAsync((void **)&h->d_pod_node, (size_t)cap * sizeof(int32_t), h->stream));
     h->pod_cap = cap;
   }
-  // restore the working copies of the mutable columns from the snapshot (a Run never changes the loaded snapshot)
-  cudaStream_t s = h->stream;
+  const int32_t n = h->n; cudaStream_t s = h->stream;
   if (n) {
     CK(cudaMemcpyAsync(h->w_req_cpu, h->s_req_cpu, (size_t)n * 8, cudaMemcpyDeviceToDevice, s));
     CK(cudaMemcpyAsync(h->w_req_mem, h->s_req_mem, (size_t)n * 8, cudaMemcpyDeviceToDevice, s));
@@ -1263,48 +1250,33 @@ static int run_prepare(ccsim_handle *h, int64_t max_pods) {
   CK(cudaMemsetAsync(h->d_slots, 0, sizeof(unsigned long long) * SLOTS_WORDS, s));
   // (the cross-GPU buffer is NOT cleared here: peers may already be writing wave 0 of this run; stale words are
   //  harmless because runs advance a per-handle epoch that is folded into the tag)
+  return CCSIM_OK;
+}
 
-  if (n == 0) {   // ErrNoNodesAvailable (scheduler.go:68): nothing to evaluate; the host formats the message
-    CK(cudaStreamSynchronize(s));
-    pl.empty = true; pl.valid = true;
-    return CCSIM_OK;
-  }
+// The persistent grid and every kernel's parameters; advances the epoch (every rank of a sharded run prepares alike, refused or not)
+static void fill_params(ccsim_handle *h, DevParams &p, int64_t max_pods) {
+  memset(&p, 0, sizeof(p));
+  const ccsim_nodes &nd = h->meta;
   // grid: one persistent CTA per SM (fewer for tiny clusters: the exchange cost grows with the CTA count)
-  int grid = std::min(h->sm_count, CCSIM_MAX_GRID);
   // (node-sharded runs: every rank sizes the grid from the largest shard, so that all ranks launch the same grid and every
   //  rank knows how many candidate lines its peers publish)
-  const int32_t n_grid = h->cfg.world > 1 ? (h->n_global + h->cfg.world - 1) / h->cfg.world : n;
-  const int want = (n_grid + BLOCK_THREADS - 1) / BLOCK_THREADS;
-  if (want < grid) grid = want;
-  if (grid < 1) grid = 1;
-  h->grid = grid;
-  DevParams p;
-  fill_params(h, p, max_pods);
-  p.grid = grid;
-  p.chunk = (n + grid - 1) / grid;
-  h->epoch = (h->epoch % 255u) + 1u;     // every rank of a sharded run calls ccsim_run the same number of times
+  const int32_t n_grid = h->cfg.world > 1 ? (h->n_global + h->cfg.world - 1) / h->cfg.world : h->n;
+  p.grid = std::max(1, std::min({h->sm_count, CCSIM_MAX_GRID, (n_grid + BLOCK_THREADS - 1) / BLOCK_THREADS}));
+  h->grid = p.grid;
+  p.n = h->n; p.n_global = h->n_global; p.node_base = h->node_base;
+  p.chunk = (p.n + p.grid - 1) / p.grid;
+  p.chunk_pad = (p.chunk + 3) & ~3;
+  p.n_scalars = nd.n_scalars; p.taint_words = nd.taint_words; p.static_words = nd.static_words; p.n_topo = nd.n_topo_cols;
+  p.n_templates = h->n_templates; p.n_counters = h->n_counters;
+  for (int j = 0; j < h->n_counters; j++) if (h->counters[j].topo_col < 0) p.n_local++;
+  p.smem_cnt_ints = h->smem_cnt_ints;
+  p.n_classes = h->max_prefer_pop + 1;
+  p.rank = h->cfg.rank; p.world = h->cfg.world;
+  h->epoch = (h->epoch % 255u) + 1u;
   p.epoch = h->epoch;
   p.xwave0 = h->xwave0;
   p.debug_flags = getenv("CCSIM_DEBUG_FLAGS") ? (uint32_t)atoi(getenv("CCSIM_DEBUG_FLAGS")) : 0u;
-  // resident mode: every column the Filter/Score pass reads is staged into shared memory once
-  int n_local = 0;
-  for (int j = 0; j < h->n_counters; j++) if (h->counters[j].topo_col < 0) n_local++;
-  p.n_local = n_local;
-  p.chunk_pad = (p.chunk + 3) & ~3;
-  p.smem_cnt_ints = h->smem_cnt_ints;
-  const size_t cnt_bytes = ((size_t)h->smem_cnt_ints * 4 + 15) & ~(size_t)15;
-  const size_t per_node = 8 * (9 + (h->meta.static_words > 0 ? 1 : 0)) + 4 * (4 + h->meta.n_topo_cols + n_local);
-  const size_t smem_res = cnt_bytes + per_node * (size_t)p.chunk_pad;
-  const size_t smem_str = cnt_bytes;
-  const bool resident = smem_res + sizeof(WaveShared) + 1024 <= h->smem_optin;
-  p.tile_resident = resident ? 1 : 0;
-  size_t smem = resident ? smem_res : smem_str;
-  const void *kern = resident ? (const void *)ccsim_wave_kernel<true> : (const void *)ccsim_wave_kernel<false>;
-  int block = BLOCK_THREADS;
-  // lean resident kernel: the common case (see ccsim_lean.cuh for the eligibility rules)
-  // reference sampling mode (ccsim_config.sampling): numFeasibleNodesToFind (schedule_one.go:697-723)
-  const bool faithful = h->cfg.sampling == CCSIM_SAMPLING_REFERENCE;
-  {
+  {   // reference sampling mode (ccsim_config.sampling): numFeasibleNodesToFind (schedule_one.go:697-723)
     const long long N = h->n_global;
     long long pct = h->cfg.pct_nodes_to_score, kf = N;
     if (N >= 100) {
@@ -1314,155 +1286,182 @@ static int run_prepare(ccsim_handle *h, int64_t max_pods) {
     }
     p.sample_k = kf;
   }
-  LeanParams lp; memset(&lp, 0, sizeof(lp));
-  // the lean kernel (768 threads) takes every eligible workload
-  // normalised soft scorers / ImageLocality columns run in the generic kernel only (multi-phase waves)
-  bool has_pref = false, has_soft = false;
-  for (auto &T : h->h_templates) {
-    if (T.n_pref_terms > 0 && (T.score_enable & CCSIM_PL_NODE_AFFINITY)) has_soft = true;
-    if (T.n_spts > 0 && (T.score_enable & CCSIM_PL_POD_TOPOLOGY_SPREAD)) has_soft = true;
-    if (T.n_ipa_score > 0 && (T.score_enable & CCSIM_PL_INTER_POD_AFFINITY)) has_soft = true;
-    if (T.image_score && (T.score_enable & CCSIM_PL_IMAGE_LOCALITY)) has_pref = true;
+  p.alloc_cpu = h->d_alloc_cpu; p.alloc_mem = h->d_alloc_mem; p.alloc_eph = h->d_alloc_eph; p.alloc_pods = h->d_alloc_pods;
+  for (int k = 0; k < nd.n_scalars; k++) { p.alloc_scalar[k] = h->d_alloc_scalar[k]; p.req_scalar[k] = h->w_req_scalar[k]; }
+  p.taint_mask = h->d_taint; p.static_mask = h->d_static;
+  for (int k = 0; k < nd.n_topo_cols; k++) { p.topo[k] = h->d_topo[k]; p.topo_full[k] = h->d_topo_full[k]; }
+  for (int r = 0; r < CCSIM_MAX_WORLD; r++) p.xslots_peer[r] = h->x_peer[r];
+  p.req_cpu = h->w_req_cpu; p.req_mem = h->w_req_mem; p.req_eph = h->w_req_eph; p.nz_cpu = h->w_nz_cpu; p.nz_mem = h->w_nz_mem;
+  p.npods = h->w_npods; p.placed_mask = h->w_placed; p.score_cache = h->w_score; p.feas = h->w_feas;
+  for (int c = 0; c < CCSIM_MAX_PTS; c++) p.stamp[c] = h->d_stamp[c];
+  for (int w = 0; w < CCSIM_MAX_TAINT_WORDS; w++) { p.taint_nosched[w] = nd.taint_nosched[w]; p.taint_prefer[w] = nd.taint_prefer[w]; }
+  p.templates = h->d_templates;
+  for (int j = 0; j < h->n_counters; j++) { p.counters[j] = h->counters[j]; p.final_off[j] = h->final_off[j]; }
+  p.final_cnt = h->d_final_cnt;
+  p.slots = h->d_slots;
+  p.pod_node = h->d_pod_node; p.pod_cap = h->pod_cap; p.max_pods = max_pods;
+  p.out = h->d_out;
+  p.taint_list_off = h->d_taint_off; p.taint_list = h->d_taint_list;
+  p.self = h->d_params;
+}
+
+// Takes kernel `e` with `dyn` bytes of dynamic shared memory if they fit next to its static structs, with 1 KB to spare
+static bool take_if_fits(const ccsim_handle *h, RunPlan &pl, const WaveKernel *&k, const WaveKernel &e, size_t dyn) {
+  if (dyn + e.static_smem + 1024 > h->smem_optin) return false;
+  k = &e; pl.smem = dyn;
+  return true;
+}
+
+// The lean resident kernel (ccsim_lean.cuh: eligibility): a record slot per topology column and node-local counter, the tile layout
+static bool plan_lean(const ccsim_handle *h, RunPlan &pl, bool faithful, const WaveKernel *&k) {
+  if (!h->tf.lean_filter || h->n_templates != 1) return false;
+  const ccsim_template &T = h->h_templates[0];
+  if (T.n_pts + T.n_aff + T.n_anti > LEAN_MAX_TERMS) return false;
+  LeanParams &lp = pl.lp;
+  int ns = 0;
+  for (int j = 0; j < h->n_counters; j++) {
+    const DevCounter &dc = h->counters[j];
+    if (dc.topo_col >= 0 && dc.smem_off < 0) return false;
+    int slot = -1;
+    if (dc.topo_col >= 0) for (int q = 0; q < ns; q++) if (lp.slot_topo[q] == dc.topo_col) slot = q;
+    if (slot < 0) {
+      if (ns >= LEAN_MAX_SLOTS) return false;
+      slot = ns++;
+      lp.slot_topo[slot] = dc.topo_col >= 0 ? dc.topo_col : -1;
+      lp.slot_counter[slot] = dc.topo_col >= 0 ? -1 : j;
+    }
+    lp.counter_slot[j] = slot;
   }
-  for (int j = 0; j < h->n_counters; j++) if (h->counters[j].elig_bit >= 0) has_soft = true;
-  if (has_soft && (h->cfg.world > 1 || h->n_templates > 1))
+  lp.n_slots = ns;
+  lean_layout(lp, h->smem_cnt_ints, pl.p.chunk_pad);
+  return take_if_fits(h, pl, k, WAVE_KERNELS[faithful ? WK_LEAN_SAMPLING : WK_LEAN],
+                      lean_smem_bytes(lp, pl.p.chunk_pad, faithful ? 8 : 0));     // + the sampling pass's feasibility and rank
+}
+
+// Multi-commit waves (ccsim_multi.cuh) on the lean tile: one template coupled through per-domain counters, one node per thread
+static void plan_multi(const ccsim_handle *h, RunPlan &pl, const WaveKernel *&k) {
+  const ccsim_template &T = h->h_templates[0];
+  const DevParams &p = pl.p;
+  if (h->n_counters == 0 || h->max_prefer_pop != 0 || h->cfg.engine != CCSIM_ENGINE_AUTO || T.n_aff != 0 ||
+      p.chunk > LEAN_THREADS || h->n_global >= (1 << MULTI_IDX_BITS) || p.grid * MULTI_M > MULTI_EPT * LEAN_THREADS)
+    return;
+  int refs[CCSIM_MAX_COUNTERS] = {}, gt = 0;      // Filter terms reading each counter; those reading a replicated one
+  if (T.filter_enable & CCSIM_PL_POD_TOPOLOGY_SPREAD) for (int c = 0; c < T.n_pts; c++) refs[T.pts[c].counter]++;
+  if (T.filter_enable & CCSIM_PL_INTER_POD_AFFINITY) for (int a = 0; a < T.n_anti; a++) refs[T.anti_counter[a]]++;
+  for (int j = 0; j < h->n_counters; j++) {
+    const DevCounter &dc = h->counters[j];
+    if (dc.inc < 0) return;                         // feasibility must be monotone within a wave
+    if (dc.topo_col >= 0) gt += refs[j];
+    // (a committed node may win again inside a wave: every candidate carries its key after one more clone, MULTI_NEXT_SHIFT)
+    // the replay updates counters term by term: every incremented replicated counter must be read by exactly one Filter term
+    if (dc.topo_col >= 0 && dc.inc != 0 && refs[j] != 1) return;
+  }
+  if (gt > MULTI_GT) return;
+  const LeanParams &lp = pl.lp; MultiParams &mp = pl.mp;
+  uint32_t shift = 0;
+  for (int sl = 0; sl < lp.n_slots; sl++) {
+    if (lp.slot_topo[sl] < 0) continue;
+    int maxd = 1;
+    for (int j = 0; j < h->n_counters; j++) if (lp.counter_slot[j] == sl && h->counters[j].topo_col >= 0) maxd = std::max(maxd, h->counters[j].n_domains);
+    uint32_t bits = 0; while ((1u << bits) <= (uint32_t)maxd) bits++;        // values 0..maxd (dom + 1)
+    if (shift + bits + 1 > MULTI_PAY_BITS) return;
+    mp.pay_shift[sl] = shift; mp.pay_mask[sl] = (1u << bits) - 1u; shift += bits + 1;   // + a zero guard bit (the replay's SWAR kill test)
+  }
+  // + the per-node payload column, and 16 bytes that nothing reads: kept so that the kernel's shared-memory size, which
+  //   run_stats() reports, stays what it has been
+  take_if_fits(h, pl, k, WAVE_KERNELS[h->cfg.world > 1 ? WK_MULTI_SHARDED : WK_MULTI], lean_smem_bytes(lp, p.chunk_pad, 8) + 16);
+}
+
+// Streaming waves (ccsim_stream.cuh: TMA-staged tiles, per-template score memo) when the lean tile is not taken; fills its padded columns
+static int plan_stream(ccsim_handle *h, RunPlan &pl, const WaveKernel *&k) {
+  if (!h->tf.lean_filter || h->n_counters != 0 || h->max_prefer_pop != 0) return CCSIM_OK;
+  const DevParams &p = pl.p; StreamParams &sp = pl.sp;
+  free_pool(h, h->stream_allocs);
+  bool masks = false;
+  for (const ccsim_template &T : h->h_templates) {
+    uint64_t tb = 0;
+    if (T.filter_enable & CCSIM_PL_TAINT_TOLERATION) tb |= h->meta.taint_nosched[0] & ~T.tol_nosched[0] & ~(1ull << CCSIM_TAINT_UNSCHEDULABLE_BIT);
+    if ((T.filter_enable & CCSIM_PL_NODE_UNSCHEDULABLE) && !(T.flags & CCSIM_TF_TOLERATES_UNSCHEDULABLE)) tb |= 1ull << CCSIM_TAINT_UNSCHEDULABLE_BIT;
+    if (tb & h->taint_or0) masks = true;
+    if (h->meta.static_words > 0) {
+      if ((T.filter_enable & CCSIM_PL_NODE_AFFINITY) && (T.flags & CCSIM_TF_HAS_NODE_SELECTOR) && T.sel_mask[0]) masks = true;
+      if ((T.filter_enable & CCSIM_PL_NODE_PORTS) && (T.flags & CCSIM_TF_HAS_HOST_PORTS) && T.port_static_mask[0]) masks = true;
+      if ((T.filter_enable & CCSIM_PL_INTER_POD_AFFINITY) && T.existing_anti_mask[0]) masks = true;
+    }
+  }
+  sp.use_masks = masks ? 1 : 0;
+  sp.chunk_pad = ((p.chunk + STREAM_TILE - 1) / STREAM_TILE) * STREAM_TILE;
+  sp.tiles = sp.chunk_pad / STREAM_TILE;
+  sp.n_pad = (long long)p.grid * sp.chunk_pad;
+  int rc;
+  unsigned long long *mt = nullptr, *mst = nullptr;
+  if ((rc = dev_alloc<long long>(h, h->stream_allocs, &sp.f_cpu, (size_t)sp.n_pad))) return rc;
+  if ((rc = dev_alloc<long long>(h, h->stream_allocs, &sp.f_mem, (size_t)sp.n_pad))) return rc;
+  if ((rc = dev_alloc<int32_t>(h, h->stream_allocs, &sp.f_pods, (size_t)sp.n_pad))) return rc;
+  if (masks) {
+    if ((rc = dev_alloc<unsigned long long>(h, h->stream_allocs, &mt, (size_t)sp.n_pad))) return rc;
+    if ((rc = dev_alloc<unsigned long long>(h, h->stream_allocs, &mst, (size_t)sp.n_pad))) return rc;
+  }
+  sp.m_taint = mt; sp.m_static = mst;
+  if ((rc = dev_alloc<int32_t>(h, h->stream_allocs, &sp.memo, (size_t)sp.n_pad * h->n_templates))) return rc;
+  CK(cudaMemsetAsync(sp.memo, 0xFF, (size_t)sp.n_pad * h->n_templates * 4, h->stream));
+  ccsim_stream_prep_kernel<<<std::min<long long>(8LL * h->sm_count, (sp.n_pad + 255) / 256), 256, 0, h->stream>>>(p, sp);
+  h->launches++;
+  CK(cudaGetLastError());
+  // resident free_* columns when the chunk fits next to the memo ring (24 B per node: up to ~7.8k nodes per SM)
+  sp.res_rows = (p.chunk + 31) & ~31;
+  k = &WAVE_KERNELS[WK_STREAM + (masks ? 1 : 0)]; pl.smem = stream_smem_bytes(masks ? 1 : 0, 0);
+  if (!masks && sp.tiles <= STREAM_STAGES_RES && !getenv("CCSIM_STREAM_ALL"))
+    take_if_fits(h, pl, k, WAVE_KERNELS[WK_STREAM + 2], stream_smem_bytes(2, sp.res_rows));
+  return CCSIM_OK;
+}
+
+// Everything a Run does before the wave kernel starts: output / streaming buffers, restoring the working columns, choosing the
+// kernel, uploading the parameters. Kept apart from the launch (ccsim_prepare) for hosts that drive several ranks from one
+// process: every rank must be past its allocations before any rank's persistent kernel starts waiting for its peers.
+static int run_prepare(ccsim_handle *h, int64_t max_pods) {
+  if (!h->have_nodes || !h->have_templates) return fail(h, CCSIM_ESTATE, "load_nodes and set_templates must come first");
+  if (h->cfg.world > 1 && !h->peers_ready) return fail(h, CCSIM_ESTATE, "sharded run: ccsim_peer_import must come first");
+  CK(cudaSetDevice(h->cfg.device));
+  RunPlan &pl = h->plan;
+  pl = RunPlan();                         // no kernel name until a kernel is chosen; the parameter blocks zeroed
+  pl.max_pods = max_pods;
+  int64_t cap = 0; int rc;
+  if ((rc = check_run_bounds(h, max_pods, cap)) || (rc = restore_run_state(h, cap))) return rc;
+  if (h->n == 0) {   // ErrNoNodesAvailable (scheduler.go:68): nothing to evaluate; the host formats the message
+    CK(cudaStreamSynchronize(h->stream));
+    pl.empty = true; pl.valid = true;
+    return CCSIM_OK;
+  }
+  DevParams &p = pl.p;
+  fill_params(h, p, max_pods);
+  // 1. the generic kernel, its tile resident in shared memory if it fits (the order of DESIGN.md §4; each refusal at its point)
+  const WaveKernel *k = &WAVE_KERNELS[WK_WAVE_STREAMED];
+  pl.smem = wave_smem_bytes(p, false);
+  p.tile_resident = take_if_fits(h, pl, k, WAVE_KERNELS[WK_WAVE], wave_smem_bytes(p, true)) ? 1 : 0;
+  if (h->tf.has_soft && (h->cfg.world > 1 || h->n_templates > 1))
     return fail(h, CCSIM_EUNSUPPORTED, "normalised soft scorers (preferred nodeAffinity, ScheduleAnyway spreading, pod-affinity scoring): single template, single GPU only");
-  has_pref = has_pref || has_soft;
-  bool lean = resident && !has_pref && h->n_templates == 1 && h->meta.taint_words == 1 && h->meta.static_words <= 1;
-  if (lean) {
-    const ccsim_template &T = h->h_templates[0];
-    if (needs_extras(h, T)) lean = false;
-    if (T.n_pts + T.n_aff + T.n_anti > LEAN_MAX_TERMS) lean = false;
-    int ns = 0;
-    for (int j = 0; j < h->n_counters && lean; j++) {
-      const DevCounter &dc = h->counters[j];
-      if (dc.topo_col >= 0 && dc.smem_off < 0) { lean = false; break; }
-      int slot = -1;
-      if (dc.topo_col >= 0) for (int q = 0; q < ns; q++) if (lp.slot_topo[q] == dc.topo_col) slot = q;
-      if (slot < 0) {
-        if (ns >= LEAN_MAX_SLOTS) { lean = false; break; }
-        slot = ns++;
-        lp.slot_topo[slot] = dc.topo_col >= 0 ? dc.topo_col : -1;
-        lp.slot_counter[slot] = dc.topo_col >= 0 ? -1 : j;
-      }
-      lp.counter_slot[j] = slot;
-    }
-    if (lean) {
-      lp.n_slots = ns;
-      lean_layout(lp, h->smem_cnt_ints, p.chunk_pad);
-      const size_t smem_lean = lean_smem_bytes(lp, p.chunk_pad, faithful ? 8 : 0);     // + the sampling pass's feasibility and rank
-      if (smem_lean + sizeof(LeanShared) + 1024 > h->smem_optin) lean = false;
-      else { smem = smem_lean; kern = faithful ? (const void *)ccsim_wave_lean_kernel<true> : (const void *)ccsim_wave_lean_kernel<false>; block = LEAN_THREADS; }
-    }
-  }
+  // 2. the lean kernel if eligible
+  const bool faithful = h->cfg.sampling == CCSIM_SAMPLING_REFERENCE;
+  const bool lean = p.tile_resident && plan_lean(h, pl, faithful, k);
   if (faithful && (!lean || h->cfg.world > 1))
     return fail(h, CCSIM_EUNSUPPORTED, "reference sampling mode needs the lean resident kernel on a single GPU (one template, <=1 taint/static word, no extras)");
-  // batched tie-run engine (ccsim_batched.cuh): one template, node-local predicates and scorers only
-  bool batched = lean && !faithful && h->n_counters == 0 && h->max_prefer_pop == 0 && h->cfg.world == 1 &&
-                 h->cfg.engine != CCSIM_ENGINE_SEQUENTIAL;
-  if (batched) {
-    const size_t smem_b = lean_smem_bytes(lp, p.chunk_pad, 12);     // + run length, score after the run, run offset
-    if (smem_b + sizeof(LeanShared) + sizeof(BatchShared) + 1024 > h->smem_optin) batched = false;
-    else { smem = smem_b; kern = (const void *)ccsim_wave_batched_kernel; }
-  }
+  // 3. tie-run batching (ccsim_batched.cuh: node-local predicates and scorers only; + run length, score after the run, run offset
+  //    per node) or multi-commit waves on the lean tile
+  const bool batched = lean && !faithful && h->n_counters == 0 && h->max_prefer_pop == 0 && h->cfg.world == 1 &&
+                       h->cfg.engine != CCSIM_ENGINE_SEQUENTIAL &&
+                       take_if_fits(h, pl, k, WAVE_KERNELS[WK_BATCHED], lean_smem_bytes(pl.lp, p.chunk_pad, 12));
   if (h->cfg.engine == CCSIM_ENGINE_BATCHED && !batched)
     return fail(h, CCSIM_EUNSUPPORTED, "batched engine needs one template with node-local predicates only, no PreferNoSchedule taints, a resident tile and a single GPU");
-  // multi-commit waves (ccsim_multi.cuh): one template coupled through per-domain counters, one node per thread
-  MultiParams mp; memset(&mp, 0, sizeof(mp));
-  bool multi = lean && !faithful && !batched && h->n_counters > 0 && h->max_prefer_pop == 0 &&
-               h->cfg.engine == CCSIM_ENGINE_AUTO && h->h_templates[0].n_aff == 0 &&
-               p.chunk <= LEAN_THREADS && h->n_global < (1 << MULTI_IDX_BITS) && grid * MULTI_M <= MULTI_EPT * LEAN_THREADS;
-  if (multi) {
-    for (int j = 0; j < h->n_counters; j++) if (h->counters[j].inc < 0) multi = false;   // feasibility must be monotone within a wave
-    {
-      const ccsim_template &T = h->h_templates[0];
-      int gt = 0;
-      if (T.filter_enable & CCSIM_PL_POD_TOPOLOGY_SPREAD) for (int c = 0; c < T.n_pts; c++) if (h->counters[T.pts[c].counter].topo_col >= 0) gt++;
-      if (T.filter_enable & CCSIM_PL_INTER_POD_AFFINITY) for (int a = 0; a < T.n_anti; a++) if (h->counters[T.anti_counter[a]].topo_col >= 0) gt++;
-      if (gt > MULTI_GT) multi = false;
-      // (a committed node may win again inside a wave: every candidate carries its key after one more clone, MULTI_NEXT_SHIFT)
-      // the replay updates counters term by term: every incremented replicated counter must be read by exactly one Filter term
-      for (int j = 0; j < h->n_counters; j++) {
-        if (h->counters[j].topo_col < 0 || h->counters[j].inc == 0) continue;
-        int refs = 0;
-        if (T.filter_enable & CCSIM_PL_POD_TOPOLOGY_SPREAD) for (int c = 0; c < T.n_pts; c++) if (T.pts[c].counter == j) refs++;
-        if (T.filter_enable & CCSIM_PL_INTER_POD_AFFINITY) for (int a = 0; a < T.n_anti; a++) if (T.anti_counter[a] == j) refs++;
-        if (refs != 1) multi = false;
-      }
-    }
-    uint32_t shift = 0;
-    for (int sl = 0; sl < lp.n_slots && multi; sl++) {
-      if (lp.slot_topo[sl] < 0) continue;
-      int maxd = 1;
-      for (int j = 0; j < h->n_counters; j++) if (lp.counter_slot[j] == sl && h->counters[j].topo_col >= 0) maxd = std::max(maxd, h->counters[j].n_domains);
-      uint32_t bits = 0; while ((1u << bits) <= (uint32_t)maxd) bits++;        // values 0..maxd (dom + 1)
-      if (shift + bits + 1 > MULTI_PAY_BITS) { multi = false; break; }
-      mp.pay_shift[sl] = shift; mp.pay_mask[sl] = (1u << bits) - 1u; shift += bits + 1;   // + a zero guard bit (the replay's SWAR kill test)
-    }
-    // + the per-node payload column, and 16 bytes that nothing reads: kept so that the kernel's shared-memory size, which
-    //   run_stats() reports, stays what it has been
-    const size_t smem_m = lean_smem_bytes(lp, p.chunk_pad, 8) + 16;
-    if (smem_m + sizeof(LeanShared) + sizeof(MultiShared) + 1024 > h->smem_optin) multi = false;
-    if (multi) { kern = h->cfg.world > 1 ? (const void *)ccsim_wave_multi_kernel<true> : (const void *)ccsim_wave_multi_kernel<false>; smem = smem_m; }
-  }
-  // streaming engine (ccsim_stream.cuh): node-local templates when the tile is not resident, or several templates; the node
-  // tiles go through shared memory with bulk-async copies (TMA) and the score is memoised per (template, node)
-  StreamParams sp; memset(&sp, 0, sizeof(sp));
-  int stream_mode = 0;
-  bool stream = !lean && !has_pref && h->n_counters == 0 && h->max_prefer_pop == 0 && !faithful &&
-                h->meta.taint_words == 1 && h->meta.static_words <= 1;
-  if (stream)
-    for (const ccsim_template &T : h->h_templates)
-      if (needs_extras(h, T) || T.n_pts || T.n_aff || T.n_anti) stream = false;
-  if (stream) {
-    free_pool(h, h->stream_allocs);
-    bool masks = false;
-    for (const ccsim_template &T : h->h_templates) {
-      uint64_t tb = 0;
-      if (T.filter_enable & CCSIM_PL_TAINT_TOLERATION) tb |= h->meta.taint_nosched[0] & ~T.tol_nosched[0] & ~(1ull << CCSIM_TAINT_UNSCHEDULABLE_BIT);
-      if ((T.filter_enable & CCSIM_PL_NODE_UNSCHEDULABLE) && !(T.flags & CCSIM_TF_TOLERATES_UNSCHEDULABLE)) tb |= 1ull << CCSIM_TAINT_UNSCHEDULABLE_BIT;
-      if (tb & h->taint_or0) masks = true;
-      if (h->meta.static_words > 0) {
-        if ((T.filter_enable & CCSIM_PL_NODE_AFFINITY) && (T.flags & CCSIM_TF_HAS_NODE_SELECTOR) && T.sel_mask[0]) masks = true;
-        if ((T.filter_enable & CCSIM_PL_NODE_PORTS) && (T.flags & CCSIM_TF_HAS_HOST_PORTS) && T.port_static_mask[0]) masks = true;
-        if ((T.filter_enable & CCSIM_PL_INTER_POD_AFFINITY) && T.existing_anti_mask[0]) masks = true;
-      }
-    }
-    sp.use_masks = masks ? 1 : 0;
-    sp.chunk_pad = ((p.chunk + STREAM_TILE - 1) / STREAM_TILE) * STREAM_TILE;
-    sp.tiles = sp.chunk_pad / STREAM_TILE;
-    sp.n_pad = (long long)grid * sp.chunk_pad;
-    int rc2;
-    unsigned long long *mt = nullptr, *mst = nullptr;
-    if ((rc2 = dev_alloc<long long>(h, h->stream_allocs, &sp.f_cpu, (size_t)sp.n_pad))) return rc2;
-    if ((rc2 = dev_alloc<long long>(h, h->stream_allocs, &sp.f_mem, (size_t)sp.n_pad))) return rc2;
-    if ((rc2 = dev_alloc<int32_t>(h, h->stream_allocs, &sp.f_pods, (size_t)sp.n_pad))) return rc2;
-    if (masks) {
-      if ((rc2 = dev_alloc<unsigned long long>(h, h->stream_allocs, &mt, (size_t)sp.n_pad))) return rc2;
-      if ((rc2 = dev_alloc<unsigned long long>(h, h->stream_allocs, &mst, (size_t)sp.n_pad))) return rc2;
-    }
-    sp.m_taint = mt; sp.m_static = mst;
-    if ((rc2 = dev_alloc<int32_t>(h, h->stream_allocs, &sp.memo, (size_t)sp.n_pad * h->n_templates))) return rc2;
-    CK(cudaMemsetAsync(sp.memo, 0xFF, (size_t)sp.n_pad * h->n_templates * 4, s));
-    ccsim_stream_prep_kernel<<<std::min<long long>(8LL * h->sm_count, (sp.n_pad + 255) / 256), 256, 0, s>>>(p, sp);
-    h->launches++;
-    CK(cudaGetLastError());
-    // resident free_* columns when the chunk fits next to the memo ring (24 B per node: up to ~7.8k nodes per SM)
-    sp.res_rows = (p.chunk + 31) & ~31;
-    const size_t smem_resf = (size_t)STREAM_STAGES_RES * STREAM_TILE * 4 + (size_t)sp.res_rows * 24 + 128;
-    stream_mode = masks ? 1 : ((smem_resf + sizeof(StreamShared) + 1024 <= h->smem_optin && sp.tiles <= STREAM_STAGES_RES && !getenv("CCSIM_STREAM_ALL")) ? 2 : 0);
-    kern = stream_mode == 1 ? (const void *)ccsim_wave_stream_kernel<1> : stream_mode == 2 ? (const void *)ccsim_wave_stream_kernel<2> : (const void *)ccsim_wave_stream_kernel<0>;
-    smem = stream_mode == 2 ? smem_resf : (size_t)STREAM_STAGES * STREAM_TILE * (masks ? 40 : 24) + 128;
-    block = STREAM_BLOCK;
-  }
-  p.self = h->d_params;
-  CK(cudaMemcpyAsync(h->d_params, &p, sizeof(DevParams), cudaMemcpyHostToDevice, s));
+  if (lean && !faithful && !batched) plan_multi(h, pl, k);
+  // 4. streaming waves when the lean tile is not taken
+  if (!lean && (rc = plan_stream(h, pl, k))) return rc;
+  // 5. the parameters, and the persistent grid must be co-resident
+  CK(cudaMemcpyAsync(h->d_params, &p, sizeof(DevParams), cudaMemcpyHostToDevice, h->stream));
   int occ = 0;
-  CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, block, smem));
-  if (occ < 1 || occ * h->sm_count < grid) return fail(h, CCSIM_ECUDA, "persistent grid %d does not fit (occupancy %d x %d SMs)", grid, occ, h->sm_count);
-  pl.p = p; pl.lp = lp; pl.mp = mp; pl.sp = sp; pl.kern = kern; pl.grid = grid; pl.block = block; pl.smem = smem;
-  pl.stream = stream; pl.multi = multi; pl.batched = batched; pl.lean = lean; pl.resident = resident;
-  pl.kernel_name = kernel_name_of(kern);
+  CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k->fn, k->block, pl.smem));
+  if (occ < 1 || occ * h->sm_count < p.grid) return fail(h, CCSIM_ECUDA, "persistent grid %d does not fit (occupancy %d x %d SMs)", p.grid, occ, h->sm_count);
+  pl.kern = k;
   pl.valid = true;
   return CCSIM_OK;
 }
@@ -1487,16 +1486,16 @@ extern "C" int ccsim_run(ccsim_handle *h, int64_t max_pods, ccsim_result *out) {
   const int32_t n = h->n;
   cudaStream_t s = h->stream;
   DevParams &p = pl.p; LeanParams &lp = pl.lp; MultiParams &mp = pl.mp; StreamParams &sp = pl.sp;
-  const void *kern = pl.kern; const int grid = pl.grid, block = pl.block; const size_t smem = pl.smem;
-  const bool stream = pl.stream, multi = pl.multi, batched = pl.batched, lean = pl.lean, resident = pl.resident;
-  (void)resident;      // read by the CCSIM_PHASE_TIMERS report only
+  const WaveKernel &k = *pl.kern;
+  const int grid = p.grid; const size_t smem = pl.smem;
+  const bool stream = k.engine == ENG_STREAM;
   void *args[] = { (void *)&p, stream ? (void *)&sp : (void *)&lp, (void *)&mp };
   CK(cudaEventRecord(h->ev0, s));
   // Cooperative launch = the driver guarantees that the whole persistent grid is co-resident (the kernels never use grid.sync()).
   // Ranks that share a process (ccsim_peer_import_local) may share a device; cooperative launches of different streams are not
   // run concurrently there, so those ranks use a plain launch: the occupancy check above still holds for each grid on its own.
-  if (h->peers_local) CK(cudaLaunchKernel(kern, dim3(grid), dim3(block), args, smem, s));
-  else CK(cudaLaunchCooperativeKernel(kern, dim3(grid), dim3(block), args, smem, s));
+  if (h->peers_local) CK(cudaLaunchKernel(k.fn, dim3(grid), dim3(k.block), args, smem, s));
+  else CK(cudaLaunchCooperativeKernel(k.fn, dim3(grid), dim3(k.block), args, smem, s));
   h->launches++;
   CK(cudaEventRecord(h->ev1, s));
   DevOut ho;
@@ -1515,7 +1514,7 @@ extern "C" int ccsim_run(ccsim_handle *h, int64_t max_pods, ccsim_result *out) {
     }
   }
 #ifdef CCSIM_PHASE_TIMERS
-  fprintf(stderr, "[ccsim %s tile %zu B smem] ", multi ? "multi" : batched ? "batched" : (lean ? "lean" : (resident ? "resident" : "streaming")), smem);
+  fprintf(stderr, "[ccsim %s tile %zu B smem] ", k.name, smem);
   fprintf(stderr, "[ccsim phases, CTA0 cycles/wave] scan=%.0f S1=%.0f publish=%.0f gather=%.0f commit=%.0f S2=%.0f (waves=%lld, %.3f ms)\n",
           (double)ho.phase_cycles[0] / ho.waves, (double)ho.phase_cycles[1] / ho.waves, (double)ho.phase_cycles[2] / ho.waves,
           (double)ho.phase_cycles[3] / ho.waves, (double)ho.phase_cycles[4] / ho.waves, (double)ho.phase_cycles[5] / ho.waves,
@@ -1523,8 +1522,8 @@ extern "C" int ccsim_run(ccsim_handle *h, int64_t max_pods, ccsim_result *out) {
   fprintf(stderr, "[ccsim phases 6/7] %.0f %.0f\n", (double)ho.phase_cycles[6] / ho.waves, (double)ho.phase_cycles[7] / ho.waves);
 #endif
   if (h->cfg.world > 1) h->xwave0 += (uint32_t)ho.waves;    // identical on every rank: the engines run the same waves everywhere
-  h->last_stat[0] = stream ? 4 : multi ? 3 : batched ? 2 : lean ? 1 : 0; h->last_stat[1] = ho.waves; h->last_stat[2] = ho.placed;
-  h->last_stat[3] = ho.stat[0]; h->last_stat[4] = ho.stat[1]; h->last_stat[5] = grid; h->last_stat[6] = block; h->last_stat[7] = (int64_t)smem;
+  h->last_stat[0] = k.engine; h->last_stat[1] = ho.waves; h->last_stat[2] = ho.placed;
+  h->last_stat[3] = ho.stat[0]; h->last_stat[4] = ho.stat[1]; h->last_stat[5] = grid; h->last_stat[6] = k.block; h->last_stat[7] = (int64_t)smem;
   for (int q = 0; q < 8; q++) h->last_stat[8 + q] = ho.phase_cycles[q];
   out->placed = ho.placed; out->stop_code = ho.stop_code; out->waves = ho.waves; out->evals = ho.evals; out->run_ms = ms;
   out->examined = ho.examined ? ho.examined : ho.evals;
@@ -1580,7 +1579,7 @@ extern "C" int ccsim_device_info(ccsim_handle *h, int32_t *sm_count, int32_t *gr
 
 extern "C" int64_t ccsim_kernel_launches(const ccsim_handle *h) { return h ? h->launches : 0; }
 
-extern "C" const char *ccsim_kernel_name(const ccsim_handle *h) { return h ? h->plan.kernel_name : ""; }
+extern "C" const char *ccsim_kernel_name(const ccsim_handle *h) { return h && h->plan.kern ? h->plan.kern->name : ""; }
 
 extern "C" int ccsim_run_stats(const ccsim_handle *h, int64_t out[16]) {
   if (!h || !out) return CCSIM_EINVAL;

@@ -1,6 +1,6 @@
 // ccsim_lean.cuh — the lean resident wave kernel: the common case of the hot path, written for latency.
 //
-// Eligibility (decided on the host, see ccsim_run): the CTA tiles fit in shared memory, one template, one taint word,
+// Eligibility (decided on the host, plan_lean): the CTA tiles fit in shared memory, one template, one taint word,
 // at most one static word, none of the "extras" predicates (extended resources, nodeAffinity terms, nodeName, hostPort
 // clones, ephemeral storage), every per-domain counter replicated in shared memory or node-local.
 // Everything else runs on the generic kernel (ccsim_wave_kernel) with identical results.

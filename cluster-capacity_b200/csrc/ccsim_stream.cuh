@@ -101,6 +101,12 @@ __global__ void ccsim_stream_prep_kernel(const DevParams p, const StreamParams s
   }
 }
 
+// Dynamic shared memory of ccsim_wave_stream_kernel<mode> as it carves it: NST stages of STAGE_BYTES, mode 2's 24-B rows, 128 B spare
+constexpr size_t stream_smem_bytes(int mode, size_t res_rows) {
+  return mode == 2 ? (size_t)STREAM_STAGES_RES * STREAM_TILE * 4 + res_rows * 24 + 128
+                   : (size_t)STREAM_STAGES * STREAM_TILE * (mode == 1 ? 40 : 24) + 128;
+}
+
 // MODE 0: everything streamed (24 B per node and wave); 1: + taint/static words (40 B); 2: the free_* columns of the CTA's chunk stay in
 // shared memory for the whole run (24 B per node, sized by the chunk rather than its tile padding: 1M nodes fit in the 132 SMs' shared
 // memory of an H100) and only the score memo column of the wave's template is streamed (4 B per node and wave)

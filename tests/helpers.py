@@ -99,11 +99,11 @@ def persistent_grid(n, sm_count, world=1):
 
 
 # ---- node-sharded ranks on one device -------------------------------------------------------------------------------
-def sharded_engines(snap, tmpl, ctr, world, kind):
+def sharded_engines(snap, tmpl, ctr, world, kind, **engine_kw):
     """`world` handles of this process on device 0 (rank r = the r-th), loaded and wired to each other by pointer
     (Engine.connect_local): the same in-kernel exchange as across GPUs, only the stores do not cross NVLink."""
     engine = importlib.import_module("cluster-capacity_b200.engine")
-    engs = [engine.Engine(device=0, engine=kind, rank=r, world=world) for r in range(world)]
+    engs = [engine.Engine(device=0, engine=kind, rank=r, world=world, **engine_kw) for r in range(world)]
     try:
         for e in engs:
             e.load_nodes(snap)
