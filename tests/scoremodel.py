@@ -7,8 +7,36 @@ classes in any taint word (tolerated ones excluded), NodeAffinity preferred term
 DefaultNormalizeScore(100, false)), the PodTopologySpread score on any topology column (podtopologyspread/scoring.go:60-265) and
 the InterPodAffinity score (interpodaffinity/scoring.go:236-290), with every counter updated per commit: spread counters only when
 the winner carries the counter's elig_bit, hostname counters always, InterPodAffinity counters by their signed increment.
-Not modelled (asserted absent): required (anti-)affinity, node selectors and required node-affinity terms, host ports, NoSchedule
-taints, and hard spread terms that could bind.
+The Filter runs every default-profile plugin per node, in the order of apis/config/v1/default_plugins.go:33-47, the first
+failing plugin deciding the node's status (framework/runtime/framework.go RunFilterPlugins):
+  1. the PreFilterResult node set (schedule_one.go:523-534: nodes outside it are UnschedulableAndUnresolvable);
+  2. NodeUnschedulable (nodeunschedulable/node_unschedulable.go:133-150; the node's spec.unschedulable is bit 63 of taint word 0,
+     which is no taint);
+  3. NodeName (nodename/node_name.go:72-83);
+  4. TaintToleration (tainttoleration/taint_toleration.go:111-122): NoSchedule and NoExecute taints in any taint word; the reason
+     names the first untolerated taint in node.Spec.Taints order (component-helpers/scheduling/corev1/helpers.go:78-86), the
+     lowest taint id when the snapshot carries no taint lists;
+  5. NodeAffinity (nodeaffinity/node_affinity.go:206-227): the selector's bits AND the OR of the required terms (zero terms
+     match nothing);
+  6. NodePorts (nodeports/node_ports.go:157-192): static conflicts, and clones of a conflicting template already on the node;
+  7. NodeResourcesFit (noderesources/fit.go:509-533, 564-654): every insufficient resource is a reason, the status is
+     UnschedulableAndUnresolvable iff some request exceeds the allocatable itself; "Too many pods" is always Unschedulable;
+  8. PodTopologySpread (podtopologyspread/filtering.go:311-356), per constraint in order: a node without the key is
+     UnschedulableAndUnresolvable; else cnt + self_match - min > maxSkew is Unschedulable, min being the minimum over the
+     present domains [0, n_present) (filtering.go:56-69, 98-137; MaxInt32 without one), 0 when min_zero (fewer domains than
+     minDomains). A node whose domain lies outside [0, n_present) reads its counter value, as the flat-struct contract of
+     the encoder states; the reference cannot reach that state, since a node that passes every filter has its domain counted,
+     and an uncounted domain reads 0 there (filtering.go:347);
+  9. InterPodAffinity (interpodaffinity/filtering.go:352-432), in the order of :419-429: the pod's required affinity (every key
+     present, every count > 0, or no matching pod in the cluster and the pod matching all its own terms: :382-408;
+     UnschedulableAndUnresolvable), its required anti-affinity (a node without the key passes: :367-379; Unschedulable), then
+     the existing pods' anti-affinity (:352-364; Unschedulable).
+FitError diagnosis (framework/types.go:787-838): the reason histogram over every node, and the preemption split
+(preemption/preemption.go:309-331): Unschedulable nodes are the candidates, of which none has a lower-priority victim ("No
+preemption victims found"); every other node is "Preemption is not helpful". Every counter moves per commit in exact Python ints,
+aff_total included (the pod's own affinity counts move only when it matches all its terms: filtering.go:234-271); the templates
+placed on each node are tracked for NodePorts.
+Not modelled: reference sampling below 100 %.
 
 PodTopologySpread, per cycle: the scored nodes are the feasible nodes outside IgnoredNodes (spts_ignored_bit; only explicit
 constraints ignore nodes, and then exactly the nodes that miss a constraint key). Per constraint w = go_log(size + 2), where size
@@ -24,8 +52,8 @@ Python / int64 values: where the engine's int32 counters could wrap, the model s
 
 exact=True swaps BalancedAllocation for rational arithmetic and the InterPodAffinity normalisation for integer arithmetic. Those
 are not what the reference computes: a test runs them only to prove that its inputs sit where the rounding decides the result.
-mutate=<name> (one of MUTATIONS) makes the soft path subtly wrong in one named way, for the same purpose: a test proves that its
-cases would notice a kernel with that defect.
+mutate=<name> (one of MUTATIONS or FILTER_MUTATIONS) makes the soft path or the Filter subtly wrong in one named way, for the
+same purpose: a test proves that its cases would notice a kernel with that defect.
 """
 import importlib
 from fractions import Fraction
@@ -48,6 +76,28 @@ MUTATIONS = (
     "commits_ignore_elig",     # spread counters incremented on every winner, whatever its elig_bit
     "ipa_inc_dropped",         # InterPodAffinity counters never incremented
 )
+
+FILTER_MUTATIONS = (
+    "skew_ge",                 # spread skew tested with >= instead of >
+    "min_all_domains",         # spread minimum over every domain instead of the present ones
+    "min_zero_ignored",        # spread minimum taken over the domains even when fewer than minDomains exist
+    "self_match_one",          # spread self_match taken as 1
+    "missing_key_as_skew",     # a node without a spread key counted as a skew failure (Unschedulable)
+    "aff_bypass_never",        # the first-pod affinity bypass never applies
+    "aff_bypass_sticky",       # ... outlives the first clone (aff_total never moves)
+    "anti_missing_key_fails",  # anti-affinity fails a node without the term's key
+    "taint_bit_order",         # the first untolerated taint in taint-id order instead of Spec order
+    "fit_first_reason",        # only the first insufficient resource kept as a reason
+    "fit_all_unschedulable",   # every NodeResourcesFit failure Unschedulable
+    "ports_after_fit",         # NodePorts checked after NodeResourcesFit
+    "ports_cross_template",    # clones of other templates never conflict on a host port
+    "hostname_anti_frozen",    # hostname anti-affinity counters never incremented
+    "diag_ptsmin_stale",       # the FitError diagnosis reads the spread minimum of the last placing cycle, not the failing one
+)
+
+UNSCHEDULABLE, UNRESOLVABLE = 1, 2       # status codes (kube-scheduler framework/interface.go)
+MAX_INT32 = 2 ** 31 - 1
+U64 = (1 << 64) - 1
 
 
 def go_div(a, b):
@@ -151,7 +201,7 @@ def _edge_kind(raw, mx):
 
 # ---- the sequential loop -------------------------------------------------------------------------------------------------
 class Result:
-    def __init__(self, pod_node, stop_code, reason_hist, ipa_edges, preempt=(0, 0), soft=None):
+    def __init__(self, pod_node, stop_code, reason_hist, ipa_edges, preempt=(0, 0), soft=None, hard=None):
         self.pod_node = np.asarray(pod_node, np.int32)
         self.placed = len(self.pod_node)
         self.stop_code = stop_code
@@ -161,24 +211,17 @@ class Result:
         # what the soft path met, for the generator guards: spread sizes per cycle, truncation edges of the NodeAffinity and
         # PodTopologySpread normalisations ("at" / "below" a multiple of max), cycles where max == 0, cycles without a scored node
         self.soft = soft or {}
+        # what the Filter met, for the generator guards: edge name -> number of cycles (or nodes at the terminal cycle) that met it
+        self.hard = hard or {}
 
 
 def _bit(snap, b):
     return ((snap.static_mask[b >> 6] >> np.uint64(b & 63)) & np.uint64(1)).astype(bool)
 
 
-def _check_supported(snap, tmpl, ctr, bound):
+def _check_supported(snap, tmpl, ctr):
     for t in tmpl:
-        assert t.n_aff == 0 and t.n_anti == 0 and t.nodename_idx < 0, "not modelled"
-        assert not (t.flags & (abi.TF_HAS_NODE_SELECTOR | abi.TF_HAS_AFFINITY_TERMS | abi.TF_HAS_HOST_PORTS | abi.TF_PREFILTER_NODES
-                               | abi.TF_FIT_ALL_ZERO)), "not modelled"
-        assert t.req_eph == 0 and t.least_cpu == t.nz_cpu and t.least_mem == t.nz_mem, "not modelled"
-        assert all(int(t.tol_nosched[w]) == 0 for w in range(snap.taint_words)), "not modelled"
-        for c in range(t.n_pts):      # hard spread terms must never bind (skew <= max count + clones * inc + 1): the model has no such filter
-            cc = ctr[t.pts[c].counter]
-            init = np.asarray(cc._keep, np.int64)
-            assert t.pts[c].max_skew > int(init.max(initial=0)) + bound * abs(cc.inc) + 1, "binding spread term"
-            assert cc.topo_col >= 0 and int(snap.topo[cc.topo_col].min(initial=0)) >= 0, "not modelled: a node without a hard spread key"
+        assert t.least_cpu == t.nz_cpu and t.least_mem == t.nz_mem, "not modelled"
         if t.spts_ignored_bit >= 0 and t.n_spts:      # explicit constraints: IgnoredNodes are exactly the nodes that miss a key
             missing = np.zeros(snap.n, bool)
             for c in range(t.n_spts):
@@ -189,27 +232,46 @@ def _check_supported(snap, tmpl, ctr, bound):
                 else:
                     missing |= snap.topo[ctr[sc.counter].topo_col] < 0
             assert np.array_equal(missing, _bit(snap, t.spts_ignored_bit)), "IgnoredNodes must be the nodes that miss a key"
-    assert all(int(m) == 0 for m in snap.taint_nosched), "not modelled"
+
+
+def _covers(snap, idx, masks):
+    """Per node of idx: every bit of masks (one uint64 per static word) is set on the node; a word the snapshot lacks is 0."""
+    ok = np.ones(len(idx), bool)
+    for w in range(abi.MAX_STATIC_WORDS):
+        m = int(masks[w])
+        if m:
+            ok &= (snap.static_mask[w][idx] & np.uint64(m)) == np.uint64(m) if w < snap.static_words else False
+    return ok
+
+
+def _meets(snap, idx, masks):
+    """Per node of idx: some bit of masks is set on the node."""
+    hit = np.zeros(len(idx), bool)
+    for w in range(snap.static_words):
+        if int(masks[w]):
+            hit |= (snap.static_mask[w][idx] & np.uint64(int(masks[w]))) != 0
+    return hit
 
 
 def run(snap, tmpl, ctr=(), max_pods=0, exact=False, mutate=None):
     """The schedule-one-pod-then-update loop (schedule_one.go) over the modelled plugins. Pod k is a clone of template k % len(tmpl);
     the highest total among the feasible nodes wins, ties go to the lowest index."""
-    assert mutate is None or mutate in MUTATIONS, mutate
+    assert mutate is None or mutate in MUTATIONS + FILTER_MUTATIONS, mutate
     n = snap.n
-    bound = int(np.maximum(snap.alloc_pods.astype(np.int64) - snap.npods, 0).sum())
-    if max_pods:
-        bound = min(bound, max_pods)
-    _check_supported(snap, tmpl, ctr, bound)
+    _check_supported(snap, tmpl, ctr)
     a_cpu, a_mem = [int(x) for x in snap.alloc_cpu], [int(x) for x in snap.alloc_mem]
     r_cpu, r_mem = [int(x) for x in snap.req_cpu], [int(x) for x in snap.req_mem]
     z_cpu, z_mem = [int(x) for x in snap.nz_cpu], [int(x) for x in snap.nz_mem]
     free_cpu = snap.alloc_cpu - snap.req_cpu
     free_mem = snap.alloc_mem - snap.req_mem
+    free_eph = snap.alloc_eph - snap.req_eph
     free_pods = snap.alloc_pods.astype(np.int64) - snap.npods
     free_sc = [a - r for a, r in snap.scalars]
     cnt = [np.asarray(c._keep, np.int64).copy() for c in ctr]      # exact counts: the reference's are int64
+    aff_total = int(tmpl[0].aff_total_init)                        # pods matching the pod's required affinity terms, cluster-wide
+    placed = [0] * n                                               # bit q: a clone of template q sits on the node
     ipa_counters = {int(t.ipa_score_counter[k]) for t in tmpl for k in range(t.n_ipa_score)}
+    anti_host = {int(t.anti_counter[a]) for t in tmpl for a in range(t.n_anti) if ctr[t.anti_counter[a]].topo_col < 0}
 
     def local(t, i):
         s = 0
@@ -220,36 +282,159 @@ def run(snap, tmpl, ctr=(), max_pods=0, exact=False, mutate=None):
             s += t.w_balanced * balanced((a_cpu[i], a_mem[i]), (r_cpu[i] + t.bal_cpu, r_mem[i] + t.bal_mem), exact)
         return s
 
-    live = np.nonzero(free_pods >= 1)[0]          # free pods only shrink: the other nodes are never feasible
+    # free pods only shrink: while NodeResourcesFit filters, the other nodes are never feasible
+    fit_all = all(t.filter_enable & abi.PL_FIT for t in tmpl)
+    live = np.nonzero(free_pods >= 1)[0] if fit_all else np.arange(n)
 
-    def feasible(t):
-        ok = free_pods[live] >= 1
-        if t.req_cpu > 0:
-            ok &= free_cpu[live] >= t.req_cpu
-        if t.req_mem > 0:
-            ok &= free_mem[live] >= t.req_mem
-        for k, f in enumerate(free_sc):
-            if t.req_scalar[k]:
-                ok &= f[live] >= t.req_scalar[k]
-        return live[ok]
+    def domain(j, idx):
+        return idx if ctr[j].topo_col < 0 else snap.topo[ctr[j].topo_col][idx]
 
-    def reasons(t):
-        """FitError histogram and preemption counts: NodeResourcesFit fails on every node (status Unschedulable unless a request
-        exceeds the allocatable itself: UnschedulableAndUnresolvable, fit.go:564-660)."""
+    def count(j, dom):
+        return np.where(dom >= 0, cnt[j][np.maximum(dom, 0)], 0)
+
+    def pts_min(t):
+        """Per hard spread constraint: the critical path's count (filtering.go:56-69, 98-137)."""
+        out = []
+        for c in range(t.n_pts):
+            p = t.pts[c]
+            if p.min_zero and mutate != "min_zero_ignored":
+                out.append(0)
+                continue
+            hi = ctr[p.counter].n_domains if mutate == "min_all_domains" else ctr[p.counter].n_present
+            out.append(int(cnt[p.counter][:hi].min()) if hi > 0 else MAX_INT32)
+        return out
+
+    def first_taint(t, i):
+        """The first untolerated NoSchedule / NoExecute taint of node i (helpers.go:78-86)."""
+        if snap.taint_list_off is not None and mutate != "taint_bit_order":
+            for tid in snap.taint_list[snap.taint_list_off[i]:snap.taint_list_off[i + 1]]:
+                w, b = int(tid) >> 6, int(tid) & 63
+                if (int(snap.taint_nosched[w]) >> b) & 1 and not (int(t.tol_nosched[w]) >> b) & 1:
+                    return int(tid)
+        for w in range(snap.taint_words):
+            m = int(snap.taint_mask[w][i]) & untol_mask(t, w)
+            if m:
+                return 64 * w + (m & -m).bit_length() - 1
+        raise AssertionError("no untolerated taint")
+
+    def untol_mask(t, w):
+        m = int(snap.taint_nosched[w]) & ~int(t.tol_nosched[w]) & U64
+        return m & ~(1 << abi.TAINT_UNSCHEDULABLE_BIT) if w == 0 else m
+
+    def filt(t, ti, idx, ptsmin, diag=False, seen=None):
+        """Status per node of idx (0: passes), first failing plugin wins; with diag also the FitError reasons."""
+        st = np.zeros(len(idx), np.int8)
         hist = np.zeros(abi.R_TOTAL, np.int64)
-        hist[abi.R_TOO_MANY_PODS] = int((free_pods < 1).sum())
-        unres = np.zeros(n, bool)
-        if t.req_cpu > 0:
-            hist[abi.R_INSUFFICIENT_CPU] = int((free_cpu < t.req_cpu).sum())
-            unres |= snap.alloc_cpu < t.req_cpu
-        if t.req_mem > 0:
-            hist[abi.R_INSUFFICIENT_MEMORY] = int((free_mem < t.req_mem).sum())
-            unres |= snap.alloc_mem < t.req_mem
-        for k, f in enumerate(free_sc):
-            if t.req_scalar[k]:
-                hist[abi.R_SCALAR0 + k] = int((f < t.req_scalar[k]).sum())
-                unres |= snap.scalars[k][0] < t.req_scalar[k]
-        return hist, (n - int(unres.sum()), int(unres.sum()))
+        fe = t.filter_enable
+
+        def fail(bad, status, reason=None):
+            bad = bad & (st == 0)
+            st[bad] = status
+            if reason is not None:
+                hist[reason] += int(bad.sum())
+            return bad
+
+        def ports():
+            if (fe & abi.PL_NODE_PORTS) and (t.flags & abi.TF_HAS_HOST_PORTS):
+                conflict = int(t.port_tmpl_conflict) & (1 << ti if mutate == "ports_cross_template" else U64)
+                mine = np.array([placed[i] & conflict != 0 for i in idx], bool) if conflict else np.zeros(len(idx), bool)
+                fail(_meets(snap, idx, t.port_static_mask) | mine, UNSCHEDULABLE, abi.R_NODE_PORTS)
+
+        if (t.flags & abi.TF_PREFILTER_NODES) and t.prefilter_bit >= 0:
+            fail(~_bit(snap, t.prefilter_bit)[idx], UNRESOLVABLE, abi.R_PREFILTER_NODES)
+        if (fe & abi.PL_NODE_UNSCHEDULABLE) and not (t.flags & abi.TF_TOLERATES_UNSCHEDULABLE):
+            fail((snap.taint_mask[0][idx] >> np.uint64(abi.TAINT_UNSCHEDULABLE_BIT)) & np.uint64(1) != 0, UNRESOLVABLE, abi.R_UNSCHEDULABLE)
+        if (fe & abi.PL_NODE_NAME) and t.nodename_idx >= 0:
+            fail(idx != t.nodename_idx, UNRESOLVABLE, abi.R_NODE_NAME)
+        if fe & abi.PL_TAINT_TOLERATION:
+            untol = np.zeros(len(idx), bool)
+            for w in range(snap.taint_words):
+                untol |= (snap.taint_mask[w][idx] & np.uint64(untol_mask(t, w))) != 0
+            bad = fail(untol, UNRESOLVABLE)
+            if diag:
+                for i in idx[bad]:
+                    hist[abi.R_TAINT0 + first_taint(t, int(i))] += 1
+        if (fe & abi.PL_NODE_AFFINITY) and (t.flags & (abi.TF_HAS_NODE_SELECTOR | abi.TF_HAS_AFFINITY_TERMS)):
+            ok = _covers(snap, idx, t.sel_mask)
+            if t.flags & abi.TF_HAS_AFFINITY_TERMS:
+                any_term = np.zeros(len(idx), bool)
+                for k in range(t.n_aff_terms):
+                    any_term |= _covers(snap, idx, t.aff_term_mask[k])
+                ok &= any_term
+            fail(~ok, UNRESOLVABLE, abi.R_NODE_AFFINITY)
+        if mutate != "ports_after_fit":
+            ports()
+        if fe & abi.PL_FIT:
+            rs = [(free_pods[idx] < 1, abi.R_TOO_MANY_PODS, np.zeros(len(idx), bool))]
+            for q, free, alloc, r in ((t.req_cpu, free_cpu, snap.alloc_cpu, abi.R_INSUFFICIENT_CPU),
+                                      (t.req_mem, free_mem, snap.alloc_mem, abi.R_INSUFFICIENT_MEMORY),
+                                      (t.req_eph, free_eph, snap.alloc_eph, abi.R_INSUFFICIENT_EPHEMERAL)):
+                if q > 0:
+                    rs.append((free[idx] < q, r, alloc[idx] < q))
+            for k, f in enumerate(free_sc):
+                q = int(t.req_scalar[k])
+                if q:
+                    rs.append((f[idx] < q, abi.R_SCALAR0 + k, snap.scalars[k][0][idx] < q))
+            open_ = st == 0
+            bad, unres, first = np.zeros(len(idx), bool), np.zeros(len(idx), bool), np.zeros(len(idx), bool)
+            for short, r, beyond in rs:
+                counted = short & open_ & ~first if mutate == "fit_first_reason" else short & open_
+                hist[r] += int(counted.sum())
+                first |= short
+                bad |= short
+                unres |= short & beyond
+            if mutate == "fit_all_unschedulable":
+                unres[:] = False
+            fail(bad & unres, UNRESOLVABLE)
+            fail(bad, UNSCHEDULABLE)
+        if mutate == "ports_after_fit":
+            ports()
+        if fe & abi.PL_POD_TOPOLOGY_SPREAD:
+            for c in range(t.n_pts):
+                p = t.pts[c]
+                dom = domain(p.counter, idx)
+                missing = dom < 0
+                if seen is not None:
+                    seen["missing_key"] += bool((missing & (st == 0)).any())
+                if mutate == "missing_key_as_skew":
+                    fail(missing, UNSCHEDULABLE, abi.R_PTS_SKEW)
+                else:
+                    fail(missing, UNRESOLVABLE, abi.R_PTS_MISSING_LABEL)
+                skew = count(p.counter, dom) + (1 if mutate == "self_match_one" else p.self_match) - ptsmin[c]
+                over = skew >= p.max_skew if mutate == "skew_ge" else skew > p.max_skew
+                if seen is not None:
+                    open_ = (st == 0) & ~missing
+                    seen["skew_at_max"] += bool((open_ & (skew == p.max_skew)).any())
+                    seen["skew_one_over"] += bool((open_ & (skew == p.max_skew + 1)).any())
+                    seen["outside_present"] += bool((open_ & (dom >= ctr[p.counter].n_present)).any())
+                fail(~missing & over, UNSCHEDULABLE, abi.R_PTS_SKEW)
+        if fe & abi.PL_INTER_POD_AFFINITY:
+            if t.n_aff:
+                missing, exist = np.zeros(len(idx), bool), np.ones(len(idx), bool)
+                for a in range(t.n_aff):
+                    dom = domain(t.aff_counter[a], idx)
+                    missing |= dom < 0
+                    exist &= count(t.aff_counter[a], dom) > 0
+                bypass = aff_total == 0 and bool(t.flags & abi.TF_AFF_SELF_MATCH_ALL) and mutate != "aff_bypass_never"
+                if seen is not None and bypass:
+                    seen["bypass"] += 1
+                fail(missing | (~exist & (not bypass)), UNRESOLVABLE, abi.R_IPA_AFFINITY)
+            for a in range(t.n_anti):
+                dom = domain(t.anti_counter[a], idx)
+                bad = count(t.anti_counter[a], dom) > 0
+                if seen is not None:
+                    seen["anti_missing_key"] += bool(((dom < 0) & (st == 0)).any())
+                fail(bad | (dom < 0) if mutate == "anti_missing_key_fails" else bad, UNSCHEDULABLE, abi.R_IPA_ANTI_AFFINITY)
+            fail(_meets(snap, idx, t.existing_anti_mask), UNSCHEDULABLE, abi.R_IPA_EXISTING_ANTI)
+        return st, hist
+
+    def reasons(t, ti, ptsmin):
+        """FitError histogram over every node, and the preemption split: Unschedulable nodes are preemption candidates without
+        lower-priority victims, every other node is "not helpful" (preemption.go:262-277, 309-331)."""
+        st, hist = filt(t, ti, np.arange(n), ptsmin, diag=True)
+        assert not (st == 0).any()
+        unsched = int((st == UNSCHEDULABLE).sum())
+        return hist, (unsched, n - unsched)
 
     cache, img, prefer, na_raw, ignored = [], [], [], [], []
     for t in tmpl:
@@ -330,15 +515,26 @@ def run(snap, tmpl, ctr=(), max_pods=0, exact=False, mutate=None):
         return out
 
     soft = {"sizes": [], "no_scored": 0, "pts_max0": 0, "na_max0": 0, "pts_edges": set(), "na_edges": set()}
+    hard = dict.fromkeys(("skew_at_max", "skew_one_over", "missing_key", "outside_present", "min_zero_above", "min_moved_last",
+                          "bypass", "bypass_ended", "anti_missing_key"), 0)
     pod_node, ipa_edges = [], set()
     k = 0
+    last_min = None
     while True:
         ti = k % len(tmpl)
         t = tmpl[ti]
-        feas = feasible(t)
+        ptsmin = pts_min(t)
+        for c in range(t.n_pts):
+            p = t.pts[c]
+            hard["min_zero_above"] += bool(p.min_zero and ctr[p.counter].n_present > 0
+                                           and int(cnt[p.counter][:ctr[p.counter].n_present].min()) > 0)
+        st, _ = filt(t, ti, live, ptsmin, seen=hard)
+        feas = live[st == 0]
         if len(feas) == 0:
-            hist, preempt = reasons(t)
-            return Result(pod_node, abi.STOP_UNSCHEDULABLE, hist, ipa_edges, preempt, soft)
+            hard["min_moved_last"] = int(last_min is not None and last_min != ptsmin)
+            hist, preempt = reasons(t, ti, last_min if mutate == "diag_ptsmin_stale" and last_min is not None else ptsmin)
+            return Result(pod_node, abi.STOP_UNSCHEDULABLE, hist, ipa_edges, preempt, soft, hard)
+        last_min = ptsmin
         total = cache[ti][feas].copy()
         if t.score_enable & abi.PL_TAINT_TOLERATION:
             total += t.w_taint * taint_norm(prefer[ti][feas])
@@ -372,22 +568,32 @@ def run(snap, tmpl, ctr=(), max_pods=0, exact=False, mutate=None):
         z_mem[w] += t.nz_mem
         free_cpu[w] -= t.req_cpu
         free_mem[w] -= t.req_mem
+        free_eph[w] -= t.req_eph
         free_pods[w] -= 1
+        if free_pods[w] < 1 and fit_all:
+            live = live[live != w]
+        placed[w] |= 1 << ti
         for q, f in enumerate(free_sc):
             f[w] -= t.req_scalar[q]
         for q, tq in enumerate(tmpl):
             cache[q][w] = local(tq, w)
-        for j, c in enumerate(ctr):      # the next cycle's PreScore recount sees this clone
-            if c.inc == 0 or (mutate == "ipa_inc_dropped" and j in ipa_counters):
+        aff = {int(t.aff_counter[a]) for a in range(t.n_aff)}
+        for j, c in enumerate(ctr):      # the next cycle's PreFilter / PreScore recount sees this clone
+            if c.inc == 0 or (mutate == "ipa_inc_dropped" and j in ipa_counters) or (mutate == "hostname_anti_frozen" and j in anti_host):
                 continue
+            if j in aff and not (t.flags & abi.TF_AFF_SELF_MATCH_ALL):
+                continue          # the clone matches its own affinity terms only if it matches all of them (filtering.go:124-130, 187-199)
             if c.elig_bit >= 0 and mutate != "commits_ignore_elig" and not _bit(snap, c.elig_bit)[w]:
                 continue
             dom = w if c.topo_col < 0 else int(snap.topo[c.topo_col][w])
             if dom >= 0:
                 cnt[j][dom] += c.inc
+                if j in aff and mutate != "aff_bypass_sticky":
+                    hard["bypass_ended"] += aff_total == 0
+                    aff_total += c.inc
         k += 1
         if max_pods and k >= max_pods:
-            return Result(pod_node, abi.STOP_LIMIT_REACHED, np.zeros(abi.R_TOTAL, np.int64), ipa_edges, soft=soft)
+            return Result(pod_node, abi.STOP_LIMIT_REACHED, np.zeros(abi.R_TOTAL, np.int64), ipa_edges, soft=soft, hard=hard)
 
 
 # ---- fp32 emulations of the kernels' screens (generator guards only) ----------------------------------------------------------
