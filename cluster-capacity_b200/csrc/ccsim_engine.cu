@@ -1521,6 +1521,21 @@ extern "C" int ccsim_run(ccsim_handle *h, int64_t max_pods, ccsim_result *out) {
           (long long)ho.waves, ms);
   fprintf(stderr, "[ccsim phases 6/7] %.0f %.0f\n", (double)ho.phase_cycles[6] / ho.waves, (double)ho.phase_cycles[7] / ho.waves);
 #endif
+#ifdef MULTI_GATHER_PROFILE
+  if (k.engine == ENG_MULTI && ho.waves > 0) {     // skew of the publishes per wave on the clock all SMs share: latest CTA minus CTA 0
+    const long long nw = std::min<long long>(ho.waves, GP_MAX_WAVES);
+    std::vector<long long> t((size_t)nw * CCSIM_MAX_GRID), skew((size_t)nw);
+    CK(cudaMemcpyFromSymbol(t.data(), gp_pub_ns, t.size() * sizeof(long long)));
+    for (long long w = 0; w < nw; w++) {
+      long long mx = t[(size_t)w * CCSIM_MAX_GRID];
+      for (int c = 1; c < grid; c++) mx = std::max(mx, t[(size_t)w * CCSIM_MAX_GRID + c]);
+      skew[(size_t)w] = mx - t[(size_t)w * CCSIM_MAX_GRID];
+    }
+    std::sort(skew.begin(), skew.end());
+    fprintf(stderr, "gather profile: publish skew (latest CTA - CTA 0, %%globaltimer) over %lld waves: median %lld ns, max %lld ns\n",
+            nw, skew[(size_t)nw / 2], skew.back());
+  }
+#endif
   if (h->cfg.world > 1) h->xwave0 += (uint32_t)ho.waves;    // identical on every rank: the engines run the same waves everywhere
   h->last_stat[0] = k.engine; h->last_stat[1] = ho.waves; h->last_stat[2] = ho.placed;
   h->last_stat[3] = ho.stat[0]; h->last_stat[4] = ho.stat[1]; h->last_stat[5] = grid; h->last_stat[6] = k.block; h->last_stat[7] = (int64_t)smem;

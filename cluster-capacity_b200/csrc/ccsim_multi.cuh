@@ -93,6 +93,27 @@ static_assert(4 + 2 * MULTI_CAP <= CCSIM_MAX_GRID * SLOT_STRIDE, "node shards: a
 #define RP_ADD(i, cyc, n) do { } while (0)
 #endif
 
+// Gather profile (profiling builds only: -DMULTI_GATHER_PROFILE; the hooks expand to nothing otherwise). CTA 0 adds up, per wave:
+// the cycles from its own publish to the poll round in which the last of its entries was valid (the latest of its threads), and
+// the number of poll rounds (the most any thread took); from there to the point where the CTA may read every entry (G1); the
+// first append pass up to G2; the bar-raise path (histogram, raise, second pass) and how often it ran. Every CTA also writes its
+// %globaltimer at publish into gp_pub_ns[wave][CTA]; the host reports the skew of the publishes, latest minus CTA 0's, per wave.
+// scripts/gather_profile.sh prints both.
+#define GP_POLL 0
+#define GP_SYNC 1
+#define GP_APPEND 2
+#define GP_RAISE 3
+#define GP_ROUNDS 4               /* (event count only) */
+#define GP_N 5
+#define GP_MAX_WAVES 4096         /* waves with a publish time */
+#ifdef MULTI_GATHER_PROFILE
+#define GPROF(...) __VA_ARGS__
+__device__ long long gp_pub_ns[GP_MAX_WAVES * CCSIM_MAX_GRID];
+__device__ __forceinline__ long long globaltimer_ns() { long long t; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t)); return t; }
+#else
+#define GPROF(...)
+#endif
+
 // cross-GPU line buffers inside every rank's exchange allocation (64-bit words): [parity][source rank][CTA][16]
 #define XLEAN_WORDS (2 * CCSIM_MAX_WORLD * SLOT_STRIDE)
 #define XLINES_OFF XLEAN_WORDS
@@ -120,6 +141,10 @@ struct __align__(16) MultiShared {
   long long ph[8], tc0, st_cand, st_overflow, st_rounds;       // CTA 0 / thread 0: clock cycles per phase, replay statistics
 #ifdef MULTI_ROUND_PROFILE
   long long rp_cyc[RP_N], rp_cnt[RP_N], rp_t;                  // CTA 0's replay warp: cycles and events per part of the replay
+#endif
+#ifdef MULTI_GATHER_PROFILE
+  unsigned long long gp_valid, gp_spins;                       // CTA 0, this wave: latest clock at which a thread's entries were all valid, most poll rounds
+  long long gp_pub, gp_cyc[GP_N], gp_cnt[GP_N];                // CTA 0: its publish clock; cycles and events per part of the gather
 #endif
 };
 
@@ -170,20 +195,30 @@ __device__ __forceinline__ void multi_append(bool keep, uint32_t ck, unsigned lo
 }
 
 // More candidates than the replay holds: the bar T is raised to the lowest of MULTI_BINS equal steps between T and the best key
-// that leaves <= MULTI_CAP candidates; every CTA sees the same data and decides alike. The caller counts its candidates into
-// ms.hist with multi_hist_add; multi_raise_bar returns the new T with the candidate arrays emptied (all threads, two barriers).
+// that leaves <= MULTI_CAP candidates; every CTA sees the same data and decides alike. The caller zeroes ms.hist; after a barrier
+// it counts its candidates into it with multi_hist_add and empties the candidate arrays (multi_bar_reset: every thread has read
+// ms.ncand before that barrier); after one more barrier multi_raise_bar returns the new T. Every warp computes it alike from the
+// histogram, so no barrier follows: the next write of ms.hist or ms.ncand is behind the barrier that ends the second append pass.
 __device__ __forceinline__ void multi_hist_add(uint32_t ck, uint32_t T, unsigned long long range) {
   if (ck != 0u && ck >= T) atomicAdd(&ms.hist[(unsigned)(((unsigned long long)(ck - T) * MULTI_BINS) / range)], 1u);
 }
-__device__ __forceinline__ uint32_t multi_raise_bar(uint32_t T, uint32_t kbest, unsigned long long range, int cta) {
-  int bsel = MULTI_BINS;
-  { unsigned sum = 0; for (int bq = MULTI_BINS - 1; bq >= 0; bq--) { sum += ms.hist[bq]; if (sum > (unsigned)MULTI_CAP) break; bsel = bq; } }
-  T = (bsel >= MULTI_BINS) ? kbest : T + (uint32_t)(((unsigned long long)bsel * range + (MULTI_BINS - 1)) / MULTI_BINS);
-  __syncthreads();
+__device__ __forceinline__ void multi_bar_reset(int cta) {
   if (threadIdx.x == 0) ms.ncand = 0;
   if (cta == 0 && threadIdx.x == 0) ms.st_overflow++;
-  __syncthreads();
-  return T;
+}
+static_assert(MULTI_BINS == 64, "multi_raise_bar: two histogram bins per lane");
+__device__ __forceinline__ uint32_t multi_raise_bar(uint32_t T, uint32_t kbest, unsigned long long range) {
+  // suf(b) = the candidates in bins >= b does not grow with b, so the lowest bin with suf(b) <= MULTI_CAP is the number of bins
+  // with suf(b) > MULTI_CAP (MULTI_BINS when even the top bin holds more: the bar goes to the best key). Lane l holds bins 2l and
+  // 2l + 1; a suffix sum over the lanes gives suf(2l), and suf(2l + 1) = suf(2l) - hist[2l]. (Every thread used to walk down the
+  // 64 bins one by one, a compare and a branch per bin, and two more block barriers followed.)
+  const int lane = threadIdx.x & 31;
+  const uint32_t h0 = ms.hist[2 * lane], h1 = ms.hist[2 * lane + 1];
+  uint32_t suf = h0 + h1;
+  #pragma unroll
+  for (int o = 1; o < 32; o <<= 1) { const uint32_t v = __shfl_down_sync(0xffffffffu, suf, o); if (lane + o < 32) suf += v; }
+  const int bsel = __popc(__ballot_sync(0xffffffffu, suf > (uint32_t)MULTI_CAP)) + __popc(__ballot_sync(0xffffffffu, suf - h0 > (uint32_t)MULTI_CAP));
+  return (bsel >= MULTI_BINS) ? kbest : T + (uint32_t)(((unsigned long long)bsel * range + (MULTI_BINS - 1)) / MULTI_BINS);
 }
 
 // phase timers live in shared memory (thread 0 of CTA 0 only): registers are what this kernel is short of
@@ -210,7 +245,8 @@ __global__ void __launch_bounds__(LEAN_THREADS, 1) ccsim_wave_multi_kernel(const
   if (tid == 0) { ms.accepted = 0; ms.dead = 0; ms.stopb = 0; ms.n_gt = 0; ms.ncand = 0; ms.delta = 1u << MULTI_IDX_BITS; ms.force_strict = 0; ms.st_relaxed = 0; ms.st_empty = 0;
                   for (int q = 0; q < LEAN_MAX_TERMS; q++) ms.relax[q] = 0;
                   for (int q = 0; q < 8; q++) ms.ph[q] = 0; ms.tc0 = 0; ms.st_cand = 0; ms.st_overflow = 0; ms.st_rounds = 0;
-                  RPROF(for (int q = 0; q < RP_N; q++) ms.rp_cyc[q] = ms.rp_cnt[q] = 0; ms.rp_t = 0;) }
+                  RPROF(for (int q = 0; q < RP_N; q++) ms.rp_cyc[q] = ms.rp_cnt[q] = 0; ms.rp_t = 0;)
+                  GPROF(for (int q = 0; q < GP_N; q++) ms.gp_cyc[q] = ms.gp_cnt[q] = 0; ms.gp_valid = ms.gp_spins = 0ull; ms.gp_pub = 0;) }
   ms.mult[tid] = 0;
   lean_stage(p, lp, t, lo, cnt_nodes);
   for (int c = 0; c < ls.tmpl.n_pts; c++) lean_pts_recount(p, smem_cnt, c);
@@ -354,6 +390,7 @@ __global__ void __launch_bounds__(LEAN_THREADS, 1) ccsim_wave_multi_kernel(const
           st_slot(&myslots[SLOT_STRIDE + lane], pay | tagbits);
         }
       }
+      GPROF(if (lane == 0) { if (cta == 0) ms.gp_pub = clock64(); if (wv < GP_MAX_WAVES) gp_pub_ns[wv * CCSIM_MAX_GRID + cta] = globaltimer_ns(); })
     }
     MPH_MARK(2);
     // ---- gather, level 1: the lines of THIS GPU's CTAs. Every thread waits for its own (<= MULTI_EPT) entries — key word and payload
@@ -385,6 +422,7 @@ __global__ void __launch_bounds__(LEAN_THREADS, 1) ccsim_wave_multi_kernel(const
           break;
         }
       }
+      GPROF(if (cta == 0) { atomicMax(&ms.gp_valid, (unsigned long long)clock64()); atomicMax(&ms.gp_spins, (unsigned long long)spins); })
       #pragma unroll
       for (int u = 0; u < MULTI_EPT; u++) {
         const int e = tid + u * LEAN_THREADS, ee = e & (MULTI_M - 1);
@@ -401,6 +439,12 @@ __global__ void __launch_bounds__(LEAN_THREADS, 1) ccsim_wave_multi_kernel(const
     uint32_t Tlist = __reduce_max_sync(0xffffffffu, lane < LEAN_WARPS ? ms.red[lane] : 0u);
     uint32_t kbest = __reduce_max_sync(0xffffffffu, lane < LEAN_WARPS ? ms.red2[lane] : 0u);
     bool dead = ms.dead != 0;
+    GPROF(long long gp_t = 0;
+          if (cta == 0 && tid == 0) {
+            gp_t = clock64();
+            ms.gp_cyc[GP_POLL] += (long long)ms.gp_valid - ms.gp_pub; ms.gp_cyc[GP_SYNC] += gp_t - (long long)ms.gp_valid;
+            ms.gp_cnt[GP_ROUNDS] += (long long)ms.gp_spins; ms.gp_valid = ms.gp_spins = 0ull;
+          })
     // The replay bar: T = the largest "last key" of a list whose tile has unseen feasible nodes is the lowest VALID bar; any
     // higher bar is valid too, just more conservative. The replay holds MULTI_CAP candidates, and it rarely needs more than the
     // best few dozen before a PTS minimum moves, so the bar is set `delta` below the best key (never below T); delta follows the
@@ -417,14 +461,16 @@ __global__ void __launch_bounds__(LEAN_THREADS, 1) ccsim_wave_multi_kernel(const
       }
       __syncthreads();                                                  // G2
       C = ms.ncand;
+      GPROF(if (cta == 0 && tid == 0) { const long long t2 = clock64(); ms.gp_cyc[pass ? GP_RAISE : GP_APPEND] += t2 - gp_t; ms.gp_cnt[pass ? GP_RAISE : GP_APPEND]++; gp_t = t2; })
       if (C <= MULTI_CAP || pass == 1) break;
       if (tid < MULTI_BINS) ms.hist[tid] = 0u;
       __syncthreads();
       const unsigned long long range = (unsigned long long)(kbest - T) + 1ull;
       #pragma unroll
       for (int u = 0; u < MULTI_EPT; u++) multi_hist_add((uint32_t)ea[u], T, range);
+      multi_bar_reset(cta);
       __syncthreads();
-      T = multi_raise_bar(T, kbest, range, cta);
+      T = multi_raise_bar(T, kbest, range);
     }
     if (XGPU) {
       // ---- gather, level 2 (node shards): every rank now holds ITS candidates keyed >= its bar T_r (<= MULTI_CAP of them, the same in
@@ -509,8 +555,9 @@ __global__ void __launch_bounds__(LEAN_THREADS, 1) ccsim_wave_multi_kernel(const
         multi_hist_add(lkey, T, range);
         #pragma unroll
         for (int u = 0; u < MULTI_XPT; u++) multi_hist_add(rkey[u], T, range);
+        multi_bar_reset(cta);
         __syncthreads();
-        T = multi_raise_bar(T, kbest, range, cta);
+        T = multi_raise_bar(T, kbest, range);
       }
       dead = dead || ms.dead != 0;
     }
@@ -845,6 +892,14 @@ __global__ void __launch_bounds__(LEAN_THREADS, 1) ccsim_wave_multi_kernel(const
         if (ms.rp_cnt[RP_MINMOVE + q])
           printf("round profile: term %d minimum moves %lld, %.0f cycles each, %.0f cycles/wave\n", q, ms.rp_cnt[RP_MINMOVE + q],
                  ms.rp_cyc[RP_MINMOVE + q] / (double)ms.rp_cnt[RP_MINMOVE + q], ms.rp_cyc[RP_MINMOVE + q] / w);
+    }
+#endif
+#ifdef MULTI_GATHER_PROFILE
+    {
+      const double w = (double)(limit_hit ? wv : wv + 1), nr = (double)(ms.gp_cnt[GP_RAISE] > 0 ? ms.gp_cnt[GP_RAISE] : 1);
+      printf("gather profile (CTA 0): waves %.0f | publish -> all own entries valid %.0f cycles/wave, %.1f poll rounds/wave | -> entries readable (G1) %.0f"
+             " | first append pass %.0f | bar raise %lld waves, %.0f cycles each, %.0f cycles/wave\n", w, ms.gp_cyc[GP_POLL] / w, ms.gp_cnt[GP_ROUNDS] / w,
+             ms.gp_cyc[GP_SYNC] / w, ms.gp_cyc[GP_APPEND] / w, ms.gp_cnt[GP_RAISE], ms.gp_cyc[GP_RAISE] / nr, ms.gp_cyc[GP_RAISE] / w);
     }
 #endif
   }
