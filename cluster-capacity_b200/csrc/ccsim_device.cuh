@@ -41,7 +41,8 @@ struct DevOut {
   unsigned long long preempt_no_victims;
   unsigned long long n_diag;
   long long phase_cycles[8];       // CTA 0's cycles per phase (multi-commit kernel: always; other kernels: CCSIM_PHASE_TIMERS builds)
-  long long stat[4];               // multi-commit kernel: [0] candidates replayed (sum over waves), [1] waves that had to raise the bar T
+  long long stat[4];               // multi-commit kernel: [0] candidates replayed (sum over waves), [1] waves that had to raise the bar T,
+                                   // [2] replay rounds, [3] waves replayed in key order
 };
 
 struct DevParams {
@@ -53,7 +54,8 @@ struct DevParams {
   int32_t chunk;        // nodes per CTA (contiguous ownership)
   int32_t rank, world;
   uint32_t epoch;       // run counter (1..255), folded into every exchanged word
-  uint32_t debug_flags; // CCSIM_DEBUG_FLAGS (kernel experiments): bit 0 = multi-commit waves end at every PTS minimum move
+  uint32_t debug_flags; // CCSIM_DEBUG_FLAGS (kernel experiments): bit 0 = multi-commit waves end at every PTS minimum move, ...,
+                        // bit 6 = single-use multi-commit waves keep the arg-max round (INTEGRATION.md lists them all)
   uint32_t xwave0;      // node-sharded runs: exchanges done by earlier runs of this handle; the double-buffer parity of the cross-GPU
                         // buffers continues across runs, so wave 0 of a run never lands in the buffer a lagging peer CTA still reads
   long long sample_k;   // numFeasibleNodesToFind (reference sampling mode)

@@ -823,6 +823,7 @@ struct ccsim_handle {
   uint32_t epoch = 0;
   uint32_t xwave0 = 0;                                    // exchanges of earlier sharded runs (buffer parity continues across runs)
   int64_t last_stat[16] = {};                             // ccsim_run_stats
+  int64_t last_key_order_waves = 0;                       // ccsim_key_order_waves
   RunPlan plan;
   int32_t *d_topo_full[CCSIM_MAX_TOPO_COLS] = {};
   int32_t *d_pod_node = nullptr; int64_t pod_cap = 0;
@@ -1540,6 +1541,7 @@ extern "C" int ccsim_run(ccsim_handle *h, int64_t max_pods, ccsim_result *out) {
   h->last_stat[0] = k.engine; h->last_stat[1] = ho.waves; h->last_stat[2] = ho.placed;
   h->last_stat[3] = ho.stat[0]; h->last_stat[4] = ho.stat[1]; h->last_stat[5] = grid; h->last_stat[6] = k.block; h->last_stat[7] = (int64_t)smem;
   for (int q = 0; q < 8; q++) h->last_stat[8 + q] = ho.phase_cycles[q];
+  h->last_key_order_waves = k.engine == ENG_MULTI ? ho.stat[3] : 0;
   out->placed = ho.placed; out->stop_code = ho.stop_code; out->waves = ho.waves; out->evals = ho.evals; out->run_ms = ms;
   out->examined = ho.examined ? ho.examined : ho.evals;
   h->last_placed = ho.placed;
@@ -1601,6 +1603,8 @@ extern "C" int ccsim_run_stats(const ccsim_handle *h, int64_t out[16]) {
   memcpy(out, h->last_stat, sizeof(h->last_stat));
   return CCSIM_OK;
 }
+
+extern "C" int64_t ccsim_key_order_waves(const ccsim_handle *h) { return h ? h->last_key_order_waves : 0; }
 
 extern "C" int ccsim_flush_l2(ccsim_handle *h) {
   if (!h) return CCSIM_EINVAL;

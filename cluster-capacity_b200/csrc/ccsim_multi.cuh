@@ -41,6 +41,11 @@
 //   those cycles (scripts/round_profile.sh). Work around the round stays on this warp: moved onto the whole block (the set-up
 //   between G1 and G2, the look-ahead decision after R) it measured slower on C4, whose terms have 8 and 64 domains.
 //   Row updates of the winners are done by each node's own thread after that barrier (a thread owns its node).
+// Key order (single-use templates: no second lives): the block ranks the wave's candidates once after compaction, and the replay
+//   warp holds them in rows of 32 in key order; a round is ballot(live) -> the lowest live lane -> one SHFL of its payload -> the same
+//   commit -> the kill test on each lane's one slot. A row is judged by a full cell test when the replay reaches it; a wake-up goes
+//   back to row 0 (see "the round in key order" below). C4: 778 -> 515 profiled cycles per round, kernel time 21.67-21.72 ->
+//   20.87-21.01 ms (one H100 80GB HBM3, 700 W power limit). CCSIM_DEBUG_FLAGS bit 6 keeps the arg-max round.
 // Look-ahead waves: a PodTopologySpread minimum move that REOPENS closed domains would end the wave (the reopened nodes were
 //   rejected by the scan and are in nobody's list). When a term's limit is about to move, the scan publishes the nodes of its
 //   closed cells too; they sit in the replay as dormant candidates (key 0: set-up reads the look-ahead terms' cells) and are
@@ -67,6 +72,10 @@
 #define MULTI_RELAX_K 8           /* look-ahead on a PTS term when at most this many of its domains still sit at the global minimum ... */
 #define MULTI_RELAX_R 3           /* ... nodes in cells up to this far over the limit are published as dormant candidates */
 #define MULTI_XPT (((CCSIM_MAX_WORLD - 1) * MULTI_CAP + LEAN_THREADS - 1) / LEAN_THREADS)   /* node shards: remote candidates per thread */
+#define MULTI_RANK_PARTS (LEAN_THREADS / MULTI_CAP)                       /* key order: threads that count one candidate's rank ... */
+#define MULTI_RANK_SPAN (((MULTI_CAP + MULTI_RANK_PARTS - 1) / MULTI_RANK_PARTS + 3) & ~3)   /* ... each over this many keys (16-byte loads) */
+static_assert(MULTI_RANK_PARTS >= 1 && MULTI_RANK_SPAN < 256, "key order: a partial rank fits a byte");
+static_assert(MULTI_CPT <= 32, "key order: one won bit per row");
 static_assert(MULTI_M == SLOT_STRIDE, "the keys of a CTA's list fill exactly one slot line");
 static_assert(4 + 2 * MULTI_CAP <= CCSIM_MAX_GRID * SLOT_STRIDE, "node shards: a rank's summary fits its region of the line buffer");
 
@@ -84,7 +93,10 @@ static_assert(4 + 2 * MULTI_CAP <= CCSIM_MAX_GRID * SLOT_STRIDE, "node shards: a
 #define RP_HANDOFF 5              /* after the loop: winners -> ms.mult */
 #define RP_DECIDE 6               /* after the loop: the next wave's look-ahead decision */
 #define RP_MINMOVE 7              /* + term q */
-#define RP_N (RP_MINMOVE + MULTI_GT)
+#define RP_RANK (RP_MINMOVE + MULTI_GT)   /* key order: ranking the wave's candidates (block-wide, up to the barrier after it) */
+#define RP_KROUND (RP_RANK + 1)   /* key order: the common round (ballot -> commit -> kill) */
+#define RP_ADVANCE (RP_RANK + 2)  /* key order: moving on to the next row (loads + full cell test), per row loaded */
+#define RP_N (RP_RANK + 3)
 #ifdef MULTI_ROUND_PROFILE
 #define RPROF(...) __VA_ARGS__
 #define RP_ADD(i, cyc, n) do { if (cta == 0 && lane == 0) { ms.rp_cyc[i] += (cyc); ms.rp_cnt[i] += (n); } } while (0)
@@ -124,7 +136,9 @@ struct __align__(16) MultiShared {
   uint32_t wtop[LEAN_WARPS][MULTI_M];               // per-warp top-M (compact) keys of this wave
   int32_t gt_c1[MULTI_GT][4];                       // per replicated-counter term: {limit, payload shift, payload mask, domains of the counter}
   int32_t gt_commit[MULTI_GT][4];                   // ... {counter base, inc, PTS constraint tracked or -1, n_present}
-  uint32_t ckey[MULTI_CAP], cdom[MULTI_CAP], cnext[MULTI_CAP];   // the wave's candidates keyed >= T (unordered)
+  uint32_t ckey[MULTI_CAP], cdom[MULTI_CAP], cnext[MULTI_CAP];   // the wave's candidates keyed >= T (unordered); in a key-order wave
+                                                                 // (no second lives) cnext[r] = the candidate of rank r
+  uint8_t kpart[MULTI_RANK_PARTS][MULTI_CAP];       // key order: partial ranks (keys greater than candidate i in one span of the array)
   uint32_t red[LEAN_WARPS], red2[LEAN_WARPS];       // block reductions (T, best key)
   uint32_t hist[MULTI_BINS];
   int32_t wfeas[LEAN_WARPS];
@@ -138,7 +152,7 @@ struct __align__(16) MultiShared {
   uint32_t delta, pad_ms;
   int32_t relax[LEAN_MAX_TERMS];                    // per Filter term: this wave's look-ahead over the limit (0: strict), see "dormant candidates"
   int32_t force_strict, st_relaxed, st_empty, pad_r;
-  long long ph[8], tc0, st_cand, st_overflow, st_rounds;       // CTA 0 / thread 0: clock cycles per phase, replay statistics
+  long long ph[8], tc0, st_cand, st_overflow, st_rounds, st_key_order;   // CTA 0 / thread 0: clock cycles per phase, replay statistics
 #ifdef MULTI_ROUND_PROFILE
   long long rp_cyc[RP_N], rp_cnt[RP_N], rp_t;                  // CTA 0's replay warp: cycles and events per part of the replay
 #endif
@@ -149,6 +163,7 @@ struct __align__(16) MultiShared {
 };
 
 __shared__ MultiShared ms;
+static_assert(offsetof(MultiShared, ckey) % 16 == 0 && (MULTI_RANK_SPAN * 4) % 16 == 0, "key order: 16-byte loads of ckey");
 
 struct MultiParams {
   uint32_t pay_shift[LEAN_MAX_SLOTS];   // record slot s (a topology column) -> bit position of its dom+1 field in the payload
@@ -244,7 +259,7 @@ __global__ void __launch_bounds__(LEAN_THREADS, 1) ccsim_wave_multi_kernel(const
 
   if (tid == 0) { ms.accepted = 0; ms.dead = 0; ms.stopb = 0; ms.n_gt = 0; ms.ncand = 0; ms.delta = 1u << MULTI_IDX_BITS; ms.force_strict = 0; ms.st_relaxed = 0; ms.st_empty = 0;
                   for (int q = 0; q < LEAN_MAX_TERMS; q++) ms.relax[q] = 0;
-                  for (int q = 0; q < 8; q++) ms.ph[q] = 0; ms.tc0 = 0; ms.st_cand = 0; ms.st_overflow = 0; ms.st_rounds = 0;
+                  for (int q = 0; q < 8; q++) ms.ph[q] = 0; ms.tc0 = 0; ms.st_cand = 0; ms.st_overflow = 0; ms.st_rounds = 0; ms.st_key_order = 0;
                   RPROF(for (int q = 0; q < RP_N; q++) ms.rp_cyc[q] = ms.rp_cnt[q] = 0; ms.rp_t = 0;)
                   GPROF(for (int q = 0; q < GP_N; q++) ms.gp_cyc[q] = ms.gp_cnt[q] = 0; ms.gp_valid = ms.gp_spins = 0ull; ms.gp_pub = 0;) }
   ms.mult[tid] = 0;
@@ -565,6 +580,36 @@ __global__ void __launch_bounds__(LEAN_THREADS, 1) ccsim_wave_multi_kernel(const
     if (C > MULTI_CAP) C = MULTI_CAP;     // (cannot happen after the second pass: the raised T admits <= MULTI_CAP keys)
     if (cta == 0 && tid == 0) ms.st_cand += C;
     MPH_MARK(3);
+    // ---- key order (single-use templates): no candidate comes back after it wins, so its key stands for the whole wave and the
+    //      winner of every round is the first live candidate in key order. Rank them once, with the whole block (the other warps
+    //      only wait at R): rank = the number of greater keys (keys are unique), counted by MULTI_RANK_PARTS threads per candidate
+    //      over one span of the array each, then cnext[rank] = candidate. CCSIM_DEBUG_FLAGS bit 6 keeps the arg-max round. ----
+    const bool key_order = ms.single_use != 0 && !(p.debug_flags & 64u) && !dead;     // (block-uniform)
+    if (key_order) {
+      const int i = tid % MULTI_CAP, part = tid / MULTI_CAP;
+      if (i < C && part < MULTI_RANK_PARTS) {
+        const uint32_t mine = ms.ckey[i];
+        const int span = ((C + MULTI_RANK_PARTS - 1) / MULTI_RANK_PARTS + 3) & ~3;     // (<= MULTI_RANK_SPAN)
+        const int j0 = part * span, j1 = min(j0 + span, C);
+        int r = 0, j = j0;
+        #pragma unroll 2
+        for (; j + 4 <= j1; j += 4) {
+          const uint4 v = *reinterpret_cast<const uint4 *>(&ms.ckey[j]);
+          r += (int)(v.x > mine) + (int)(v.y > mine) + (int)(v.z > mine) + (int)(v.w > mine);
+        }
+        for (; j < j1; j++) r += (int)(ms.ckey[j] > mine);
+        ms.kpart[part][i] = (uint8_t)r;
+      }
+      __syncthreads();                                                  // K1
+      if (tid < C) {
+        int r = 0;
+        #pragma unroll
+        for (int q = 0; q < MULTI_RANK_PARTS; q++) r += ms.kpart[q][tid];
+        ms.cnext[r] = (uint32_t)tid;
+      }
+      __syncthreads();                                                  // K2
+      RPROF(if (warp == 0) RP_ADD(RP_RANK, clock64() - ms.tc0, 1);)
+    }
     // ---- replay: the reference cycles k, k+1, ... this wave can decide; every CTA does the same, in ONE warp and without a
     //      barrier: MULTI_CPT candidates per lane in registers, lane q < n_gt also owns counter term q (its constants, and the
     //      minimum / multiplicity of the PTS constraint it tracks, stay in registers for the whole wave) ----
@@ -579,7 +624,7 @@ __global__ void __launch_bounds__(LEAN_THREADS, 1) ccsim_wave_multi_kernel(const
         for (int j = 0; j < MULTI_CPT; j++) {
           const int idx = j * 32 + lane;
           ck[j] = 0u; cd[j] = 0u;
-          if (idx < C) { ck[j] = ms.ckey[idx]; cd[j] = ms.cdom[idx]; }
+          if (idx < C && !key_order) { ck[j] = ms.ckey[idx]; cd[j] = ms.cdom[idx]; }
         }
         int4 gc = make_int4(0, 0, -1, 0), c1 = make_int4(0, 0, 0, 0);
         int32_t my_min = 0, my_num = 0;
@@ -636,9 +681,9 @@ __global__ void __launch_bounds__(LEAN_THREADS, 1) ccsim_wave_multi_kernel(const
             int32_t m = INT32_MAX;
             #pragma unroll 1
             for (int d = lane; d < ndom; d += 32) { const int32_t c = lds_s32(ca + 4u * d); if (c > publim) m = min(m, c); }
-            // this term's dormant candidates
+            // this term's dormant candidates (key order: the full cell test of each row when it is loaded finds them)
             #pragma unroll
-            for (int j = 0; j < MULTI_CPT; j++) {
+            for (int j = 0; j < MULTI_CPT; j++) if (!key_order) {
               const uint32_t f = (cd[j] >> sh) & mk;           // dom + 1 (0: no domain; cell 0 is read and ignored)
               const int32_t c = lds_s32(ca + 4u * (uint32_t)max((int32_t)f - 1, 0));
               if ((f != 0u) & (c > lim)) ck[j] = 0u;
@@ -648,8 +693,140 @@ __global__ void __launch_bounds__(LEAN_THREADS, 1) ccsim_wave_multi_kernel(const
           }
           if (cta == 0 && lane == 0) ms.st_relaxed++;
         }
+        // ---- commit pod k+acc, whose node's payload is `pay` (assume -> AssumePod -> NodeInfo.update(+1): schedule_one.go:967-984,
+        //      types.go:409-427). Only what the next round depends on happens here: the counter cells of the winner's domains (lane
+        //      q = term q; the host guarantees one term per incremented replicated counter), whether a cell went over its limit,
+        //      whether a PTS minimum moved. The winner's row (NodeInfo.update, node-local counters) is brought up to date by its own
+        //      thread after the wave. Returns the OR of the filled cells, with "a minimum moved" in bit 31. ----
+        auto commit = [&](const uint32_t pay, bool &rescan, bool &woke RPROF(, long long &rp_mm)) -> uint32_t {
+          // (lanes >= n_gt have a zero field mask: no domain, nothing written)
+          const uint32_t fpay = pay & fmask;                     // the winner's field of this lane's term, in place
+          const bool has = fpay != 0u;
+          const uint32_t ca = cnt_sa + 4u * (uint32_t)(gc.x + max((int32_t)(fpay >> c1.y) - 1, 0));
+          const int32_t old = lds_s32(ca), nv = old + gc.y;
+          if (has) sts_s32(ca, nv);
+          // candidates in a cell that went over its limit are dead from now on: its field, with the field's guard bit
+          const uint32_t fullf = (has & (nv > c1.x)) ? (fpay | fglane) : 0u;
+          const bool atmin = has & trk & ((int32_t)(fpay >> c1.y) - 1 < gc.w) & (old == my_min);   // a domain leaves the global minimum ...
+          my_num -= (int32_t)atmin;
+          const bool minchg = atmin & (my_num <= 0);                                                  // ... the last one: the minimum moves
+          // one OR-reduction carries the filled cells (the fields of different terms are disjoint bit ranges) and, in bit 31, that
+          // some term's minimum moved
+          const uint32_t F = __reduce_or_sync(0xffffffffu, fullf | ((uint32_t)minchg << 31));
+          // A PTS minimum moved (filtering.go:56-69: minMatchNum): recount it and move the term's limit. The wave goes on unless
+          // the move changes some node's feasibility: that takes a domain whose count lies in (old limit, new limit] — nodes there
+          // were rejected by the scan (or killed earlier in this wave) and pass now. Without such a domain every verdict so far
+          // stands (the 8-region constraint of C4 moves its minimum every 8 placements and never binds).
+          const unsigned mc = (F >> 31) ? __ballot_sync(0xffffffffu, minchg) : 0u;
+          for (unsigned nm = mc; nm; nm &= nm - 1) {
+            RPROF(const long long rp_m0 = clock64();)
+            const int q = __ffs(nm) - 1;
+            const int32_t off = __shfl_sync(0xffffffffu, gc.x, q), npres = __shfl_sync(0xffffffffu, gc.w, q), ndom = __shfl_sync(0xffffffffu, c1.w, q);
+            const int32_t lim_old = __shfl_sync(0xffffffffu, c1.x, q), loff = __shfl_sync(0xffffffffu, lim_off, q);
+            const uint32_t ca = cnt_sa + 4u * (uint32_t)off;
+            // one pass over the cells (one per lane for a term of <= 32 domains): this lane's minimum over the present domains and
+            // how many sit at it, and its lowest count over the old limit — the move changes verdicts iff that one is <= the new limit
+            int32_t mn = INT32_MAX, num = 0, up = INT32_MAX;
+            #pragma unroll 1
+            for (int d = lane; d < ndom; d += 32) {
+              const int32_t c = lds_s32(ca + 4u * d);
+              if (c > lim_old) up = min(up, c);
+              if (d < npres) { num = c < mn ? 0 : num; mn = min(mn, c); num += c == mn; }
+            }
+            const int32_t lmn = mn;
+            mn = __reduce_min_sync(0xffffffffu, mn);
+            up = __reduce_min_sync(0xffffffffu, up);
+            num = __reduce_add_sync(0xffffffffu, lmn == mn ? num : 0);
+            const long long liml = (long long)loff + (long long)mn;
+            const int32_t lim_new = liml > INT32_MAX ? INT32_MAX : (liml < INT32_MIN ? INT32_MIN : (int32_t)liml);
+            const bool hit = up <= lim_new;
+            // a term scanned with look-ahead published the nodes of its closed cells: the move only matters when the new limit
+            // reaches a cell that was not published; the cells in (old limit, new limit] wake their candidates up instead
+            const bool rq = __shfl_sync(0xffffffffu, rlx, q) > 0;
+            if (rq) { rescan |= (lim_new >= __shfl_sync(0xffffffffu, unpub_min, q)) | (p.debug_flags & 1); woke = true; }
+            else rescan |= hit | (p.debug_flags & 1);
+            if (lane == q) { my_min = mn; my_num = num; c1.x = lim_new; lim_moved = true; sts_s32(MS_SA(gt_c1) + 16u * (uint32_t)q, lim_new); }
+            RPROF(__syncwarp(); const long long rp_m1 = clock64(); RP_ADD(RP_MINMOVE + q, rp_m1 - rp_m0, 1); rp_mm += rp_m1 - rp_m0;)
+          }
+          return F;
+        };
         if (cta == 0 && lane == 0) ms.ph[6] += clock64() - ms.tc0;      // replay set-up
-        for (;;) {
+        // ---- the round in key order (single-use waves). Lane l holds the candidate of rank 32 * row + l: its payload, its key, and
+        //      whether it is live. At the start of every round a candidate is live iff it has not won in this wave and, for every
+        //      term with a field in its payload, its cell count is <= the term's current limit: the scan held every term but the
+        //      look-ahead ones to its limit, counts only grow, a kill follows every cell that goes over, a minimum move that does
+        //      not end the wave leaves no cell in (old limit, new limit] unless it wakes candidates up, and a won candidate never
+        //      comes back (single use). So a row is judged when the replay reaches it, by one full cell test against the counters
+        //      and limits as they stand; a wake-up sends the replay back to row 0 (rows above may hold revived candidates; the won
+        //      bits keep winners out). The winner is the lowest live lane of the first row that has one: a ballot instead of the
+        //      arg-max, one shuffle for its payload, a kill test on one slot. Every compacted candidate is keyed >= T, so "no live
+        //      candidate left" is the arg-max round's `g < Tr`. ----
+        if (key_order) {
+          const int nrows = (C + 31) >> 5;
+          int row = 0;
+          uint32_t won = 0u;                   // bit r: this lane's candidate of row r has won
+          uint32_t kd = 0u, kk = 0u;           // its payload and key
+          bool live = false;
+          auto load_row = [&]() {
+            __syncwarp();                      // the counter cells / limits written by the term lanes, before every lane reads them
+            const int idx = row * 32 + lane;
+            const bool present = idx < C;
+            const uint32_t o = present ? (uint32_t)lds_s32(MS_SA(cnext) + 4u * (uint32_t)idx) : 0u;
+            kk = present ? (uint32_t)lds_s32(MS_SA(ckey) + 4u * o) : 0u;
+            kd = present ? (uint32_t)lds_s32(MS_SA(cdom) + 4u * o) : 0u;   // (0: no field, every cell read is cell 0 of its counter)
+            // the full cell test. The term constants come from the term lanes' registers (lane q holds term q's current limit;
+            // lanes >= n_gt hold zeros: no field, cell 0 of the first counter), so nothing here branches and every load is
+            // issued before its first use.
+            uint32_t f[MULTI_GT];
+            int32_t cv[MULTI_GT], lim[MULTI_GT];
+            #pragma unroll
+            for (int q = 0; q < MULTI_GT; q++) {
+              const int32_t off = __shfl_sync(0xffffffffu, gc.x, q);
+              const uint32_t sh = (uint32_t)__shfl_sync(0xffffffffu, c1.y, q), mk = (uint32_t)__shfl_sync(0xffffffffu, c1.z, q);
+              lim[q] = __shfl_sync(0xffffffffu, c1.x, q);
+              f[q] = (kd >> sh) & mk;                                                  // dom + 1 (0: no domain; cell 0 is read and ignored)
+              cv[q] = lds_s32(cnt_sa + 4u * (uint32_t)(off + max((int32_t)f[q] - 1, 0)));
+            }
+            bool bad = false;
+            #pragma unroll
+            for (int q = 0; q < MULTI_GT; q++) bad |= (f[q] != 0u) & (cv[q] > lim[q]);
+            live = present & !bad & !((won >> row) & 1u);
+          };
+          load_row();
+          if (cta == 0 && lane == 0) ms.st_key_order++;
+          for (;;) {
+            RPROF(long long rp_t0 = clock64(), rp_mm = 0;)
+            unsigned lv = __ballot_sync(0xffffffffu, live);
+            if (lv == 0u) {                    // the row is used up: the next one, judged as counters and limits stand now
+              RPROF(int rp_n = 0;)
+              while (lv == 0u && ++row < nrows) { load_row(); lv = __ballot_sync(0xffffffffu, live); RPROF(rp_n++;) }
+              RPROF(const long long rp_a1 = clock64(); RP_ADD(RP_ADVANCE, rp_a1 - rp_t0, rp_n); rp_t0 = rp_a1;)
+              if (lv == 0u) { ran_dry = true; RP_ADD(RP_KROUND, clock64() - rp_t0, 1); break; }
+            }
+            const int w = __ffs(lv) - 1;
+            const uint32_t pay = __shfl_sync(0xffffffffu, kd, w);
+            if (lane == w) { live = false; won |= 1u << row; sts_s32(MS_SA(acc_node) + 4u * (uint32_t)acc, ckey_index(kk)); }
+            acc++;
+            bool rescan = false, woke = false;
+            const uint32_t F = commit(pay, rescan, woke RPROF(, rp_mm));
+            if (rescan | (acc >= acc_limit)) { ended_by_rescan = rescan; RP_ADD(RP_KROUND, clock64() - rp_t0 - rp_mm, 1); break; }
+            if (woke) {
+              RPROF(const long long rp_w0 = clock64();)
+              row = 0;
+              load_row();
+              RPROF(const long long rp_w1 = clock64(); RP_ADD(RP_REBUILD, rp_w1 - rp_w0, 1); rp_mm += rp_w1 - rp_w0;)
+            } else {
+              // the single-slot form of the SWAR kill test below (only this row can hold live candidates)
+              const uint32_t Fc = F & ((1u << MULTI_PAY_BITS) - 1u);
+              if (Fc) {
+                const uint32_t fv = Fc & ~fguard, fg = Fc & fguard;
+                if (~(((kd ^ fv) | fguard) - flsb) & fg) live = false;
+                RP_ADD(RP_KILL, 0, 1);
+              }
+            }
+            RP_ADD(RP_KROUND, clock64() - rp_t0 - rp_mm, 1);
+          }
+        } else for (;;) {                      // ---- the arg-max round: second lives, and CCSIM_DEBUG_FLAGS bit 6 ----
           RPROF(long long rp_t0 = clock64(), rp_mm = 0;)
           if (need_rebuild) {       // (one call site, off the round's critical path; see "dormant candidates")
             need_rebuild = false;
@@ -714,61 +891,10 @@ __global__ void __launch_bounds__(LEAN_THREADS, 1) ccsim_wave_multi_kernel(const
           #pragma unroll
           for (int j = 0; j < MULTI_CPT; j++) ck[j] = (ck[j] == g) ? nk : ck[j];
           second |= (uint32_t)(m == g) << ((pm >> MULTI_PAY_BITS) & 7u);
-          // Only what the next round depends on happens here: the counter cells of the winner's domains (lane q = term q; the
-          // host guarantees one term per incremented replicated counter), whether a cell went over its limit, whether a PTS
-          // minimum moved. The winner's row (NodeInfo.update, node-local counters) is brought up to date by its own thread after the wave.
-          // (lanes >= n_gt have a zero field mask: no domain, nothing written)
-          const uint32_t fpay = pay & fmask;                     // the winner's field of this lane's term, in place
-          const bool has = fpay != 0u;
-          const uint32_t ca = cnt_sa + 4u * (uint32_t)(gc.x + max((int32_t)(fpay >> c1.y) - 1, 0));
-          const int32_t old = lds_s32(ca), nv = old + gc.y;
-          if (has) sts_s32(ca, nv);
-          // candidates in a cell that went over its limit are dead from now on: its field, with the field's guard bit
-          const uint32_t fullf = (has & (nv > c1.x)) ? (fpay | fglane) : 0u;
-          const bool atmin = has & trk & ((int32_t)(fpay >> c1.y) - 1 < gc.w) & (old == my_min);   // a domain leaves the global minimum ...
-          my_num -= (int32_t)atmin;
-          const bool minchg = atmin & (my_num <= 0);                                                  // ... the last one: the minimum moves
           if (lane == 0) sts_s32(MS_SA(acc_node) + 4u * (uint32_t)acc, ckey_index(g));
           acc++;
-          // one OR-reduction carries the filled cells (the fields of different terms are disjoint bit ranges) and, in bit 31, that
-          // some term's minimum moved
-          const uint32_t F = __reduce_or_sync(0xffffffffu, fullf | ((uint32_t)minchg << 31));
-          // A PTS minimum moved (filtering.go:56-69: minMatchNum): recount it and move the term's limit. The wave goes on unless
-          // the move changes some node's feasibility: that takes a domain whose count lies in (old limit, new limit] — nodes there
-          // were rejected by the scan (or killed earlier in this wave) and pass now. Without such a domain every verdict so far
-          // stands (the 8-region constraint of C4 moves its minimum every 8 placements and never binds).
           bool rescan = false, woke = false;
-          const unsigned mc = (F >> 31) ? __ballot_sync(0xffffffffu, minchg) : 0u;
-          for (unsigned nm = mc; nm; nm &= nm - 1) {
-            RPROF(const long long rp_m0 = clock64();)
-            const int q = __ffs(nm) - 1;
-            const int32_t off = __shfl_sync(0xffffffffu, gc.x, q), npres = __shfl_sync(0xffffffffu, gc.w, q), ndom = __shfl_sync(0xffffffffu, c1.w, q);
-            const int32_t lim_old = __shfl_sync(0xffffffffu, c1.x, q), loff = __shfl_sync(0xffffffffu, lim_off, q);
-            const uint32_t ca = cnt_sa + 4u * (uint32_t)off;
-            // one pass over the cells (one per lane for a term of <= 32 domains): this lane's minimum over the present domains and
-            // how many sit at it, and its lowest count over the old limit — the move changes verdicts iff that one is <= the new limit
-            int32_t mn = INT32_MAX, num = 0, up = INT32_MAX;
-            #pragma unroll 1
-            for (int d = lane; d < ndom; d += 32) {
-              const int32_t c = lds_s32(ca + 4u * d);
-              if (c > lim_old) up = min(up, c);
-              if (d < npres) { num = c < mn ? 0 : num; mn = min(mn, c); num += c == mn; }
-            }
-            const int32_t lmn = mn;
-            mn = __reduce_min_sync(0xffffffffu, mn);
-            up = __reduce_min_sync(0xffffffffu, up);
-            num = __reduce_add_sync(0xffffffffu, lmn == mn ? num : 0);
-            const long long liml = (long long)loff + (long long)mn;
-            const int32_t lim_new = liml > INT32_MAX ? INT32_MAX : (liml < INT32_MIN ? INT32_MIN : (int32_t)liml);
-            const bool hit = up <= lim_new;
-            // a term scanned with look-ahead published the nodes of its closed cells: the move only matters when the new limit
-            // reaches a cell that was not published; the cells in (old limit, new limit] wake their candidates up instead
-            const bool rq = __shfl_sync(0xffffffffu, rlx, q) > 0;
-            if (rq) { rescan |= (lim_new >= __shfl_sync(0xffffffffu, unpub_min, q)) | (p.debug_flags & 1); woke = true; }
-            else rescan |= hit | (p.debug_flags & 1);
-            if (lane == q) { my_min = mn; my_num = num; c1.x = lim_new; lim_moved = true; sts_s32(MS_SA(gt_c1) + 16u * (uint32_t)q, lim_new); }
-            RPROF(__syncwarp(); const long long rp_m1 = clock64(); RP_ADD(RP_MINMOVE + q, rp_m1 - rp_m0, 1); rp_mm += rp_m1 - rp_m0;)
-          }
+          const uint32_t F = commit(pay, rescan, woke RPROF(, rp_mm));
           need_rebuild = woke & !rescan;
           // (no statistics, special registers or kernel parameters are touched inside the round loop: one S2R on this dependent
           //  chain costs as much as ten ALU instructions)
@@ -872,7 +998,7 @@ __global__ void __launch_bounds__(LEAN_THREADS, 1) ccsim_wave_multi_kernel(const
     o->evals = o->waves * (long long)p.n;
     o->examined = o->evals;
     for (int q = 0; q < 8; q++) o->phase_cycles[q] = ms.ph[q];
-    o->stat[0] = ms.st_cand; o->stat[1] = ms.st_overflow; o->stat[2] = ms.st_rounds;
+    o->stat[0] = ms.st_cand; o->stat[1] = ms.st_overflow; o->stat[2] = ms.st_rounds; o->stat[3] = ms.st_key_order;
     if (p.debug_flags & 8u)
       printf("multi-commit replay: waves %lld rounds %lld look-ahead waves %d (without a placement: %d) | cycles: replay %lld set-up %lld, per round %.0f\n",
              limit_hit ? wv : wv + 1, ms.st_rounds, ms.st_relaxed, ms.st_empty, ms.ph[4], ms.ph[6],
@@ -888,6 +1014,11 @@ __global__ void __launch_bounds__(LEAN_THREADS, 1) ccsim_wave_multi_kernel(const
       printf("round profile: after the loop %lld waves, %.0f cycles/wave (hand-off %.0f, look-ahead decision %.0f)\n", ms.rp_cnt[RP_AFTER],
              ms.rp_cyc[RP_AFTER] / w, ms.rp_cyc[RP_HANDOFF] / w, ms.rp_cyc[RP_DECIDE] / w);
       printf("round profile: rounds with a non-zero kill mask %lld\n", ms.rp_cnt[RP_KILL]);
+      printf("round profile: key order %lld waves | ranking %.0f cycles/wave | common round %lld events, %.0f cycles/round, %.0f cycles/wave"
+             " | row advances %lld, %.0f cycles each, %.0f cycles/wave\n", ms.st_key_order,
+             ms.rp_cyc[RP_RANK] / (double)(ms.rp_cnt[RP_RANK] > 0 ? ms.rp_cnt[RP_RANK] : 1),
+             ms.rp_cnt[RP_KROUND], ms.rp_cyc[RP_KROUND] / (double)(ms.rp_cnt[RP_KROUND] > 0 ? ms.rp_cnt[RP_KROUND] : 1), ms.rp_cyc[RP_KROUND] / w,
+             ms.rp_cnt[RP_ADVANCE], ms.rp_cyc[RP_ADVANCE] / (double)(ms.rp_cnt[RP_ADVANCE] > 0 ? ms.rp_cnt[RP_ADVANCE] : 1), ms.rp_cyc[RP_ADVANCE] / w);
       for (int q = 0; q < MULTI_GT; q++)
         if (ms.rp_cnt[RP_MINMOVE + q])
           printf("round profile: term %d minimum moves %lld, %.0f cycles each, %.0f cycles/wave\n", q, ms.rp_cnt[RP_MINMOVE + q],

@@ -17,7 +17,7 @@ _lib = None
 EXPORTS = ["ccsim_create", "ccsim_destroy", "ccsim_last_error", "ccsim_abi_version", "ccsim_load_nodes",
            "ccsim_set_templates", "ccsim_run", "ccsim_prepare", "ccsim_node_counts", "ccsim_peer_export", "ccsim_peer_import",
            "ccsim_device_info", "ccsim_kernel_launches", "ccsim_kernel_name", "ccsim_flush_l2", "ccsim_run_stats", "ccsim_peer_local",
-           "ccsim_peer_import_local"]
+           "ccsim_peer_import_local", "ccsim_key_order_waves"]
 
 
 class EngineError(RuntimeError):
@@ -61,6 +61,8 @@ def lib():
         L.ccsim_peer_import_local.argtypes = [C.c_void_p, C.c_int32, C.POINTER(C.c_void_p)]
         L.ccsim_run_stats.restype = C.c_int
         L.ccsim_run_stats.argtypes = [C.c_void_p, abi.P64]
+        L.ccsim_key_order_waves.restype = C.c_int64
+        L.ccsim_key_order_waves.argtypes = [C.c_void_p]
         L.ccsim_peer_export.restype = C.c_int
         L.ccsim_peer_export.argtypes = [C.c_void_p, abi.PU8]
         L.ccsim_peer_import.restype = C.c_int
@@ -171,6 +173,10 @@ class Engine:
         return {"engine": self.ENGINE_NAMES[int(v[0])], "kernel": self.kernel_name(), "waves": int(v[1]), "placed": int(v[2]),
                 "candidates": int(v[3]), "bar_raised_waves": int(v[4]), "grid": int(v[5]), "block": int(v[6]), "smem_bytes": int(v[7]),
                 "phase_cycles": [int(x) for x in v[8:16]]}
+
+    def key_order_waves(self):
+        """Waves of the last run the multi-commit kernel replayed in key order (see ccsim_key_order_waves in include/ccsim.h)."""
+        return int(lib().ccsim_key_order_waves(self._h))
 
     def kernel_launches(self):
         return int(lib().ccsim_kernel_launches(self._h))

@@ -335,6 +335,10 @@ int  ccsim_flush_l2(ccsim_handle *h);                  /* writes a buffer larger
  * raised the candidate bar [5] grid [6] block [7] dynamic shared memory bytes [8..15] CTA 0's clock cycles per phase, summed
  * over waves (multi-commit: scan, barrier, merge+publish, gather, replay, row updates+recount; 0 for the other engines) */
 int  ccsim_run_stats(const ccsim_handle *h, int64_t out[16]);
+/* waves of the last run that the multi-commit kernel replayed in key order (single-use templates: the candidates ranked once, each
+ * winner taken by a ballot); 0 for the other engines, for templates whose winners may come back in their wave, and under
+ * CCSIM_DEBUG_FLAGS bit 6 */
+int64_t ccsim_key_order_waves(const ccsim_handle *h);
 
 #ifdef __cplusplus
 }
