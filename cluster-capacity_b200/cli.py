@@ -3,7 +3,8 @@ top of the GPU path:
 
     python -m cluster-capacity_b200.cli --podspec examples/pod.yaml --snapshot cluster.json [--max-limit N]
            [--exclude-nodes a,b] [--default-config cfg.yaml] [--verbose] [-o json|yaml] [--kubeconfig KUBECONFIG]
-    (--podspec may be repeated or name a directory: several podspecs are simulated round-robin, e.g. the genpod output of 64 namespaces)
+    (--podspec may be repeated or name a directory: several podspecs are simulated round-robin, e.g. the genpod output of 64 namespaces;
+     with --each every podspec is analysed on its own, as if `cluster-capacity --podspec <file>` ran once per file)
 
 The analysis needs the LISTed Node/Pod/Namespace objects. `--snapshot` takes a JSON/YAML file
 {"nodes": [...], "pods": [...], "namespaces": [...]} (or a directory with nodes.json / pods.json / namespaces.json);
@@ -124,6 +125,9 @@ def main(argv=None):
     ap.add_argument("--verbose", action="store_true", help="Verbose mode")
     ap.add_argument("-o", "--output", default="", help="Output format. One of: json|yaml")
     ap.add_argument("--snapshot", default="", help="Node/Pod/Namespace lists as a file or directory (instead of a live API server)")
+    ap.add_argument("--each", action="store_true",
+                    help="Analyse every podspec of --podspec on its own against the same snapshot (one review per podspec, in order; "
+                         "-o json prints them as one JSON array, -o yaml separates them by ---).")
     ap.add_argument("--device", type=int, default=0)
     a = ap.parse_args(argv)
     if not a.podspec:
@@ -140,15 +144,22 @@ def main(argv=None):
             else:
                 files.append(path)
         pods = [parse_api_spec(f) for f in files]
-        pod = pods[0] if len(pods) == 1 else pods
+        pod = pods if a.each else (pods[0] if len(pods) == 1 else pods)
         objs = load_snapshot(a.snapshot) if a.snapshot else list_from_cluster(a.kubeconfig)
         cc = fw.New(load_scheduler_config(a.default_config), None, pod, a.max_limit, [x for x in a.exclude_nodes.split(",") if x], device=a.device)
         cc.SyncWithClient(fw.ListClient(objs["nodes"], objs["pods"], objs["namespaces"], objs["services"], objs["replicationcontrollers"],
                                         objs["replicasets"], objs["statefulsets"]))
         for w in cc.Warnings():
             print("warning: " + w, file=sys.stderr)
-        cc.Run()
-        fw.ClusterCapacityReviewPrint(cc, a.verbose, a.output)
+        if a.each:
+            reviews = [r.Print(a.verbose, a.output) for r in cc.RunEach()]
+            if a.output == "json":
+                print("[" + ",".join(r.rstrip("\n") for r in reviews) + "]")
+            else:
+                print(("---\n" if a.output == "yaml" else "").join(reviews), end="")
+        else:
+            cc.Run()
+            fw.ClusterCapacityReviewPrint(cc, a.verbose, a.output)
     except (fw.FrameworkError, OSError, subprocess.CalledProcessError) as e:   # the reference prints the error and exits 0 (server.go:68-71)
         print(e)
     return 0

@@ -37,6 +37,7 @@
 #include "ccsim_batched.cuh"
 #include "ccsim_multi.cuh"
 #include "ccsim_stream.cuh"
+#include "ccsim_each.cuh"
 
 #define BLOCK_THREADS 512
 #define MAX_WARPS (BLOCK_THREADS / 32)
@@ -725,7 +726,7 @@ __global__ void ccsim_flush_kernel(unsigned long long *buf, size_t n, unsigned l
 // host side of the C-ABI
 // ------------------------------------------------------------------------------------------------------------------
 // Every wave-kernel instantiation run_prepare may pick, in the order of the WK_* indices, and what the host knows about it
-enum EngineCode { ENG_GENERIC, ENG_LEAN, ENG_TIE_RUN, ENG_MULTI, ENG_STREAM };   // ccsim_run_stats[0]
+enum EngineCode { ENG_GENERIC, ENG_LEAN, ENG_TIE_RUN, ENG_MULTI, ENG_STREAM, ENG_EACH };   // ccsim_run_stats[0]
 struct WaveKernel {
   const void *fn;
   const char *name;        // ccsim_kernel_name
@@ -745,9 +746,10 @@ static const WaveKernel WAVE_KERNELS[] = {
   {(const void *)ccsim_wave_stream_kernel<0>, "stream<0>", ENG_STREAM, STREAM_BLOCK, sizeof(StreamShared), stream_smem_bytes(0, 0)},
   {(const void *)ccsim_wave_stream_kernel<1>, "stream<1>", ENG_STREAM, STREAM_BLOCK, sizeof(StreamShared), stream_smem_bytes(1, 0)},
   {(const void *)ccsim_wave_stream_kernel<2>, "stream<2>", ENG_STREAM, STREAM_BLOCK, sizeof(StreamShared), 0},
+  {(const void *)ccsim_each_kernel, "each", ENG_EACH, EACH_THREADS, sizeof(EachShared), 0},     // ccsim_run_each only
 };
-enum { WK_WAVE, WK_WAVE_STREAMED, WK_LEAN, WK_LEAN_SAMPLING, WK_BATCHED, WK_MULTI, WK_MULTI_SHARDED, WK_STREAM /* + mode */ };
-static_assert(sizeof(WAVE_KERNELS) / sizeof(WAVE_KERNELS[0]) == WK_STREAM + 3, "one WAVE_KERNELS entry per WK_* index");
+enum { WK_WAVE, WK_WAVE_STREAMED, WK_LEAN, WK_LEAN_SAMPLING, WK_BATCHED, WK_MULTI, WK_MULTI_SHARDED, WK_STREAM /* + mode */, WK_EACH = WK_STREAM + 3 };
+static_assert(sizeof(WAVE_KERNELS) / sizeof(WAVE_KERNELS[0]) == WK_EACH + 1, "one WAVE_KERNELS entry per WK_* index");
 
 struct RunPlan {      // what run_prepare decided, consumed by the launch
   bool valid = false, empty = false;
@@ -832,6 +834,12 @@ struct ccsim_handle {
   DevParams *d_params = nullptr;
   int64_t last_placed = 0;
   void *d_flush = nullptr; size_t flush_bytes = 0;
+  // ccsim_run_each: per-analysis state, sequences and results of the last per-analysis run (each_ran until the next ccsim_run / prepare)
+  std::vector<void *> each_allocs;
+  bool each_ran = false;
+  int32_t *d_each_seq = nullptr; int64_t each_seq_cap = 0;
+  std::vector<int64_t> each_placed;
+  std::vector<std::vector<int32_t>> each_seq;
 };
 
 static std::string g_create_err;
@@ -936,7 +944,7 @@ extern "C" void ccsim_destroy(ccsim_handle *h) {
   if (!h) return;
   cudaSetDevice(h->cfg.device);
   cudaStreamSynchronize(h->stream);
-  free_pool(h, h->allocs); free_pool(h, h->tmpl_allocs); free_pool(h, h->stream_allocs); drop_cache(h);
+  free_pool(h, h->allocs); free_pool(h, h->tmpl_allocs); free_pool(h, h->stream_allocs); free_pool(h, h->each_allocs); drop_cache(h);
   for (int r = 0; r < CCSIM_MAX_WORLD; r++) if (h->x_peer[r] && r != h->cfg.rank && !h->peers_local) cudaIpcCloseMemHandle(h->x_peer[r]);
   cudaFree(h->d_xslots);
   if (h->d_pod_node) { cudaFreeAsync(h->d_pod_node, h->stream); cudaStreamSynchronize(h->stream); }
@@ -1070,7 +1078,7 @@ extern "C" int ccsim_set_templates(ccsim_handle *h, int32_t n_templates, const c
     return fail(h, CCSIM_EUNSUPPORTED, "PodTopologySpread/InterPodAffinity templates are single-template only");
   CK(cudaSetDevice(h->cfg.device));
   free_pool(h, h->tmpl_allocs);
-  h->have_templates = false; h->plan.valid = false;
+  h->have_templates = false; h->plan.valid = false; h->each_ran = false;
   const ccsim_nodes &nd = h->meta;
   for (int t = 0; t < n_templates; t++) {
     const ccsim_template &T = templates[t];
@@ -1426,6 +1434,7 @@ static int run_prepare(ccsim_handle *h, int64_t max_pods) {
   CK(cudaSetDevice(h->cfg.device));
   RunPlan &pl = h->plan;
   pl = RunPlan();                         // no kernel name until a kernel is chosen; the parameter blocks zeroed
+  h->each_ran = false;
   pl.max_pods = max_pods;
   int64_t cap = 0; int rc;
   if ((rc = check_run_bounds(h, max_pods, cap)) || (rc = restore_run_state(h, cap))) return rc;
@@ -1563,19 +1572,172 @@ extern "C" int ccsim_run(ccsim_handle *h, int64_t max_pods, ccsim_result *out) {
   return CCSIM_OK;
 }
 
+// Entries of tree level l (l >= 1) over all classes of an analysis: sum_c ceil(n_c / 32^l) <= ceil(N / 32^l) + classes
+static long long each_level_bound(long long n, int l, int ncls) {
+  const long long span = 1ll << (5 * l);
+  return (n + span - 1) / span + ncls;
+}
+
+extern "C" int ccsim_run_each(ccsim_handle *h, int64_t max_pods, ccsim_result *out) {
+  if (!h || !out) return fail(h, CCSIM_EINVAL, "null argument");
+  if (!h->have_nodes || !h->have_templates) return fail(h, CCSIM_ESTATE, "load_nodes and set_templates must come first");
+  const int T = h->n_templates;
+  // the per-analysis kernel covers node-local templates only: placing a clone must change nothing but its node
+  if (h->cfg.world > 1) return fail(h, CCSIM_EUNSUPPORTED, "per-analysis runs: node-sharded runs (world %d) are not supported", h->cfg.world);
+  if (h->cfg.sampling == CCSIM_SAMPLING_REFERENCE) return fail(h, CCSIM_EUNSUPPORTED, "per-analysis runs: reference sampling is not supported");
+  if (h->n_counters > 0)
+    return fail(h, CCSIM_EUNSUPPORTED, "per-analysis runs: per-domain counters (topology spread, pod (anti-)affinity) are not supported");
+  if (h->w_placed) return fail(h, CCSIM_EUNSUPPORTED, "per-analysis runs: hostPorts (placed mask) are not supported");
+  for (int t = 0; t < T; t++) {
+    const ccsim_template &P = h->h_templates[t];
+    if ((P.n_pref_terms > 0 && (P.score_enable & CCSIM_PL_NODE_AFFINITY)) || (P.n_spts > 0 && (P.score_enable & CCSIM_PL_POD_TOPOLOGY_SPREAD)) ||
+        (P.n_ipa_score > 0 && (P.score_enable & CCSIM_PL_INTER_POD_AFFINITY)))
+      return fail(h, CCSIM_EUNSUPPORTED, "per-analysis runs: template %d has a normalised soft scorer (preferred nodeAffinity, ScheduleAnyway spreading, pod-affinity scoring)", t);
+  }
+  // every analysis is bounded like a run of its template alone (check_run_bounds); the sequences hold the largest bound
+  int64_t cap = 1;
+  for (int t = 0; t < T; t++) {
+    const bool fit_off = !(h->h_templates[t].filter_enable & CCSIM_PL_FIT);
+    if (max_pods <= 0 && fit_off)
+      return fail(h, CCSIM_EUNSUPPORTED, "template %d: NodeResourcesFit is disabled: the run is unbounded, --max-limit is required", t);
+    int64_t c = h->pod_bound + 1;
+    if (max_pods > 0 && (max_pods < c || fit_off)) c = max_pods;
+    cap = std::max(cap, c);
+  }
+  CK(cudaSetDevice(h->cfg.device));
+  const int32_t n = h->n;
+  const int ncls = h->max_prefer_pop + 1;
+  {
+    size_t free_b = 0, total_b = 0;
+    CK(cudaMemGetInfo(&free_b, &total_b));
+    const double seq_bytes = (double)T * (double)cap * 4.0;
+    if (seq_bytes > (double)free_b)
+      return fail(h, CCSIM_EUNSUPPORTED, "per-analysis runs: the sequence buffers (%d x %lld x 4 B = %.2f GiB) exceed free device memory (%.2f GiB)",
+                  T, (long long)cap, seq_bytes / (1 << 30), (double)free_b / (1 << 30));
+  }
+  h->plan = RunPlan();
+  h->each_ran = false;
+  memset(out, 0, sizeof(ccsim_result) * (size_t)T);
+  // tree shape: roots on level L (32^L >= N); levels [1, split) in global memory, [split, L] in shared memory, the lowest split whose
+  // shared levels fit next to the kernel's static structs
+  int L = 0;
+  while (n > 0 && (1ll << (5 * L)) < n) L++;
+  const WaveKernel &kern = WAVE_KERNELS[WK_EACH];
+  int split = 1;
+  size_t smem = 0;
+  for (; split <= L + 1; split++) {
+    smem = 0;
+    for (int l = split; l <= L; l++) smem += 8 * (size_t)each_level_bound(n, l, ncls);
+    if (smem + kern.static_smem + 1024 <= h->smem_optin) break;
+  }
+  EachParams ep; memset(&ep, 0, sizeof(ep));
+  ep.n_levels = L; ep.split = split; ep.max_pods = max_pods; ep.seq_cap = cap;
+  {
+    long long g = 0, s = 0;
+    for (int l = 1; l <= L; l++) {
+      if (l < split) { ep.lev_off[l] = g; g += each_level_bound(n, l, ncls); }
+      else { ep.lev_off[l] = s; s += each_level_bound(n, l, ncls); }
+    }
+    ep.glev_stride = g;
+  }
+  free_pool(h, h->each_allocs);
+  int rc;
+  const size_t tn = (size_t)T * (size_t)n;
+  if ((rc = dev_alloc<int32_t>(h, h->each_allocs, &ep.k, tn)) || (rc = dev_alloc<unsigned long long>(h, h->each_allocs, &ep.leaf, tn)) ||
+      (rc = dev_alloc<unsigned long long>(h, h->each_allocs, &ep.glev, (size_t)T * ep.glev_stride)) ||
+      (rc = dev_alloc<int32_t>(h, h->each_allocs, &ep.seq, (size_t)T * cap)) || (rc = dev_alloc<EachOut>(h, h->each_allocs, &ep.out, (size_t)T)))
+    return rc;
+  if (ncls > 1 && (rc = dev_alloc<int32_t>(h, h->each_allocs, &ep.pos, tn))) return rc;
+  DevOut *d_diag = nullptr;
+  if ((rc = dev_alloc<DevOut>(h, h->each_allocs, &d_diag, (size_t)T))) return rc;
+  ep.s_req_cpu = h->s_req_cpu; ep.s_req_mem = h->s_req_mem; ep.s_req_eph = h->s_req_eph; ep.s_nz_cpu = h->s_nz_cpu; ep.s_nz_mem = h->s_nz_mem;
+  ep.s_npods = h->s_npods;
+  for (int q = 0; q < h->meta.n_scalars; q++) ep.s_req_scalar[q] = h->s_req_scalar[q];
+  h->d_each_seq = ep.seq; h->each_seq_cap = cap;
+  cudaStream_t s = h->stream;
+  std::vector<EachOut> eo((size_t)T);
+  std::vector<DevOut> diag((size_t)T);
+  float ms = 0.f;
+  if (n > 0) {
+    DevParams p;
+    fill_params(h, p, max_pods);
+    CK(cudaMemcpyAsync(h->d_params, &p, sizeof(DevParams), cudaMemcpyHostToDevice, s));   // filter_extras reads p.self
+    CK(cudaMemsetAsync(d_diag, 0, sizeof(DevOut) * (size_t)T, s));
+    void *args[] = { (void *)&p, (void *)&ep };
+    CK(cudaEventRecord(h->ev0, s));
+    CK(cudaLaunchKernel(kern.fn, dim3(T), dim3(kern.block), args, smem, s));
+    h->launches++;
+    CK(cudaEventRecord(h->ev1, s));
+    CK(cudaMemcpyAsync(eo.data(), ep.out, sizeof(EachOut) * (size_t)T, cudaMemcpyDeviceToHost, s));
+    CK(cudaStreamSynchronize(s));
+    CK(cudaEventElapsedTime(&ms, h->ev0, h->ev1));
+    for (int t = 0; t < T; t++) if (eo[t].error) return fail(h, CCSIM_ECUDA, "per-analysis kernel: analysis %d overflowed its sequence buffer", t);
+    // the terminal diagnosis of every Unschedulable analysis: its final state into the working columns, then the wave kernels' pass
+    for (int t = 0; t < T; t++) {
+      if (eo[t].stop_code != CCSIM_STOP_UNSCHEDULABLE) continue;
+      const int blocks = std::min(4 * h->sm_count, (n + 255) / 256);
+      ccsim_each_scatter_kernel<<<blocks, 256, 0, s>>>(p, ep, t);
+      p.out = d_diag + t;
+      ccsim_diag_kernel<<<blocks, 256, 0, s>>>(p, t);
+      h->launches += 2;
+      CK(cudaGetLastError());
+    }
+    CK(cudaMemcpyAsync(diag.data(), d_diag, sizeof(DevOut) * (size_t)T, cudaMemcpyDeviceToHost, s));
+  } else {
+    for (int t = 0; t < T; t++) { eo[t].placed = 0; eo[t].stop_code = CCSIM_STOP_UNSCHEDULABLE; }   // ErrNoNodesAvailable: the host formats it
+  }
+  h->each_placed.assign((size_t)T, 0);
+  h->each_seq.assign((size_t)T, std::vector<int32_t>());
+  for (int t = 0; t < T; t++) {
+    h->each_placed[t] = eo[t].placed;
+    h->each_seq[t].resize((size_t)eo[t].placed);
+    if (eo[t].placed) CK(cudaMemcpyAsync(h->each_seq[t].data(), ep.seq + (size_t)t * cap, (size_t)eo[t].placed * 4, cudaMemcpyDeviceToHost, s));
+  }
+  CK(cudaStreamSynchronize(s));
+  int64_t waves = 0, placed = 0;
+  for (int t = 0; t < T; t++) {
+    ccsim_result &r = out[t];
+    const bool unsched = eo[t].stop_code == CCSIM_STOP_UNSCHEDULABLE;
+    r.placed = eo[t].placed; r.stop_code = eo[t].stop_code; r.n_nodes = h->n_global;
+    r.waves = eo[t].placed + (unsched ? 1 : 0);
+    r.evals = n > 0 ? (int64_t)n + eo[t].placed : 0;        // every node once, then the winner of each placement
+    r.examined = r.waves * (int64_t)n;                       // what the reference's scheduling cycles examine
+    if (unsched && n > 0) {
+      for (int q = 0; q < CCSIM_R_TOTAL; q++) r.reason_hist[q] = (int64_t)diag[t].reason_hist[q];
+      r.preempt_no_victims = (int64_t)diag[t].preempt_no_victims;
+      r.preempt_not_helpful = (int64_t)n - r.preempt_no_victims;
+    }
+    r.run_ms = ms;                                           // the whole launch: the analyses run concurrently
+    r.pod_node = h->each_seq[t].data();
+    waves += r.waves; placed += r.placed;
+  }
+  h->plan.kern = &kern;
+  memset(h->last_stat, 0, sizeof(h->last_stat));
+  h->last_stat[0] = ENG_EACH; h->last_stat[1] = waves; h->last_stat[2] = placed;
+  h->last_stat[3] = std::min(split - 1, L); h->last_stat[4] = L - std::min(split - 1, L);   // upper tree levels in global / shared memory
+  h->last_stat[5] = T; h->last_stat[6] = kern.block; h->last_stat[7] = (int64_t)smem;
+  h->last_key_order_waves = 0;
+  h->each_ran = true;
+  return CCSIM_OK;
+}
+
 extern "C" int ccsim_node_counts(ccsim_handle *h, int32_t t, int32_t *counts, int64_t *first_pod) {
   if (!h || !counts || !first_pod) return fail(h, CCSIM_EINVAL, "null argument");
   if (!h->have_templates || t < 0 || t >= h->n_templates) return fail(h, CCSIM_EINVAL, "template index");
   CK(cudaSetDevice(h->cfg.device));
+  if (h->each_ran && t >= (int32_t)h->each_placed.size()) return fail(h, CCSIM_EINVAL, "analysis index");
   const int32_t N = h->n_global;
   int32_t *d_counts = nullptr; unsigned long long *d_first = nullptr;
   CK(cudaMalloc((void **)&d_counts, (size_t)(N ? N : 1) * 4));
   CK(cudaMalloc((void **)&d_first, (size_t)(N ? N : 1) * 8));
   CK(cudaMemsetAsync(d_counts, 0, (size_t)N * 4, h->stream));
   CK(cudaMemsetAsync(d_first, 0xFF, (size_t)N * 8, h->stream));
-  if (h->last_placed > 0) {
-    ccsim_count_kernel<<<std::min<long long>(4 * h->sm_count, (h->last_placed + 255) / 256), 256, 0, h->stream>>>(
-        h->d_pod_node, h->last_placed, h->n_templates, t, d_counts, d_first);
+  // after ccsim_run_each: analysis t's own sequence, every pod of it a clone of template t
+  const int32_t *seq = h->each_ran ? h->d_each_seq + (size_t)t * h->each_seq_cap : h->d_pod_node;
+  const long long placed = h->each_ran ? h->each_placed[t] : h->last_placed;
+  if (placed > 0) {
+    ccsim_count_kernel<<<std::min<long long>(4 * h->sm_count, (placed + 255) / 256), 256, 0, h->stream>>>(
+        seq, placed, h->each_ran ? 1 : h->n_templates, h->each_ran ? 0 : t, d_counts, d_first);
     h->launches++;
   }
   CK(cudaMemcpyAsync(counts, d_counts, (size_t)N * 4, cudaMemcpyDeviceToHost, h->stream));

@@ -146,7 +146,13 @@ struct cc_handle {
   bool have_report = false;
   std::string err, out, warn;
   int64_t pending_skipped = 0;   // pods of the snapshot without spec.nodeName (not terminal): not replayed, reported by cc_warnings
+  // cc_run_each: one read-only view per podspec (cc_analysis); a view's node names are its base's
+  std::vector<std::unique_ptr<cc_handle>> analyses;
+  const cc_handle *base = nullptr;
 };
+
+// the encoding a handle's node indices refer to (a view's is its base's)
+static const Encoded &enc_of(const cc_handle *h) { return h->base ? h->base->enc : h->enc; }
 
 static std::string g_new_err;
 static int fail(cc_handle *h, int code, const std::string &m) { if (h) h->err = m; else g_new_err = m; return code; }
@@ -586,6 +592,7 @@ template <class T, class F> static ObjList<T> parse_list(const char *text, F one
 extern "C" int cc_sync_with_objects(cc_handle *h, const char *nodes_json, const char *pods_json, const char *namespaces_json) {
   if (!h) return CC_EINVAL;
   if (h->closed) return fail(h, CC_ESTATE, "closed");
+  if (h->base) return fail(h, CC_ESTATE, "an analysis view is read-only");
   try {
     h->nodes.clear(); h->pods.clear(); h->ns_labels.clear(); h->workloads.clear();
     const bool timing = getenv("CCHOST_TIMING") != nullptr;
@@ -609,6 +616,7 @@ extern "C" int cc_sync_workloads(cc_handle *h, const char *services_json, const 
                                  const char *statefulsets_json) {
   if (!h) return CC_EINVAL;
   if (h->closed) return fail(h, CC_ESTATE, "closed");
+  if (h->base) return fail(h, CC_ESTATE, "an analysis view is read-only");
   if (!h->synced) return fail(h, CC_ESTATE, "cc_sync_with_objects must come first");
   try {
     h->workloads.clear();
@@ -638,6 +646,13 @@ static ccsim_handle *engine_acquire(const ccsim_config &cfg, int &rc) {
   rc = ccsim_create(&cfg, &e);
   return rc ? nullptr : e;
 }
+static void engine_release(const ccsim_config &cfg, ccsim_handle *e);
+// A libccsim call failed: the engine is destroyed (not reused) and its error becomes the handle's
+static int engine_failed(cc_handle *h, ccsim_handle *eng, const char *what, int rc) {
+  std::string m = std::string(what) + ": " + ccsim_last_error(eng);
+  ccsim_destroy(eng);
+  return rc == CCSIM_EUNSUPPORTED ? fail(h, CC_EUNSUPPORTED, "unsupported on the GPU path: " + m) : fail(h, CC_EENGINE, m);
+}
 static void engine_release(const ccsim_config &cfg, ccsim_handle *e) {
   if (getenv("CCHOST_NO_ENGINE_REUSE")) { ccsim_destroy(e); return; }
   {
@@ -647,31 +662,38 @@ static void engine_release(const ccsim_config &cfg, ccsim_handle *e) {
   ccsim_destroy(e);
 }
 
-extern "C" int cc_run(cc_handle *h) {
-  if (!h) return CC_EINVAL;
-  if (h->closed) return fail(h, CC_ESTATE, "closed");
-  if (!h->synced) return fail(h, CC_ESTATE, "cc_sync_with_objects must come first");
-  try {
-    ensure_encoded(h);
-  } catch (const Unsupported &e) { return fail(h, CC_EUNSUPPORTED, std::string("unsupported on the GPU path: ") + e.what());
-  } catch (const std::exception &e) { return fail(h, CC_EINVAL, e.what()); }
+// The stop reason of a run that ends before the engine: no nodes (ErrNoNodesAvailable, scheduler.go:68; schedule_one.go:165-168), or
+// PreFilter rejecting the pod outright (the FitError then carries only the PreFilter message). False when the engine must run.
+static bool stop_before_engine(const Encoded &E, std::string &reason) {
+  if (E.n == 0) { reason = "Unschedulable: no nodes available to schedule pods"; return true; }
+  if (!E.prefilter_msg.empty()) {
+    reason = "Unschedulable: 0/" + std::to_string(E.n) + " nodes are available: " + E.prefilter_msg + ". preemption: " +
+             fit_error_body(E.n, {{"Preemption is not helpful for scheduling", E.n}});
+    return true;
+  }
+  return false;
+}
+
+// Status.StopReason of an engine run whose pod `failed` did not fit (or that reached max_pods): simulator.go:301,332
+static std::string stop_reason_of(const Encoded &E, const ccsim_result &res, int64_t max_pods, const Pod &failed) {
+  if (res.stop_code == CCSIM_STOP_LIMIT_REACHED) return "LimitReached: Maximum number of pods simulated: " + std::to_string(max_pods);
+  std::vector<std::pair<std::string, int64_t>> hist;
+  for (int r = 0; r < CCSIM_R_FIXED_COUNT; r++) hist.push_back({kReasonText[r], res.reason_hist[r]});
+  for (size_t k = 0; k < E.scalar_names.size(); k++) hist.push_back({"Insufficient " + E.scalar_names[k], res.reason_hist[CCSIM_R_SCALAR0 + k]});
+  for (size_t t = 0; t < E.taint_dict.size(); t++)   // taint_toleration.go:120
+    hist.push_back({"node(s) had untolerated taint {" + E.taint_dict[t].key + ": " + E.taint_dict[t].value + "}", res.reason_hist[CCSIM_R_TAINT0 + t]});
+  std::string msg = fit_error_body(E.n, hist);
+  // DefaultPreemption PostFilter (default_preemption.go:132-143; preemption.go:234-279): no victims anywhere
+  std::string post;
+  if (failed.preemption_policy == "Never") post = "not eligible due to preemptionPolicy=Never.";
+  else post = fit_error_body(E.n, {{"No preemption victims found for incoming pod", res.preempt_no_victims},
+                                   {"Preemption is not helpful for scheduling", res.preempt_not_helpful}});
+  return "Unschedulable: " + msg + " preemption: " + post;   // simulator.go:332
+}
+
+// The engine of the handle's configuration, loaded with its encoded snapshot and templates. On failure: nullptr, h->err set, rc the code.
+static ccsim_handle *loaded_engine(cc_handle *h, const ccsim_config &cfg, int &rc) {
   const Encoded &E = h->enc;
-  h->pod_node.clear();
-  h->have_report = false;
-  if (E.n == 0) {   // ErrNoNodesAvailable (scheduler.go:68; schedule_one.go:165-168)
-    h->stop_reason = "Unschedulable: no nodes available to schedule pods";
-    h->ran = true;
-    return CC_OK;
-  }
-  if (!E.prefilter_msg.empty()) {   // PreFilter rejected the pod outright: FitError carries only the PreFilter message
-    h->stop_reason = "Unschedulable: 0/" + std::to_string(E.n) + " nodes are available: " + E.prefilter_msg + ". preemption: " +
-                     fit_error_body(E.n, {{"Preemption is not helpful for scheduling", E.n}});
-    h->ran = true;
-    return CC_OK;
-  }
-  ccsim_config cfg; memset(&cfg, 0, sizeof(cfg));
-  cfg.abi_version = CCSIM_ABI_VERSION; cfg.device = h->device; cfg.engine = CCSIM_ENGINE_AUTO; cfg.rank = 0; cfg.world = 1;
-  if (h->cfg.reference_sampling && h->cfg.pct_nodes_to_score != 100) { cfg.sampling = CCSIM_SAMPLING_REFERENCE; cfg.pct_nodes_to_score = h->cfg.pct_nodes_to_score; }
   const bool timing = getenv("CCHOST_TIMING") != nullptr;
   auto tlast = std::chrono::steady_clock::now();
   auto tick = [&](const char *what) {
@@ -680,43 +702,104 @@ extern "C" int cc_run(cc_handle *h) {
     fprintf(stderr, "[cchost]   run/%s %.4f s\n", what, std::chrono::duration<double>(now - tlast).count());
     tlast = now;
   };
-  int rc = 0;
   ccsim_handle *eng = engine_acquire(cfg, rc);
-  if (!eng) return fail(h, CC_EENGINE, std::string("ccsim_create: ") + ccsim_last_error(nullptr));
+  if (!eng) { rc = fail(h, CC_EENGINE, std::string("ccsim_create: ") + ccsim_last_error(nullptr)); return nullptr; }
   tick("engine (created or taken from the idle list)");
   ccsim_nodes nd; E.fill_nodes(nd);
-  ccsim_result res;
-  auto bail = [&](const char *what) {
-    std::string m = std::string(what) + ": " + ccsim_last_error(eng);
-    ccsim_destroy(eng);
-    return rc == CCSIM_EUNSUPPORTED ? fail(h, CC_EUNSUPPORTED, "unsupported on the GPU path: " + m) : fail(h, CC_EENGINE, m);
-  };
-  if ((rc = ccsim_load_nodes(eng, &nd))) return bail("ccsim_load_nodes");
-  tick("ccsim_load_nodes");
-  if ((rc = ccsim_set_templates(eng, (int32_t)h->enc_tmpls.size(), h->enc_tmpls.data(), (int32_t)E.counters.size(), E.counters.data()))) return bail("ccsim_set_templates");
-  tick("ccsim_set_templates");
-  if ((rc = ccsim_run(eng, h->max_pods, &res))) return bail("ccsim_run");
-  tick("ccsim_run");
-  h->pod_node.assign(res.pod_node, res.pod_node + res.placed);
-  if (res.stop_code == CCSIM_STOP_LIMIT_REACHED) {
-    h->stop_reason = "LimitReached: Maximum number of pods simulated: " + std::to_string(h->max_pods);   // simulator.go:301
-  } else {
-    std::vector<std::pair<std::string, int64_t>> hist;
-    for (int r = 0; r < CCSIM_R_FIXED_COUNT; r++) hist.push_back({kReasonText[r], res.reason_hist[r]});
-    for (size_t k = 0; k < E.scalar_names.size(); k++) hist.push_back({"Insufficient " + E.scalar_names[k], res.reason_hist[CCSIM_R_SCALAR0 + k]});
-    for (size_t t = 0; t < E.taint_dict.size(); t++)   // taint_toleration.go:120
-      hist.push_back({"node(s) had untolerated taint {" + E.taint_dict[t].key + ": " + E.taint_dict[t].value + "}", res.reason_hist[CCSIM_R_TAINT0 + t]});
-    std::string msg = fit_error_body(E.n, hist);
-    // DefaultPreemption PostFilter (default_preemption.go:132-143; preemption.go:234-279): no victims anywhere
-    std::string post;
-    const Pod &failed = h->tmpls[(size_t)res.placed % h->tmpls.size()];   // the pod that did not fit: clone of template placed % T
-    if (failed.preemption_policy == "Never") post = "not eligible due to preemptionPolicy=Never.";
-    else post = fit_error_body(E.n, {{"No preemption victims found for incoming pod", res.preempt_no_victims},
-                                     {"Preemption is not helpful for scheduling", res.preempt_not_helpful}});
-    h->stop_reason = "Unschedulable: " + msg + " preemption: " + post;   // simulator.go:332
+  const char *what = "ccsim_load_nodes";
+  if (!(rc = ccsim_load_nodes(eng, &nd))) {
+    tick("ccsim_load_nodes");
+    what = "ccsim_set_templates";
+    if (!(rc = ccsim_set_templates(eng, (int32_t)h->enc_tmpls.size(), h->enc_tmpls.data(), (int32_t)E.counters.size(), E.counters.data()))) {
+      tick("ccsim_set_templates");
+      return eng;
+    }
   }
+  rc = engine_failed(h, eng, what, rc);
+  return nullptr;
+}
+
+static int encode_for_run(cc_handle *h) {
+  if (h->closed) return fail(h, CC_ESTATE, "closed");
+  if (h->base) return fail(h, CC_ESTATE, "an analysis view is read-only: run its base handle");
+  if (!h->synced) return fail(h, CC_ESTATE, "cc_sync_with_objects must come first");
+  try {
+    ensure_encoded(h);
+  } catch (const Unsupported &e) { return fail(h, CC_EUNSUPPORTED, std::string("unsupported on the GPU path: ") + e.what());
+  } catch (const std::exception &e) { return fail(h, CC_EINVAL, e.what()); }
+  return CC_OK;
+}
+
+static ccsim_config engine_config(const cc_handle *h) {
+  ccsim_config cfg; memset(&cfg, 0, sizeof(cfg));
+  cfg.abi_version = CCSIM_ABI_VERSION; cfg.device = h->device; cfg.engine = CCSIM_ENGINE_AUTO; cfg.rank = 0; cfg.world = 1;
+  if (h->cfg.reference_sampling && h->cfg.pct_nodes_to_score != 100) { cfg.sampling = CCSIM_SAMPLING_REFERENCE; cfg.pct_nodes_to_score = h->cfg.pct_nodes_to_score; }
+  return cfg;
+}
+
+extern "C" int cc_run(cc_handle *h) {
+  if (!h) return CC_EINVAL;
+  int rc = encode_for_run(h);
+  if (rc) return rc;
+  const Encoded &E = h->enc;
+  h->pod_node.clear();
+  h->have_report = false;
+  if (stop_before_engine(E, h->stop_reason)) { h->ran = true; return CC_OK; }
+  const ccsim_config cfg = engine_config(h);
+  ccsim_handle *eng = loaded_engine(h, cfg, rc);
+  if (!eng) return rc;
+  ccsim_result res;
+  const auto t0 = std::chrono::steady_clock::now();
+  if ((rc = ccsim_run(eng, h->max_pods, &res))) return engine_failed(h, eng, "ccsim_run", rc);
+  if (getenv("CCHOST_TIMING")) fprintf(stderr, "[cchost]   run/ccsim_run %.4f s\n", std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count());
+  h->pod_node.assign(res.pod_node, res.pod_node + res.placed);
+  h->stop_reason = stop_reason_of(E, res, h->max_pods, h->tmpls[(size_t)res.placed % h->tmpls.size()]);   // the pod that did not fit: clone of template placed % T
   engine_release(cfg, eng);
   h->ran = true;
+  return CC_OK;
+}
+
+extern "C" int cc_run_each(cc_handle *h) {
+  if (!h) return CC_EINVAL;
+  int rc = encode_for_run(h);
+  if (rc) return rc;
+  const Encoded &E = h->enc;
+  const size_t T = h->tmpls.size();
+  h->analyses.clear();
+  std::vector<std::unique_ptr<cc_handle>> views;
+  for (size_t t = 0; t < T; t++) {   // podspec t alone, as a handle of its own would hold it
+    std::unique_ptr<cc_handle> v(new cc_handle());
+    v->cfg = h->cfg; v->tmpl = h->tmpls[t]; v->tmpls.assign(1, h->tmpls[t]); v->max_pods = h->max_pods; v->exclude = h->exclude;
+    v->device = h->device; v->base = h;
+    views.push_back(std::move(v));
+  }
+  std::string early;
+  if (stop_before_engine(E, early)) {
+    for (auto &v : views) { v->stop_reason = early; v->ran = true; }
+    h->analyses = std::move(views);
+    return CC_OK;
+  }
+  const ccsim_config cfg = engine_config(h);
+  ccsim_handle *eng = loaded_engine(h, cfg, rc);
+  if (!eng) return rc;
+  std::vector<ccsim_result> res(T);
+  if ((rc = ccsim_run_each(eng, h->max_pods, res.data()))) return engine_failed(h, eng, "ccsim_run_each", rc);
+  for (size_t t = 0; t < T; t++) {
+    cc_handle &v = *views[t];
+    v.pod_node.assign(res[t].pod_node, res[t].pod_node + res[t].placed);
+    v.stop_reason = stop_reason_of(E, res[t], h->max_pods, h->tmpls[t]);   // every pod of analysis t is a clone of podspec t
+    v.ran = true;
+  }
+  engine_release(cfg, eng);
+  h->analyses = std::move(views);
+  return CC_OK;
+}
+
+extern "C" int cc_analysis(cc_handle *h, int32_t t, cc_handle **view) {
+  if (!h || !view) return CC_EINVAL;
+  if (h->analyses.empty()) return fail(h, CC_ESTATE, "cc_run_each must come first");
+  if (t < 0 || (size_t)t >= h->analyses.size()) return fail(h, CC_EINVAL, "analysis " + std::to_string(t) + " out of range (" + std::to_string(h->analyses.size()) + " podspecs)");
+  *view = h->analyses[(size_t)t].get();
   return CC_OK;
 }
 
@@ -777,10 +860,10 @@ static int build_report(cc_handle *h) {
   const size_t T = h->tmpls.size();
   for (size_t t = 0; t < T; t++) {
     Json rons = Json::array();
-    std::vector<int64_t> count(h->enc.n, 0); std::vector<int32_t> order;
+    std::vector<int64_t> count(enc_of(h).n, 0); std::vector<int32_t> order;
     for (size_t k = t; k < h->pod_node.size(); k += T) { const int32_t w = h->pod_node[k]; if (count[w]++ == 0) order.push_back(w); }
     rons.arr.reserve(order.size());
-    for (int32_t w : order) { Json r = Json::object(); r.obj.reserve(2); r.set("nodeName", Json::string(h->enc.names[w])); r.set("replicas", Json::number(count[w])); rons.push(std::move(r)); }
+    for (int32_t w : order) { Json r = Json::object(); r.obj.reserve(2); r.set("nodeName", Json::string(enc_of(h).names[w])); r.set("replicas", Json::number(count[w])); rons.push(std::move(r)); }
     Json podres = Json::object();
     podres.set("podName", Json::string(h->tmpls[t].name));
     podres.set("replicasOnNodes", std::move(rons));      // (moved, not copied: one entry per node that received a clone)
@@ -857,12 +940,13 @@ extern "C" const char *cc_stop_reason(cc_handle *h) { return h ? h->stop_reason.
 extern "C" int64_t cc_scheduled_count(cc_handle *h) { return h ? (int64_t)h->pod_node.size() : 0; }
 extern "C" const char *cc_scheduled_node(cc_handle *h, int64_t k) {
   if (!h || k < 0 || k >= (int64_t)h->pod_node.size()) return nullptr;
-  return h->enc.names[h->pod_node[k]].c_str();
+  return enc_of(h).names[h->pod_node[k]].c_str();
 }
-extern "C" void cc_close(cc_handle *h) { if (h) { h->closed = true; delete h; } }
+extern "C" void cc_close(cc_handle *h) { if (h && !h->base) { h->closed = true; delete h; } }   // a view goes with its base
 
 extern "C" const char *cc_debug_encoded_snapshot(cc_handle *h) {
   if (!h) return nullptr;
+  if (h->base) { fail(h, CC_ESTATE, "an analysis view has no snapshot of its own"); return nullptr; }
   try { ensure_encoded(h); }
   catch (const Unsupported &e) { fail(h, CC_EUNSUPPORTED, std::string("unsupported on the GPU path: ") + e.what()); return nullptr; }
   catch (const std::exception &e) { fail(h, CC_EINVAL, e.what()); return nullptr; }

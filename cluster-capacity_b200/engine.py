@@ -17,7 +17,7 @@ _lib = None
 EXPORTS = ["ccsim_create", "ccsim_destroy", "ccsim_last_error", "ccsim_abi_version", "ccsim_load_nodes",
            "ccsim_set_templates", "ccsim_run", "ccsim_prepare", "ccsim_node_counts", "ccsim_peer_export", "ccsim_peer_import",
            "ccsim_device_info", "ccsim_kernel_launches", "ccsim_kernel_name", "ccsim_flush_l2", "ccsim_run_stats", "ccsim_peer_local",
-           "ccsim_peer_import_local", "ccsim_key_order_waves"]
+           "ccsim_peer_import_local", "ccsim_key_order_waves", "ccsim_run_each"]
 
 
 class EngineError(RuntimeError):
@@ -45,6 +45,8 @@ def lib():
         L.ccsim_prepare.argtypes = [C.c_void_p, C.c_int64]
         L.ccsim_run.restype = C.c_int
         L.ccsim_run.argtypes = [C.c_void_p, C.c_int64, C.POINTER(abi.Result)]
+        L.ccsim_run_each.restype = C.c_int
+        L.ccsim_run_each.argtypes = [C.c_void_p, C.c_int64, C.POINTER(abi.Result)]
         L.ccsim_node_counts.restype = C.c_int
         L.ccsim_node_counts.argtypes = [C.c_void_p, C.c_int32, abi.P32, abi.P64]
         L.ccsim_device_info.restype = C.c_int
@@ -116,6 +118,7 @@ class Engine:
         T = (abi.Template * len(templates))(*templates)
         Cn = (abi.Counter * max(1, len(counters)))(*counters)
         self._check(lib().ccsim_set_templates(self._h, len(templates), T, len(counters), Cn), "ccsim_set_templates")
+        self._n_templates = len(templates)
 
     def prepare(self, max_pods=0):
         """The allocation / restore half of run(max_pods); see ccsim_prepare."""
@@ -125,6 +128,13 @@ class Engine:
         res = abi.Result()
         self._check(lib().ccsim_run(self._h, max_pods, C.byref(res)), "ccsim_run")
         return RunResult(res)
+
+    def run_each(self, max_pods=0):
+        """Every loaded template analysed on its own (ccsim_run_each): one RunResult per template, each what run() gives for a
+        handle holding that template alone."""
+        res = (abi.Result * self._n_templates)()
+        self._check(lib().ccsim_run_each(self._h, max_pods, res), "ccsim_run_each")
+        return [RunResult(r) for r in res]
 
     def connect_peers(self, dist):
         """Node-sharded multi-GPU run: all-gather the CUDA IPC handles of the exchange buffers over torch.distributed
@@ -164,15 +174,19 @@ class Engine:
         lib().ccsim_device_info(self._h, C.byref(sm), C.byref(grid), C.byref(block), C.byref(l2))
         return dict(sm_count=sm.value, grid=grid.value, block=block.value, l2_bytes=l2.value)
 
-    ENGINE_NAMES = ("generic", "lean sequential", "tie-run batching", "multi-commit", "streaming (TMA)")
+    ENGINE_NAMES = ("generic", "lean sequential", "tie-run batching", "multi-commit", "streaming (TMA)")   # what ccsim_run may choose
+    EACH_ENGINE = "per-analysis max-tree"                                                                # engine code 5: ccsim_run_each
 
     def run_stats(self):
         """Latency anatomy of the last run (see ccsim_run_stats in include/ccsim.h)."""
         v = np.zeros(16, np.int64)
         self._check(lib().ccsim_run_stats(self._h, v.ctypes.data_as(abi.P64)), "ccsim_run_stats")
-        return {"engine": self.ENGINE_NAMES[int(v[0])], "kernel": self.kernel_name(), "waves": int(v[1]), "placed": int(v[2]),
-                "candidates": int(v[3]), "bar_raised_waves": int(v[4]), "grid": int(v[5]), "block": int(v[6]), "smem_bytes": int(v[7]),
-                "phase_cycles": [int(x) for x in v[8:16]]}
+        st = {"engine": self.ENGINE_NAMES[int(v[0])] if int(v[0]) < len(self.ENGINE_NAMES) else self.EACH_ENGINE, "kernel": self.kernel_name(), "waves": int(v[1]), "placed": int(v[2]),
+              "candidates": int(v[3]), "bar_raised_waves": int(v[4]), "grid": int(v[5]), "block": int(v[6]), "smem_bytes": int(v[7]),
+              "phase_cycles": [int(x) for x in v[8:16]]}
+        if int(v[0]) == 5:      # per-analysis runs: where the upper levels of the max-trees live
+            st["global_levels"], st["shared_levels"] = int(v[3]), int(v[4])
+        return st
 
     def key_order_waves(self):
         """Waves of the last run the multi-commit kernel replayed in key order (see ccsim_key_order_waves in include/ccsim.h)."""

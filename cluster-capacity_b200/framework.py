@@ -6,6 +6,7 @@
     review = cc.Report()               # simulator.go:160 — dict with the reference's JSON shape (report.go:38-98)
     framework.ClusterCapacityReviewPrint(review_or_cc, verbose, format)   # report.go:305
     cc.ScheduledPods(); cc.Close()
+    for a in cc.RunEach(): a.Report()  # several podspecs, each analysed on its own (`cluster-capacity --podspec` per file)
 
 All the work happens in C++ (encoder) and CUDA (libccsim); this file only marshals JSON across the C-ABI.
 """
@@ -18,7 +19,8 @@ SO_PATH = os.path.join(_HERE, "libcchost.so")
 _lib = None
 
 EXPORTS = ["cc_new", "cc_new_list", "cc_sync_with_objects", "cc_sync_workloads", "cc_run", "cc_report_json", "cc_report_print", "cc_stop_reason",
-           "cc_scheduled_count", "cc_scheduled_node", "cc_close", "cc_last_error", "cc_warnings", "cc_debug_encoded_snapshot"]
+           "cc_scheduled_count", "cc_scheduled_node", "cc_close", "cc_last_error", "cc_warnings", "cc_debug_encoded_snapshot", "cc_run_each",
+           "cc_analysis"]
 
 
 class FrameworkError(RuntimeError):
@@ -45,6 +47,10 @@ def lib():
         L.cc_sync_workloads.argtypes = [C.c_void_p, C.c_char_p, C.c_char_p, C.c_char_p, C.c_char_p]
         L.cc_run.restype = C.c_int
         L.cc_run.argtypes = [C.c_void_p]
+        L.cc_run_each.restype = C.c_int
+        L.cc_run_each.argtypes = [C.c_void_p]
+        L.cc_analysis.restype = C.c_int
+        L.cc_analysis.argtypes = [C.c_void_p, C.c_int32, C.POINTER(C.c_void_p)]
         for f in ("cc_report_json", "cc_stop_reason", "cc_last_error", "cc_warnings", "cc_debug_encoded_snapshot"):
             getattr(L, f).restype = C.c_char_p
             getattr(L, f).argtypes = [C.c_void_p]
@@ -71,9 +77,10 @@ class ListClient:
 
 
 class ClusterCapacity:
-    def __init__(self, handle):
+    def __init__(self, handle, n_podspecs=1):
         self._h = handle
         self._report = None
+        self._n = n_podspecs
 
     def _err(self, rc, what):
         msg = lib().cc_last_error(self._h).decode()
@@ -98,6 +105,22 @@ class ClusterCapacity:
         if rc:
             self._err(rc, "Run")
         self._report = None
+
+    def RunEach(self):
+        """Every podspec analysed on its own against the synced snapshot, in one GPU launch (cc_run_each): a list with one result per
+        podspec, in order. Result t has Report(), Print(), StopReason() and ScheduledPods() with the meaning they have on a
+        ClusterCapacity built from podspec t alone and Run()."""
+        rc = lib().cc_run_each(self._h)
+        if rc:
+            self._err(rc, "RunEach")
+        out = []
+        for t in range(self._n):
+            v = C.c_void_p()
+            rc = lib().cc_analysis(self._h, t, C.byref(v))
+            if rc:
+                self._err(rc, "RunEach")
+            out.append(Analysis(v, self))
+        return out
 
     def Report(self):
         if self._report is None:
@@ -143,6 +166,18 @@ class ClusterCapacity:
             pass
 
 
+class Analysis(ClusterCapacity):
+    """One analysis of RunEach(): a read-only view owned by its ClusterCapacity, which it keeps alive."""
+
+    def __init__(self, handle, owner):
+        super().__init__(handle)
+        self._owner = owner
+
+    def Close(self):
+        self._h = None        # the view goes with its owner's handle
+        self._owner = None
+
+
 def New(kube_scheduler_config, kube_config, simulated_pod, max_pods=0, exclude_nodes=(), device=0):
     """framework.New (simulator.go:107). kube_scheduler_config: None for the default profile or a dict
     {"percentageOfNodesToScore", "disabledFilters", "disabledScores", "weights"}; kube_config is unused (kept for
@@ -153,11 +188,13 @@ def New(kube_scheduler_config, kube_config, simulated_pod, max_pods=0, exclude_n
     cfg = json.dumps(kube_scheduler_config).encode() if kube_scheduler_config else None
     if isinstance(simulated_pod, (list, tuple)):
         rc = lib().cc_new_list(cfg, json.dumps(list(simulated_pod)).encode(), int(max_pods), ",".join(exclude_nodes).encode(), device, C.byref(h))
+        n = len(simulated_pod)
     else:
         rc = lib().cc_new(cfg, json.dumps(simulated_pod).encode(), int(max_pods), ",".join(exclude_nodes).encode(), device, C.byref(h))
+        n = 1
     if rc:
         raise FrameworkError("New rc=%d: %s" % (rc, lib().cc_last_error(None).decode()))
-    return ClusterCapacity(h)
+    return ClusterCapacity(h, n)
 
 
 def ClusterCapacityReviewPrint(cc, verbose=False, fmt=""):

@@ -13,6 +13,7 @@
  *   cc_close             <- (*ClusterCapacity).Close()                 (simulator.go:314-325), idempotent
  *   cc_new_list          <- the roadmap's "accept a list of pods" (README.md:305-306): framework.New with several podspecs, pod k of the
  *                           run is a clone of podspec k % T (the template index parsePodsReview uses, report.go:160)
+ *   cc_run_each / cc_analysis <- `cluster-capacity --podspec <file>` once per podspec of a list (the genpod workflow), in one launch
  *   cc_stop_reason / cc_scheduled_count / cc_scheduled_node <- Status{StopReason, Pods} as the callers of Report() read them
  *                           (simulator.go:90-93; ScheduledPods in the reference's tests, simulator_test.go:226-240)
  *   cc_warnings          <- nothing in the reference: what this analysis left out that the reference would have done (pending pods)
@@ -62,6 +63,14 @@ int cc_sync_with_objects(cc_handle *h, const char *nodes_json, const char *pods_
 int cc_sync_workloads(cc_handle *h, const char *services_json, const char *rcs_json, const char *replicasets_json,
                       const char *statefulsets_json);
 int cc_run(cc_handle *h);
+/* Every podspec of the handle analysed on its own against the synced snapshot, all in one GPU launch: analysis t is what
+ * cc_new(podspec t) + cc_sync_with_objects + cc_run gives under the same configuration, max_pods and exclude_nodes. Node-local
+ * podspecs only: topology spread, pod (anti-)affinity, normalised soft scorers, hostPorts and reference sampling are refused by name. */
+int cc_run_each(cc_handle *h);
+/* After cc_run_each: a read-only view of analysis t (podspec t alone and its Status), owned by h and valid until the next
+ * cc_run_each or cc_close(h). cc_report_json / cc_report_print / cc_stop_reason / cc_scheduled_* read it like a handle of its own;
+ * cc_run, cc_run_each and the syncs fail on it with CC_ESTATE, and cc_close ignores it. */
+int cc_analysis(cc_handle *h, int32_t t, cc_handle **view);
 const char *cc_report_json(cc_handle *h);
 const char *cc_report_print(cc_handle *h, int32_t verbose, const char *format /* "", "json", "yaml" */);
 const char *cc_stop_reason(cc_handle *h);

@@ -295,13 +295,23 @@ int  ccsim_set_templates(ccsim_handle *h, int32_t n_templates, const ccsim_templ
  * counter with a domain whose |init| + m * |inc| could leave int32, m = min(max_pods, the free pod slots of the cluster, those of
  * the domain's nodes); without the slot bounds when a template disables NodeResourcesFit. */
 int  ccsim_run(ccsim_handle *h, int64_t max_pods, ccsim_result *out);
+/* Per-analysis runs: every loaded template t is analysed on its own against the loaded snapshot, all in one launch (one CTA per
+ * analysis, a max-tree over per-node keys: DESIGN.md §4.1g). out[n_templates]: out[t] is what ccsim_run gives for a handle holding
+ * template t alone (pod_node, placed, stop_code, reason_hist, preempt_*); waves = placed (+1 when Unschedulable), evals = the nodes
+ * pushed through the Filter (every node once, then each placement's winner), examined = waves * n_nodes, run_ms = the whole launch.
+ * pod_node arrays are owned by the handle until the next run. Afterwards ccsim_node_counts(h, t, ...) gives analysis t's counts.
+ * Refuses (CCSIM_EUNSUPPORTED, before any launch): per-domain counters, normalised soft scorers, hostPorts (placed mask), world > 1,
+ * reference sampling, a template without NodeResourcesFit when max_pods <= 0, and sequence buffers (n_templates x min(max_pods,
+ * free pod slots + 1) x 4 B) larger than the free device memory. */
+int  ccsim_run_each(ccsim_handle *h, int64_t max_pods, ccsim_result *out /* [n_templates] */);
 /* Optional: everything ccsim_run(h, max_pods) does BEFORE the wave kernel starts (buffers, restoring the snapshot, engine choice),
  * synchronously. A host that drives several ranks from one process calls it on every handle, then starts the ccsim_run calls
  * concurrently: no rank's persistent kernel then waits for a peer that is still inside a (device-synchronising) allocation. */
 int  ccsim_prepare(ccsim_handle *h, int64_t max_pods);
 
 /* per-node number of placed pods of template t after the last run (device histogram; report.go:146-180 without the O(P*nodes) scan)
- * and the index of the first pod placed on each node (-1 none): ReplicasOnNodes is ordered by first placement. */
+ * and the index of the first pod placed on each node (-1 none): ReplicasOnNodes is ordered by first placement. After ccsim_run_each:
+ * the counts of analysis t, first_pod indexing its own sequence. */
 int  ccsim_node_counts(ccsim_handle *h, int32_t t, int32_t *counts /*[n_nodes]*/, int64_t *first_pod /*[n_nodes]*/);
 
 /* multi-GPU (node-axis shards, SURVEY.md §8(e)): one process per GPU, rank r owns nodes [r*ceil(N/W), ...).
@@ -326,13 +336,15 @@ int64_t ccsim_kernel_launches(const ccsim_handle *h);  /* kernels launched by th
 /* the wave-kernel instantiation the last ccsim_prepare (or the prepare inside ccsim_run) chose: "wave<true>" / "wave<false>"
  * (generic, tile resident / streamed from global memory), "lean<false>" / "lean<true>" (lean, reference sampling), "batched",
  * "multi<false>" / "multi<true>" (multi-commit, sharded), "stream<0>" / "stream<1>" / "stream<2>" (TMA streaming: every column
- * streamed / with mask columns / resident free columns). "" before any prepare, after a failed one and for an empty cluster.
+ * streamed / with mask columns / resident free columns), "each" (ccsim_run_each). "" before any prepare, after a failed one and for an
+ * empty cluster.
  * Valid after ccsim_prepare alone: no kernel needs to run. The string is static. */
 const char *ccsim_kernel_name(const ccsim_handle *h);
 int  ccsim_flush_l2(ccsim_handle *h);                  /* writes a buffer larger than L2 (bench hygiene) */
 /* latency anatomy of the last run (bench.py's roofline block): [0] engine (0 generic, 1 lean sequential, 2 tie-run batching,
- * 3 multi-commit, 4 streaming) [1] waves [2] placed [3] multi-commit: candidates replayed, summed over waves [4] multi-commit: waves that
- * raised the candidate bar [5] grid [6] block [7] dynamic shared memory bytes [8..15] CTA 0's clock cycles per phase, summed
+ * 3 multi-commit, 4 streaming, 5 per-analysis max-tree) [1] waves [2] placed [3] multi-commit: candidates replayed, summed over waves;
+ * per-analysis: upper tree levels in global memory [4] multi-commit: waves that raised the candidate bar; per-analysis: upper tree
+ * levels in shared memory [5] grid [6] block [7] dynamic shared memory bytes [8..15] CTA 0's clock cycles per phase, summed
  * over waves (multi-commit: scan, barrier, merge+publish, gather, replay, row updates+recount; 0 for the other engines) */
 int  ccsim_run_stats(const ccsim_handle *h, int64_t out[16]);
 /* waves of the last run that the multi-commit kernel replayed in key order (single-use templates: the candidates ranked once, each
