@@ -45,6 +45,15 @@ struct DevOut {
                                    // [2] replay rounds, [3] waves replayed in key order
 };
 
+// DevParams::debug_flags, set from CCSIM_DEBUG_FLAGS (kernel experiments; INTEGRATION.md lists the same values)
+constexpr uint32_t DBG_RESCAN_EVERY_MOVE = 1u;    // a multi-commit wave ends at every PTS minimum move
+constexpr uint32_t DBG_RECOUNT_EVERY_WAVE = 2u;   // the multi-commit kernel recounts every PTS minimum after every wave
+constexpr uint32_t DBG_WAVE_LINES = 4u;           // one line per wave of the multi-commit kernel
+constexpr uint32_t DBG_CYCLES = 8u;               // replay / per-CTA cycle summary at the end of a run
+constexpr uint32_t DBG_STRICT_ONLY = 16u;         // strict multi-commit waves only (no look-ahead)
+constexpr uint32_t DBG_LOOKAHEAD_ALWAYS = 32u;    // look-ahead on every spread term in every wave
+constexpr uint32_t DBG_ARGMAX_ROUND = 64u;        // single-use multi-commit waves keep the arg-max replay round instead of key order
+
 struct DevParams {
   int32_t n;            // nodes of this shard
   int32_t n_global;     // nodes of the whole cluster
@@ -54,8 +63,7 @@ struct DevParams {
   int32_t chunk;        // nodes per CTA (contiguous ownership)
   int32_t rank, world;
   uint32_t epoch;       // run counter (1..255), folded into every exchanged word
-  uint32_t debug_flags; // CCSIM_DEBUG_FLAGS (kernel experiments): bit 0 = multi-commit waves end at every PTS minimum move, ...,
-                        // bit 6 = single-use multi-commit waves keep the arg-max round (INTEGRATION.md lists them all)
+  uint32_t debug_flags; // CCSIM_DEBUG_FLAGS (kernel experiments): the DBG_* bits below
   uint32_t xwave0;      // node-sharded runs: exchanges done by earlier runs of this handle; the double-buffer parity of the cross-GPU
                         // buffers continues across runs, so wave 0 of a run never lands in the buffer a lagging peer CTA still reads
   long long sample_k;   // numFeasibleNodesToFind (reference sampling mode)

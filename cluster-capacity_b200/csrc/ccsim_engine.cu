@@ -42,7 +42,6 @@
 #define BLOCK_THREADS 512
 #define MAX_WARPS (BLOCK_THREADS / 32)
 #define SMEM_CNT_MAX_INTS 16384      /* 64 KB of replicated counters in shared memory; above that: global replicas */
-#define WATCHDOG_SPINS (1u << 24)
 
 struct __align__(16) WaveShared {
   ccsim_template tmpl;                              // current template
@@ -1513,7 +1512,7 @@ extern "C" int ccsim_run(ccsim_handle *h, int64_t max_pods, ccsim_result *out) {
   CK(cudaStreamSynchronize(s));
   if (ho.error) return fail(h, CCSIM_ECUDA, "wave kernel aborted (error %d: %s)", ho.error, ho.error == 1 ? "exchange watchdog / output overflow" : "?");
   float ms = 0.f; CK(cudaEventElapsedTime(&ms, h->ev0, h->ev1));
-  if (stream && (p.debug_flags & 8u) && h->cfg.world == 1 && ho.waves > 0) {     // per-CTA cycle split of the streaming kernel (kernel experiments)
+  if (stream && (p.debug_flags & DBG_CYCLES) && h->cfg.world == 1 && ho.waves > 0) {     // per-CTA cycle split of the streaming kernel (kernel experiments)
     std::vector<unsigned long long> d((size_t)grid * 4);
     CK(cudaMemcpy(d.data(), h->d_xslots + XLINES_OFF, d.size() * 8, cudaMemcpyDeviceToHost));
     const char *nm[4] = {"mbarrier wait", "scan", "exchange", "rest"};

@@ -236,9 +236,60 @@ __device__ __forceinline__ uint32_t multi_raise_bar(uint32_t T, uint32_t kbest, 
   return (bsel >= MULTI_BINS) ? kbest : T + (uint32_t)(((unsigned long long)bsel * range + (MULTI_BINS - 1)) / MULTI_BINS);
 }
 
+// node shards: wait until the N (2 or 3) words at src — part of a peer's summary, written into this GPU's memory over NVLink — carry
+// this wave's tag; after WATCHDOG_SPINS polls the exchange is dead (ms.dead) and the words read as zeros
+template <int N>
+__device__ __forceinline__ void multi_poll_sys(const unsigned long long *src, uint32_t tag, unsigned long long (&w)[N]) {
+  static_assert(N == 2 || N == 3, "one 16-byte load, and one more word");
+  unsigned spins = 0;
+  for (;;) {
+    ld_line2<true>(src, w[0], w[1]);
+    if (N == 3) w[N - 1] = ld_slot_sys(src + 2);
+    bool ok = true;
+    #pragma unroll
+    for (int i = 0; i < N; i++) ok = ok && (uint32_t)(w[i] >> KEY_TAG_SHIFT) == tag;
+    if (ok) break;
+    if (++spins > WATCHDOG_SPINS) { ms.dead = 1; for (int i = 0; i < N; i++) w[i] = 0ull; break; }
+  }
+}
+
 // phase timers live in shared memory (thread 0 of CTA 0 only): registers are what this kernel is short of
 #define MPH_START() do { if (cta == 0 && tid == 0) ms.tc0 = clock64(); } while (0)
 #define MPH_MARK(i) do { if (cta == 0 && tid == 0) { const long long tc1_ = clock64(); ms.ph[i] += tc1_ - ms.tc0; ms.tc0 = tc1_; } } while (0)
+
+// ---- end of the run (the CTA that writes the output): the tables of the profiling builds; nothing in the shipped build ----
+__device__ __forceinline__ void multi_report(long long waves) {
+#ifdef MULTI_ROUND_PROFILE
+  {
+    const double w = (double)(waves), nr = (double)(ms.st_rounds > 0 ? ms.st_rounds : 1);
+    printf("round profile (CTA 0): waves %.0f rounds %lld | replay %.0f cycles/wave, set-up %.0f\n", w, ms.st_rounds, ms.ph[4] / w, ms.ph[6] / w);
+    printf("round profile: common round %lld events, %.0f cycles/round, %.0f cycles/wave\n", ms.rp_cnt[RP_ROUND], ms.rp_cyc[RP_ROUND] / nr, ms.rp_cyc[RP_ROUND] / w);
+    printf("round profile: wake-up rebuilds %lld, %.0f cycles each, %.0f cycles/wave\n", ms.rp_cnt[RP_REBUILD],
+           ms.rp_cyc[RP_REBUILD] / (double)(ms.rp_cnt[RP_REBUILD] > 0 ? ms.rp_cnt[RP_REBUILD] : 1), ms.rp_cyc[RP_REBUILD] / w);
+    printf("round profile: set-up: candidate load %.0f cycles/wave\n", ms.rp_cyc[RP_LOAD] / w);
+    printf("round profile: after the loop %lld waves, %.0f cycles/wave (hand-off %.0f, look-ahead decision %.0f)\n", ms.rp_cnt[RP_AFTER],
+           ms.rp_cyc[RP_AFTER] / w, ms.rp_cyc[RP_HANDOFF] / w, ms.rp_cyc[RP_DECIDE] / w);
+    printf("round profile: rounds with a non-zero kill mask %lld\n", ms.rp_cnt[RP_KILL]);
+    printf("round profile: key order %lld waves | ranking %.0f cycles/wave | common round %lld events, %.0f cycles/round, %.0f cycles/wave"
+           " | row advances %lld, %.0f cycles each, %.0f cycles/wave\n", ms.st_key_order,
+           ms.rp_cyc[RP_RANK] / (double)(ms.rp_cnt[RP_RANK] > 0 ? ms.rp_cnt[RP_RANK] : 1),
+           ms.rp_cnt[RP_KROUND], ms.rp_cyc[RP_KROUND] / (double)(ms.rp_cnt[RP_KROUND] > 0 ? ms.rp_cnt[RP_KROUND] : 1), ms.rp_cyc[RP_KROUND] / w,
+           ms.rp_cnt[RP_ADVANCE], ms.rp_cyc[RP_ADVANCE] / (double)(ms.rp_cnt[RP_ADVANCE] > 0 ? ms.rp_cnt[RP_ADVANCE] : 1), ms.rp_cyc[RP_ADVANCE] / w);
+    for (int q = 0; q < MULTI_GT; q++)
+      if (ms.rp_cnt[RP_MINMOVE + q])
+        printf("round profile: term %d minimum moves %lld, %.0f cycles each, %.0f cycles/wave\n", q, ms.rp_cnt[RP_MINMOVE + q],
+               ms.rp_cyc[RP_MINMOVE + q] / (double)ms.rp_cnt[RP_MINMOVE + q], ms.rp_cyc[RP_MINMOVE + q] / w);
+  }
+#endif
+#ifdef MULTI_GATHER_PROFILE
+  {
+    const double w = (double)(waves), nr = (double)(ms.gp_cnt[GP_RAISE] > 0 ? ms.gp_cnt[GP_RAISE] : 1);
+    printf("gather profile (CTA 0): waves %.0f | publish -> all own entries valid %.0f cycles/wave, %.1f poll rounds/wave | -> entries readable (G1) %.0f"
+           " | first append pass %.0f | bar raise %lld waves, %.0f cycles each, %.0f cycles/wave\n", w, ms.gp_cyc[GP_POLL] / w, ms.gp_cnt[GP_ROUNDS] / w,
+           ms.gp_cyc[GP_SYNC] / w, ms.gp_cyc[GP_APPEND] / w, ms.gp_cnt[GP_RAISE], ms.gp_cyc[GP_RAISE] / nr, ms.gp_cyc[GP_RAISE] / w);
+  }
+#endif
+}
 
 template <bool XGPU>
 __global__ void __launch_bounds__(LEAN_THREADS, 1) ccsim_wave_multi_kernel(const DevParams p, const LeanParams lp, const MultiParams mp) {
@@ -517,15 +568,9 @@ __global__ void __launch_bounds__(LEAN_THREADS, 1) ccsim_wave_multi_kernel(const
       if (tid < p.world) {
         int cr = 0;
         if (tid != p.rank && !dead) {
-          const unsigned long long *src = p.xslots_peer[p.rank] + XLINES_OFF + ((size_t)xpar * CCSIM_MAX_WORLD + tid) * CCSIM_MAX_GRID * SLOT_STRIDE;
-          unsigned long long a, b, c2;
-          unsigned spins = 0;
-          for (;;) {
-            ld_line2<true>(src, a, b); c2 = ld_slot_sys(src + 2);
-            if ((uint32_t)(a >> KEY_TAG_SHIFT) == tag && (uint32_t)(b >> KEY_TAG_SHIFT) == tag && (uint32_t)(c2 >> KEY_TAG_SHIFT) == tag) break;
-            if (++spins > WATCHDOG_SPINS) { ms.dead = 1; a = b = c2 = 0ull; break; }
-          }
-          xkb = (uint32_t)a; cr = (int)((a >> 32) & 0xfffu); xbar = (uint32_t)b; xtl = (uint32_t)c2;
+          unsigned long long h[3];
+          multi_poll_sys(p.xslots_peer[p.rank] + XLINES_OFF + ((size_t)xpar * CCSIM_MAX_WORLD + tid) * CCSIM_MAX_GRID * SLOT_STRIDE, tag, h);
+          xkb = (uint32_t)h[0]; cr = (int)((h[0] >> 32) & 0xfffu); xbar = (uint32_t)h[1]; xtl = (uint32_t)h[2];
           if (cr > MULTI_CAP) cr = MULTI_CAP;
         }
         ms.xcount[tid] = cr;
@@ -546,15 +591,9 @@ __global__ void __launch_bounds__(LEAN_THREADS, 1) ccsim_wave_multi_kernel(const
         int e = tid + u * LEAN_THREADS, r = 0;
         while (r < p.world && e >= ms.xcount[r]) { e -= ms.xcount[r]; r++; }
         if (r < p.world && !dead) {
-          const unsigned long long *src = p.xslots_peer[p.rank] + XLINES_OFF + ((size_t)xpar * CCSIM_MAX_WORLD + r) * CCSIM_MAX_GRID * SLOT_STRIDE + 4 + 2 * e;
-          unsigned long long a, b;
-          unsigned spins = 0;
-          for (;;) {
-            ld_line2<true>(src, a, b);
-            if ((uint32_t)(a >> KEY_TAG_SHIFT) == tag && (uint32_t)(b >> KEY_TAG_SHIFT) == tag) break;
-            if (++spins > WATCHDOG_SPINS) { ms.dead = 1; a = b = 0ull; break; }
-          }
-          rkey[u] = (uint32_t)a; rpay[u] = b;
+          unsigned long long w[2];
+          multi_poll_sys(p.xslots_peer[p.rank] + XLINES_OFF + ((size_t)xpar * CCSIM_MAX_WORLD + r) * CCSIM_MAX_GRID * SLOT_STRIDE + 4 + 2 * e, tag, w);
+          rkey[u] = (uint32_t)w[0]; rpay[u] = w[1];
         }
       }
       for (int pass = 0; pass < 2; pass++) {
@@ -584,7 +623,7 @@ __global__ void __launch_bounds__(LEAN_THREADS, 1) ccsim_wave_multi_kernel(const
     //      winner of every round is the first live candidate in key order. Rank them once, with the whole block (the other warps
     //      only wait at R): rank = the number of greater keys (keys are unique), counted by MULTI_RANK_PARTS threads per candidate
     //      over one span of the array each, then cnext[rank] = candidate. CCSIM_DEBUG_FLAGS bit 6 keeps the arg-max round. ----
-    const bool key_order = ms.single_use != 0 && !(p.debug_flags & 64u) && !dead;     // (block-uniform)
+    const bool key_order = ms.single_use != 0 && !(p.debug_flags & DBG_ARGMAX_ROUND) && !dead;     // (block-uniform)
     if (key_order) {
       const int i = tid % MULTI_CAP, part = tid / MULTI_CAP;
       if (i < C && part < MULTI_RANK_PARTS) {
@@ -743,8 +782,8 @@ __global__ void __launch_bounds__(LEAN_THREADS, 1) ccsim_wave_multi_kernel(const
             // a term scanned with look-ahead published the nodes of its closed cells: the move only matters when the new limit
             // reaches a cell that was not published; the cells in (old limit, new limit] wake their candidates up instead
             const bool rq = __shfl_sync(0xffffffffu, rlx, q) > 0;
-            if (rq) { rescan |= (lim_new >= __shfl_sync(0xffffffffu, unpub_min, q)) | (p.debug_flags & 1); woke = true; }
-            else rescan |= hit | (p.debug_flags & 1);
+            if (rq) { rescan |= (lim_new >= __shfl_sync(0xffffffffu, unpub_min, q)) | (p.debug_flags & DBG_RESCAN_EVERY_MOVE); woke = true; }
+            else rescan |= hit | (p.debug_flags & DBG_RESCAN_EVERY_MOVE);
             if (lane == q) { my_min = mn; my_num = num; c1.x = lim_new; lim_moved = true; sts_s32(MS_SA(gt_c1) + 16u * (uint32_t)q, lim_new); }
             RPROF(__syncwarp(); const long long rp_m1 = clock64(); RP_ADD(RP_MINMOVE + q, rp_m1 - rp_m0, 1); rp_mm += rp_m1 - rp_m0;)
           }
@@ -930,7 +969,7 @@ __global__ void __launch_bounds__(LEAN_THREADS, 1) ccsim_wave_multi_kernel(const
         //      the tiles' top-M lists). A look-ahead wave that could not place anything is repeated strictly. Every CTA of every rank
         //      decides alike (same counters, same replay). ----
         {
-          const bool strict_next = (acc == 0 && any_relax) || (p.debug_flags & 16u);
+          const bool strict_next = (acc == 0 && any_relax) || (p.debug_flags & DBG_STRICT_ONLY);
           const bool elig = lane < n_gt && gc.z >= 0 && gc.y > 0 && my_num <= MULTI_RELAX_K && c1.x < INT32_MAX - 2 * MULTI_RELAX_R && !strict_next;
           int32_t nrl = 0;
           for (unsigned nm = __ballot_sync(0xffffffffu, elig); nm; nm &= nm - 1) {
@@ -943,7 +982,7 @@ __global__ void __launch_bounds__(LEAN_THREADS, 1) ccsim_wave_multi_kernel(const
             closed = __reduce_add_sync(0xffffffffu, closed);
             if (lane == q && 2 * closed <= npres) nrl = MULTI_RELAX_R;
           }
-          if (p.debug_flags & 32u) nrl = (lane < n_gt && gc.z >= 0 && gc.y > 0 && c1.x < INT32_MAX - 2 * MULTI_RELAX_R && !strict_next) ? MULTI_RELAX_R : 0;   // tests: look-ahead on every PTS term, every wave
+          if (p.debug_flags & DBG_LOOKAHEAD_ALWAYS) nrl = (lane < n_gt && gc.z >= 0 && gc.y > 0 && c1.x < INT32_MAX - 2 * MULTI_RELAX_R && !strict_next) ? MULTI_RELAX_R : 0;   // tests: look-ahead on every PTS term, every wave
           if (lane < n_gt) sts_s32(MS_SA(relax) + 4u * (uint32_t)lds_s32(MS_SA(gt_term) + 4u * (uint32_t)lane), nrl);
           if (cta == 0 && lane == 0 && acc == 0 && any_relax) ms.st_empty++;
           RPROF(__syncwarp(); RP_ADD(RP_DECIDE, clock64() - rp_h1, 1);)
@@ -952,7 +991,7 @@ __global__ void __launch_bounds__(LEAN_THREADS, 1) ccsim_wave_multi_kernel(const
         if (lim_moved) { ls.terms[ms.gt_term[lane]].lim = c1.x; ms.gt_c1[lane][0] = c1.x; }
         if (lane < n_gt && gc.z >= 0) { ls.ptsmin[gc.z] = my_min; ls.ptsnum[gc.z] = my_num; }
       }
-      if (lane == 0 && cta == 0 && (p.debug_flags & 4))
+      if (lane == 0 && cta == 0 && (p.debug_flags & DBG_WAVE_LINES))
         printf("wave %lld k=%lld acc=%d C=%d T=%08x Tlist=%08x kbest=%08x delta=%08x ran_dry=%d look_ahead=%d first=%d last=%d\n", wv, k, acc, C, T, Tlist, kbest, delta,
                (int)ran_dry, (int)any_relax, acc ? ms.acc_node[0] : -1, acc ? ms.acc_node[acc - 1] : -1);
       if (lane == 0) {
@@ -988,7 +1027,7 @@ __global__ void __launch_bounds__(LEAN_THREADS, 1) ccsim_wave_multi_kernel(const
     k += acc;
     delta = ms.delta;
     if (ls.stop) break;
-    lean_pts_after_wave(p, smem_cnt, p.debug_flags & 2);
+    lean_pts_after_wave(p, smem_cnt, p.debug_flags & DBG_RECOUNT_EVERY_WAVE);
     wtag = (wtag == 4095u) ? 1u : wtag + 1u;
     tag = (p.epoch << 12) | wtag;
   }
@@ -999,39 +1038,12 @@ __global__ void __launch_bounds__(LEAN_THREADS, 1) ccsim_wave_multi_kernel(const
     o->examined = o->evals;
     for (int q = 0; q < 8; q++) o->phase_cycles[q] = ms.ph[q];
     o->stat[0] = ms.st_cand; o->stat[1] = ms.st_overflow; o->stat[2] = ms.st_rounds; o->stat[3] = ms.st_key_order;
-    if (p.debug_flags & 8u)
+    // (CCSIM_DEBUG_FLAGS bit 3's summary stays in the kernel body: a printf inlined from a helper puts its argument buffer ahead
+    //  of the MultiParams copy in the stack frame, which then grows from 136 to 192 bytes and takes a register more)
+    if (p.debug_flags & DBG_CYCLES)
       printf("multi-commit replay: waves %lld rounds %lld look-ahead waves %d (without a placement: %d) | cycles: replay %lld set-up %lld, per round %.0f\n",
              limit_hit ? wv : wv + 1, ms.st_rounds, ms.st_relaxed, ms.st_empty, ms.ph[4], ms.ph[6],
              (double)(ms.ph[4] - ms.ph[6]) / (double)(ms.st_rounds > 0 ? ms.st_rounds : 1));
-#ifdef MULTI_ROUND_PROFILE
-    {
-      const double w = (double)(limit_hit ? wv : wv + 1), nr = (double)(ms.st_rounds > 0 ? ms.st_rounds : 1);
-      printf("round profile (CTA 0): waves %.0f rounds %lld | replay %.0f cycles/wave, set-up %.0f\n", w, ms.st_rounds, ms.ph[4] / w, ms.ph[6] / w);
-      printf("round profile: common round %lld events, %.0f cycles/round, %.0f cycles/wave\n", ms.rp_cnt[RP_ROUND], ms.rp_cyc[RP_ROUND] / nr, ms.rp_cyc[RP_ROUND] / w);
-      printf("round profile: wake-up rebuilds %lld, %.0f cycles each, %.0f cycles/wave\n", ms.rp_cnt[RP_REBUILD],
-             ms.rp_cyc[RP_REBUILD] / (double)(ms.rp_cnt[RP_REBUILD] > 0 ? ms.rp_cnt[RP_REBUILD] : 1), ms.rp_cyc[RP_REBUILD] / w);
-      printf("round profile: set-up: candidate load %.0f cycles/wave\n", ms.rp_cyc[RP_LOAD] / w);
-      printf("round profile: after the loop %lld waves, %.0f cycles/wave (hand-off %.0f, look-ahead decision %.0f)\n", ms.rp_cnt[RP_AFTER],
-             ms.rp_cyc[RP_AFTER] / w, ms.rp_cyc[RP_HANDOFF] / w, ms.rp_cyc[RP_DECIDE] / w);
-      printf("round profile: rounds with a non-zero kill mask %lld\n", ms.rp_cnt[RP_KILL]);
-      printf("round profile: key order %lld waves | ranking %.0f cycles/wave | common round %lld events, %.0f cycles/round, %.0f cycles/wave"
-             " | row advances %lld, %.0f cycles each, %.0f cycles/wave\n", ms.st_key_order,
-             ms.rp_cyc[RP_RANK] / (double)(ms.rp_cnt[RP_RANK] > 0 ? ms.rp_cnt[RP_RANK] : 1),
-             ms.rp_cnt[RP_KROUND], ms.rp_cyc[RP_KROUND] / (double)(ms.rp_cnt[RP_KROUND] > 0 ? ms.rp_cnt[RP_KROUND] : 1), ms.rp_cyc[RP_KROUND] / w,
-             ms.rp_cnt[RP_ADVANCE], ms.rp_cyc[RP_ADVANCE] / (double)(ms.rp_cnt[RP_ADVANCE] > 0 ? ms.rp_cnt[RP_ADVANCE] : 1), ms.rp_cyc[RP_ADVANCE] / w);
-      for (int q = 0; q < MULTI_GT; q++)
-        if (ms.rp_cnt[RP_MINMOVE + q])
-          printf("round profile: term %d minimum moves %lld, %.0f cycles each, %.0f cycles/wave\n", q, ms.rp_cnt[RP_MINMOVE + q],
-                 ms.rp_cyc[RP_MINMOVE + q] / (double)ms.rp_cnt[RP_MINMOVE + q], ms.rp_cyc[RP_MINMOVE + q] / w);
-    }
-#endif
-#ifdef MULTI_GATHER_PROFILE
-    {
-      const double w = (double)(limit_hit ? wv : wv + 1), nr = (double)(ms.gp_cnt[GP_RAISE] > 0 ? ms.gp_cnt[GP_RAISE] : 1);
-      printf("gather profile (CTA 0): waves %.0f | publish -> all own entries valid %.0f cycles/wave, %.1f poll rounds/wave | -> entries readable (G1) %.0f"
-             " | first append pass %.0f | bar raise %lld waves, %.0f cycles each, %.0f cycles/wave\n", w, ms.gp_cyc[GP_POLL] / w, ms.gp_cnt[GP_ROUNDS] / w,
-             ms.gp_cyc[GP_SYNC] / w, ms.gp_cyc[GP_APPEND] / w, ms.gp_cnt[GP_RAISE], ms.gp_cyc[GP_RAISE] / nr, ms.gp_cyc[GP_RAISE] / w);
-    }
-#endif
+    multi_report(limit_hit ? wv : wv + 1);
   }
 }

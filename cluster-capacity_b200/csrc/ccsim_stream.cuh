@@ -189,8 +189,8 @@ __global__ void __launch_bounds__(STREAM_BLOCK, 1) ccsim_wave_stream_kernel(cons
 
   long long k = 0;
   bool limit_hit = false;
-  long long dbg_t = 0, dbg_wait = 0, dbg_scan = 0, dbg_xchg = 0, dbg_rest = 0;    // CCSIM_DEBUG_FLAGS & 8: this CTA's cycle split (thread 0)
-  const bool dbg = (p.debug_flags & 8u) != 0u && tid == 0;
+  long long dbg_t = 0, dbg_wait = 0, dbg_scan = 0, dbg_xchg = 0, dbg_rest = 0;    // DBG_CYCLES: this CTA's cycle split (thread 0)
+  const bool dbg = (p.debug_flags & DBG_CYCLES) != 0u && tid == 0;
   // Warp specialisation. Warps 0..15 SCAN. Warp 16, the EXCHANGE warp, publishes the CTA's key, requests the next wave's bulk
   // copies and polls: a wave's critical path is scan -> barrier A -> publish / poll (one L2 round trip) -> barrier B -> next scan.
   // Warp 17, the COMMIT warp, is decoupled from those barriers: it takes the winners from a small ring in shared memory and, when
