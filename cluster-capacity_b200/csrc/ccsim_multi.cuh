@@ -41,7 +41,8 @@
 //   those cycles (scripts/round_profile.sh). Work around the round stays on this warp: moved onto the whole block (the set-up
 //   between G1 and G2, the look-ahead decision after R) it measured slower on C4, whose terms have 8 and 64 domains.
 //   Row updates of the winners are done by each node's own thread after that barrier (a thread owns its node).
-// Key order (single-use templates: no second lives): the block ranks the wave's candidates once after compaction, and the replay
+// Key order (single-use templates: no second lives): the compaction stores the wave's candidates in key order (node shards: the
+//   block ranks them after the second gather level), and the replay
 //   warp holds them in rows of 32 in key order; a round is ballot(live) -> the lowest live lane -> one SHFL of its payload -> the same
 //   commit -> the kill test on each lane's one slot. A row is judged by a full cell test when the replay reaches it; a wake-up goes
 //   back to row 0 (see "the round in key order" below). C4: 778 -> 515 profiled cycles per round, kernel time 21.67-21.72 ->
@@ -68,13 +69,16 @@
 #define MULTI_CPT 8               /* candidates per replay lane */
 #endif
 #define MULTI_CAP (32 * MULTI_CPT)
-#define MULTI_BINS 64
+#define MULTI_LEVELS 4            /* compaction: score levels below the best key it ranks (one 16-bit count per level in a 64-bit word) */
+#define MULTI_GROUPS (MULTI_EPT * LEAN_WARPS)   /* compaction: groups of 32 gathered entries (two lists), one count word each */
+#define MULTI_BINS 64             /* node shards, gather level 2: histogram bins of the bar raise */
 #define MULTI_RELAX_K 8           /* look-ahead on a PTS term when at most this many of its domains still sit at the global minimum ... */
 #define MULTI_RELAX_R 3           /* ... nodes in cells up to this far over the limit are published as dormant candidates */
 #define MULTI_XPT (((CCSIM_MAX_WORLD - 1) * MULTI_CAP + LEAN_THREADS - 1) / LEAN_THREADS)   /* node shards: remote candidates per thread */
-#define MULTI_RANK_PARTS (LEAN_THREADS / MULTI_CAP)                       /* key order: threads that count one candidate's rank ... */
+#define MULTI_RANK_PARTS (LEAN_THREADS / MULTI_CAP)                       /* node shards, key order: threads that count one candidate's rank ... */
 #define MULTI_RANK_SPAN (((MULTI_CAP + MULTI_RANK_PARTS - 1) / MULTI_RANK_PARTS + 3) & ~3)   /* ... each over this many keys (16-byte loads) */
 static_assert(MULTI_RANK_PARTS >= 1 && MULTI_RANK_SPAN < 256, "key order: a partial rank fits a byte");
+static_assert(MULTI_GROUPS <= 96 && MULTI_EPT * LEAN_THREADS < 65536, "compaction: three count words per lane, a count fits 16 bits");
 static_assert(MULTI_CPT <= 32, "key order: one won bit per row");
 static_assert(MULTI_M == SLOT_STRIDE, "the keys of a CTA's list fill exactly one slot line");
 static_assert(4 + 2 * MULTI_CAP <= CCSIM_MAX_GRID * SLOT_STRIDE, "node shards: a rank's summary fits its region of the line buffer");
@@ -93,7 +97,7 @@ static_assert(4 + 2 * MULTI_CAP <= CCSIM_MAX_GRID * SLOT_STRIDE, "node shards: a
 #define RP_HANDOFF 5              /* after the loop: winners -> ms.mult */
 #define RP_DECIDE 6               /* after the loop: the next wave's look-ahead decision */
 #define RP_MINMOVE 7              /* + term q */
-#define RP_RANK (RP_MINMOVE + MULTI_GT)   /* key order: ranking the wave's candidates (block-wide, up to the barrier after it) */
+#define RP_RANK (RP_MINMOVE + MULTI_GT)   /* node shards, key order: ranking the wave's candidates (block-wide, up to the barrier after it) */
 #define RP_KROUND (RP_RANK + 1)   /* key order: the common round (ballot -> commit -> kill) */
 #define RP_ADVANCE (RP_RANK + 2)  /* key order: moving on to the next row (loads + full cell test), per row loaded */
 #define RP_N (RP_RANK + 3)
@@ -108,13 +112,13 @@ static_assert(4 + 2 * MULTI_CAP <= CCSIM_MAX_GRID * SLOT_STRIDE, "node shards: a
 // Gather profile (profiling builds only: -DMULTI_GATHER_PROFILE; the hooks expand to nothing otherwise). CTA 0 adds up, per wave:
 // the cycles from its own publish to the poll round in which the last of its entries was valid (the latest of its threads), and
 // the number of poll rounds (the most any thread took); from there to the point where the CTA may read every entry (G1); the
-// first append pass up to G2; the bar-raise path (histogram, raise, second pass) and how often it ran. Every CTA also writes its
-// %globaltimer at publish into gp_pub_ns[wave][CTA]; the host reports the skew of the publishes, latest minus CTA 0's, per wave.
-// scripts/gather_profile.sh prints both.
+// compaction in key order up to the barrier after its stores (G3), and in how many waves the level clamp raised the bar. Every CTA
+// also writes its %globaltimer at publish into gp_pub_ns[wave][CTA]; the host reports the skew of the publishes, latest minus CTA
+// 0's, per wave. scripts/gather_profile.sh prints both.
 #define GP_POLL 0
 #define GP_SYNC 1
-#define GP_APPEND 2
-#define GP_RAISE 3
+#define GP_COMPACT 2
+#define GP_CLAMP 3                /* (event count only) */
 #define GP_ROUNDS 4               /* (event count only) */
 #define GP_N 5
 #define GP_MAX_WAVES 4096         /* waves with a publish time */
@@ -136,9 +140,10 @@ struct __align__(16) MultiShared {
   uint32_t wtop[LEAN_WARPS][MULTI_M];               // per-warp top-M (compact) keys of this wave
   int32_t gt_c1[MULTI_GT][4];                       // per replicated-counter term: {limit, payload shift, payload mask, domains of the counter}
   int32_t gt_commit[MULTI_GT][4];                   // ... {counter base, inc, PTS constraint tracked or -1, n_present}
-  uint32_t ckey[MULTI_CAP], cdom[MULTI_CAP], cnext[MULTI_CAP];   // the wave's candidates keyed >= T (unordered); in a key-order wave
-                                                                 // (no second lives) cnext[r] = the candidate of rank r
-  uint8_t kpart[MULTI_RANK_PARTS][MULTI_CAP];       // key order: partial ranks (keys greater than candidate i in one span of the array)
+  uint32_t ckey[MULTI_CAP], cdom[MULTI_CAP], cnext[MULTI_CAP];   // the wave's candidates keyed >= T, in key order (node shards:
+                                                                 // unordered, and in a key-order wave cnext[r] = the candidate of rank r)
+  unsigned long long gcnt[MULTI_GROUPS];            // compaction: per group of 32 gathered entries, its candidates per level (16 bits each)
+  uint8_t kpart[MULTI_RANK_PARTS][MULTI_CAP];       // node shards, key order: partial ranks (keys greater than candidate i in one span)
   uint32_t red[LEAN_WARPS], red2[LEAN_WARPS];       // block reductions (T, best key)
   uint32_t hist[MULTI_BINS];
   int32_t wfeas[LEAN_WARPS];
@@ -192,7 +197,7 @@ __device__ __forceinline__ int nth_set_lane(unsigned m, int g) {
   return m ? __ffs(m) - 1 : -1;
 }
 
-// warp-aggregated append of the lanes' candidates to the wave's candidate arrays (order does not matter: keys are unique)
+// node shards, gather level 2: warp-aggregated append of the lanes' candidates to the wave's candidate arrays (unordered: keys are unique)
 __device__ __forceinline__ void multi_append(bool keep, uint32_t ck, unsigned long long b, int lane) {
   const unsigned m = __ballot_sync(0xffffffffu, keep);
   if (m) {
@@ -209,8 +214,8 @@ __device__ __forceinline__ void multi_append(bool keep, uint32_t ck, unsigned lo
   }
 }
 
-// More candidates than the replay holds: the bar T is raised to the lowest of MULTI_BINS equal steps between T and the best key
-// that leaves <= MULTI_CAP candidates; every CTA sees the same data and decides alike. The caller zeroes ms.hist; after a barrier
+// Node shards, gather level 2: more candidates than the replay holds. The bar T is raised to the lowest of MULTI_BINS equal steps
+// between T and the best key that leaves <= MULTI_CAP candidates; every CTA sees the same data and decides alike. The caller zeroes ms.hist; after a barrier
 // it counts its candidates into it with multi_hist_add and empties the candidate arrays (multi_bar_reset: every thread has read
 // ms.ncand before that barrier); after one more barrier multi_raise_bar returns the new T. Every warp computes it alike from the
 // histogram, so no barrier follows: the next write of ms.hist or ms.ncand is behind the barrier that ends the second append pass.
@@ -283,10 +288,10 @@ __device__ __forceinline__ void multi_report(long long waves) {
 #endif
 #ifdef MULTI_GATHER_PROFILE
   {
-    const double w = (double)(waves), nr = (double)(ms.gp_cnt[GP_RAISE] > 0 ? ms.gp_cnt[GP_RAISE] : 1);
+    const double w = (double)(waves);
     printf("gather profile (CTA 0): waves %.0f | publish -> all own entries valid %.0f cycles/wave, %.1f poll rounds/wave | -> entries readable (G1) %.0f"
-           " | first append pass %.0f | bar raise %lld waves, %.0f cycles each, %.0f cycles/wave\n", w, ms.gp_cyc[GP_POLL] / w, ms.gp_cnt[GP_ROUNDS] / w,
-           ms.gp_cyc[GP_SYNC] / w, ms.gp_cyc[GP_APPEND] / w, ms.gp_cnt[GP_RAISE], ms.gp_cyc[GP_RAISE] / nr, ms.gp_cyc[GP_RAISE] / w);
+           " | compaction in key order %.0f | bar over %d levels raised in %lld waves\n", w, ms.gp_cyc[GP_POLL] / w, ms.gp_cnt[GP_ROUNDS] / w,
+           ms.gp_cyc[GP_SYNC] / w, ms.gp_cyc[GP_COMPACT] / w, MULTI_LEVELS, ms.gp_cnt[GP_CLAMP]);
   }
 #endif
 }
@@ -517,26 +522,65 @@ __global__ void __launch_bounds__(LEAN_THREADS, 1) ccsim_wave_multi_kernel(const
     // previous waves (doubled when the replay ran out of candidates above an artificial bar, shrunk when too many qualified).
     // Every CTA of every rank computes the same sequence from the same exchanged data.
     uint32_t T = max(Tlist, kbest > delta ? kbest - delta : 0u);
-    // ---- the entries keyed >= T go into shared memory (unordered; keys are unique) ----
+    // ---- the entries keyed >= T go into shared memory in key order, straight to their ranks. Every list is sorted (keys descending,
+    //      then zeros), so its entries keyed >= T are a prefix of it, and list l is tile l: a lower list holds lower node indices, which
+    //      rank higher at the same score. An entry's level is its score's distance below the best key's score. Entry u of warp w's
+    //      threads lies in group g = w + LEAN_WARPS * u of 32 entries: lists 2g and 2g + 1, in lane order. So a candidate's rank is
+    //        #(candidates on higher levels) + #(candidates on its level in groups < g) + #(candidates on its level in lanes < its lane),
+    //      exact because keys are unique. Per-level ballots give the last term and the group's counts, one barrier publishes the
+    //      counts (one 64-bit word per group), and every warp sums what it needs of them itself.
+    //      At most MULTI_LEVELS levels are ranked: when the candidates span more, the bar goes up to the lowest key of the lowest
+    //      level ranked. More than MULTI_CAP candidates: the bar is the key of rank MULTI_CAP - 1. Either bar is above T, and any bar
+    //      above T is valid: the best candidate is still in, and a strict wave places it. ----
     int C = 0;
-    for (int pass = 0; pass < 2 && !dead; pass++) {
+    if (!dead) {
+      const uint32_t kbl = kbest >> MULTI_IDX_BITS;
+      int rk[MULTI_EPT];                       // the entry's level << 8 | its place among the group's candidates on that level; -1: none
+      bool beyond = false;                     // a candidate more than MULTI_LEVELS - 1 levels below the best key
       #pragma unroll
       for (int u = 0; u < MULTI_EPT; u++) {
-        const uint32_t ck = (uint32_t)ea[u];
-        if (u * LEAN_THREADS < tot) multi_append(ck != 0u && ck >= T, ck, eb[u], lane);      // (warp-uniform guard: warps beyond the entries skip)
+        const uint32_t ck = (uint32_t)ea[u];   // (0 beyond the entries)
+        const bool q = ck != 0u && ck >= T;
+        const uint32_t lv = kbl - (ck >> MULTI_IDX_BITS);
+        beyond |= q && lv >= MULTI_LEVELS;
+        unsigned long long wc = 0ull;
+        int pos = 0;
+        #pragma unroll
+        for (int v = 0; v < MULTI_LEVELS; v++) {
+          const unsigned b = __ballot_sync(0xffffffffu, q && lv == (uint32_t)v);
+          wc |= (unsigned long long)__popc(b) << (16 * v);
+          if (lv == (uint32_t)v) pos = __popc(b & ((1u << lane) - 1u));
+        }
+        rk[u] = (q && lv < MULTI_LEVELS) ? (int)(lv << 8) | pos : -1;
+        if (lane == 0) ms.gcnt[warp + LEAN_WARPS * u] = wc;
       }
-      __syncthreads();                                                  // G2
-      C = ms.ncand;
-      GPROF(if (cta == 0 && tid == 0) { const long long t2 = clock64(); ms.gp_cyc[pass ? GP_RAISE : GP_APPEND] += t2 - gp_t; ms.gp_cnt[pass ? GP_RAISE : GP_APPEND]++; gp_t = t2; })
-      if (C <= MULTI_CAP || pass == 1) break;
-      if (tid < MULTI_BINS) ms.hist[tid] = 0u;
-      __syncthreads();
-      const unsigned long long range = (unsigned long long)(kbest - T) + 1ull;
+      const bool clamp = __syncthreads_or(beyond);                      // G2
+      // lane l sums groups l, l + 32, l + 64: all of them (the candidates per level), and those before each of this warp's groups
+      const unsigned long long g0 = ms.gcnt[lane], g1 = ms.gcnt[lane + 32], g2 = lane + 64 < MULTI_GROUPS ? ms.gcnt[lane + 64] : 0ull;
+      const unsigned long long gs = g0 + g1 + g2;
+      const unsigned long long S = ((unsigned long long)__reduce_add_sync(0xffffffffu, (uint32_t)(gs >> 32)) << 32) | __reduce_add_sync(0xffffffffu, (uint32_t)gs);
+      const unsigned long long Sabove = S * 0x0001000100010000ull;    // field v: the candidates on levels < v
+      const int total = (int)((S * 0x0001000100010001ull) >> 48);
       #pragma unroll
-      for (int u = 0; u < MULTI_EPT; u++) multi_hist_add((uint32_t)ea[u], T, range);
-      multi_bar_reset(cta);
-      __syncthreads();
-      T = multi_raise_bar(T, kbest, range);
+      for (int u = 0; u < MULTI_EPT; u++) {
+        const int g = warp + LEAN_WARPS * u;
+        const unsigned long long ps = (lane < g ? g0 : 0ull) + (lane + 32 < g ? g1 : 0ull) + (lane + 64 < g ? g2 : 0ull);
+        const unsigned long long P = ((unsigned long long)__reduce_add_sync(0xffffffffu, (uint32_t)(ps >> 32)) << 32) | __reduce_add_sync(0xffffffffu, (uint32_t)ps);
+        if (rk[u] >= 0) {
+          const int r = (int)(((Sabove + P) >> (16 * (rk[u] >> 8))) & 0xffffu) + (rk[u] & 0xff);
+          if (r < MULTI_CAP) {
+            ms.ckey[r] = (uint32_t)ea[u];
+            ms.cdom[r] = (uint32_t)eb[u] & ((1u << MULTI_PAY_BITS) - 1u);
+            ms.cnext[r] = (uint32_t)(eb[u] >> MULTI_NEXT_SHIFT) & 0xfffu;
+          }
+        }
+      }
+      if (clamp) T = (kbl - (MULTI_LEVELS - 1)) << MULTI_IDX_BITS;
+      if (cta == 0 && tid == 0 && total > MULTI_CAP) ms.st_overflow++;
+      __syncthreads();                                                  // G3
+      if (total > MULTI_CAP) T = ms.ckey[MULTI_CAP - 1];
+      C = min(total, MULTI_CAP);
+      GPROF(if (cta == 0 && tid == 0) { const long long t2 = clock64(); ms.gp_cyc[GP_COMPACT] += t2 - gp_t; ms.gp_cnt[GP_CLAMP] += clamp; gp_t = t2; })
     }
     if (XGPU) {
       // ---- gather, level 2 (node shards): every rank now holds ITS candidates keyed >= its bar T_r (<= MULTI_CAP of them, the same in
@@ -620,11 +664,12 @@ __global__ void __launch_bounds__(LEAN_THREADS, 1) ccsim_wave_multi_kernel(const
     if (cta == 0 && tid == 0) ms.st_cand += C;
     MPH_MARK(3);
     // ---- key order (single-use templates): no candidate comes back after it wins, so its key stands for the whole wave and the
-    //      winner of every round is the first live candidate in key order. Rank them once, with the whole block (the other warps
-    //      only wait at R): rank = the number of greater keys (keys are unique), counted by MULTI_RANK_PARTS threads per candidate
-    //      over one span of the array each, then cnext[rank] = candidate. CCSIM_DEBUG_FLAGS bit 6 keeps the arg-max round. ----
+    //      winner of every round is the first live candidate in key order. One GPU: the compaction stored them in key order. Node
+    //      shards: the second gather level appends them unordered, so the block ranks them (the other warps only wait at R): rank =
+    //      the number of greater keys (keys are unique), counted by MULTI_RANK_PARTS threads per candidate over one span of the array
+    //      each, then cnext[rank] = candidate. CCSIM_DEBUG_FLAGS bit 6 keeps the arg-max round. ----
     const bool key_order = ms.single_use != 0 && !(p.debug_flags & DBG_ARGMAX_ROUND) && !dead;     // (block-uniform)
-    if (key_order) {
+    if (XGPU && key_order) {
       const int i = tid % MULTI_CAP, part = tid / MULTI_CAP;
       if (i < C && part < MULTI_RANK_PARTS) {
         const uint32_t mine = ms.ckey[i];
@@ -810,7 +855,7 @@ __global__ void __launch_bounds__(LEAN_THREADS, 1) ccsim_wave_multi_kernel(const
             __syncwarp();                      // the counter cells / limits written by the term lanes, before every lane reads them
             const int idx = row * 32 + lane;
             const bool present = idx < C;
-            const uint32_t o = present ? (uint32_t)lds_s32(MS_SA(cnext) + 4u * (uint32_t)idx) : 0u;
+            const uint32_t o = !present ? 0u : (XGPU ? (uint32_t)lds_s32(MS_SA(cnext) + 4u * (uint32_t)idx) : (uint32_t)idx);   // (node shards: ranked)
             kk = present ? (uint32_t)lds_s32(MS_SA(ckey) + 4u * o) : 0u;
             kd = present ? (uint32_t)lds_s32(MS_SA(cdom) + 4u * o) : 0u;   // (0: no field, every cell read is cell 0 of its counter)
             // the full cell test. The term constants come from the term lanes' registers (lane q holds term q's current limit;
