@@ -467,6 +467,15 @@ struct CommitInfo {
 #ifndef WATCHDOG_SPINS
 #define WATCHDOG_SPINS (1u << 24)
 #endif
+// CTA 0's cycles per phase of the lean and generic kernels; the kernel declares ph[8], tc0 and tc1 in CCSIM_PHASE_TIMERS builds
+#ifdef CCSIM_PHASE_TIMERS
+#define PH_START() do { if (cta == 0 && tid == 0) tc0 = clock64(); } while (0)
+#define PH_MARK(i) do { if (cta == 0 && tid == 0) { tc1 = clock64(); ph[i] += tc1 - tc0; tc0 = tc1; } } while (0)
+#else
+#define PH_START() do {} while (0)
+#define PH_MARK(i) do {} while (0)
+#endif
+
 // Second level of the per-wave exchange for node-sharded multi-GPU runs (warp 0 of every CTA, after the intra-GPU gather):
 // CTA 0 stores this GPU's class winners, tagged, into EVERY rank's exchange buffer (P2P stores over NVLink; 8-byte stores
 // are single transactions, the tag inside the word validates it), then every CTA polls its LOCAL copy for all ranks.

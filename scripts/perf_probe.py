@@ -1,5 +1,5 @@
 """Quick device-time probe of the wave kernel on the BASELINE configs (not the bench contract; see bench.py)."""
-import importlib, sys, os, time
+import hashlib, importlib, sys, os, time
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np
 abi = importlib.import_module("cluster-capacity_b200._abi")
@@ -16,7 +16,8 @@ def probe(name, snap, tmpl, ctr, limit, bytes_per_eval, engine_kind=abi.ENGINE_A
     us = r.run_ms * 1e3 / max(1, r.waves)
     print("%-28s n=%-8d grid=%-4d placed=%-8d waves=%-8d run=%9.3f ms  %6.2f us/wave  %.3g evals/s  %.0f GB/s algorithmic  (load %.1f ms)" % (
         name, snap.n, info["grid"], r.placed, r.waves, r.run_ms, us, r.evals / (r.run_ms * 1e-3),
-        r.evals * bytes_per_eval / (r.run_ms * 1e-3) / 1e9, (t1 - t0) * 1e3), flush=True)
+        r.evals * bytes_per_eval / (r.run_ms * 1e-3) / 1e9, (t1 - t0) * 1e3), end="")
+    print("  %s  pod->node sha1 %s" % (st["kernel"], hashlib.sha1(r.pod_node.tobytes()).hexdigest()[:16]), flush=True)
     if st["engine"] == "multi-commit":
         w = max(1, st["waves"])
         print("    engine=%s  placements/wave=%.2f  candidates/wave=%.1f  bar raised in %d waves  cycles/wave (CTA 0): scan=%d S1=%d merge+publish=%d gather=%d replay=%d tail=%d  smem=%d B" % (
@@ -35,3 +36,19 @@ if __name__ == "__main__":
         probe("C4 spread-only", snap, tmpl, ctr[:3], 20000, 92)
         probe("C4 spread-only, sequential", snap, tmpl, ctr[:3], 20000, 92, abi.ENGINE_SEQUENTIAL)
     if "c5" in which: probe("C5 1M x 64 templates", *synth.c5(), 6400, 72)
+    if "generic" in which:       # the generic wave kernel, which bench.py never reaches: normalised soft scorers and eight
+        sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests"))
+        import helpers           # PreferNoSchedule classes with an extended-resource request, resident and one node past the tile
+        def classes(n):
+            rng = np.random.Generator(np.random.PCG64(81))
+            a_cpu, a_mem, a_pods, r_cpu, r_mem, npods = synth._c2_nodes(n, rng)
+            taint = (np.uint64(1) << rng.integers(0, 8, n).astype(np.uint64)) - np.uint64(1)
+            snap = abi.Snapshot(n, a_cpu, a_mem, a_pods, req_cpu=r_cpu, req_mem=r_mem, npods=npods, taint_mask=taint.reshape(1, n),
+                                taint_prefer=[0x7F], scalars=[(rng.integers(0, 40, n), rng.integers(0, 4, n))])
+            t = abi.default_template(150, 100 << 20)
+            t.req_scalar[0] = 1
+            return snap, [t], []
+        probe("generic soft 100k", *helpers.soft_cluster(89, n=100_000), 3000, 0)
+        probe("generic 8 classes 100k", *classes(100_000), 5000, 0)
+        n = helpers.largest_n(classes, "wave<true>", 100_000, 1_000_000, max_pods=5000) + 1
+        probe("generic past the tile", *classes(n), 5000, 0)

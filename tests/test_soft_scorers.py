@@ -23,7 +23,7 @@ from oracle import binding as oracle  # noqa: E402
 
 GiB, MiB = 1 << 30, 1 << 20
 AUTO, SEQ = abi.ENGINE_AUTO, abi.ENGINE_SEQUENTIAL
-SMEM_CNT_MAX_INTS = 16384       # counters beyond this many ints live as per-CTA replicas in global memory (ccsim_engine.cu)
+SMEM_CNT_MAX_INTS = 16384       # counters beyond this many ints live as per-CTA replicas in global memory (ccsim_wave.cuh)
 
 # static bits of the generated snapshots
 B_IGNORED, B_HOST = 0, 1        # IgnoredNodes of explicit constraints; "node carries kubernetes.io/hostname"
