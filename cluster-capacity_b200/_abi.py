@@ -103,6 +103,12 @@ class Counter(C.Structure):
                 ("inc", C.c_int32), ("elig_bit", C.c_int32), ("pad", C.c_int32), ("init", P32)]
 
 
+class AnalysisTerms(C.Structure):
+    """ccsim_analysis_terms: one analysis's own counters and topology columns (ccsim_set_analyses)."""
+    _fields_ = [("n_counters", C.c_int32), ("n_topo_cols", C.c_int32), ("counters", C.POINTER(Counter)),
+                ("topo", P32 * MAX_TOPO_COLS)]
+
+
 class Pts(C.Structure):
     _fields_ = [("counter", C.c_int32), ("max_skew", C.c_int32), ("self_match", C.c_int32),
                 ("min_zero", C.c_int32)]

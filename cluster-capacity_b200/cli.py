@@ -4,7 +4,8 @@ top of the GPU path:
     python -m cluster-capacity_b200.cli --podspec examples/pod.yaml --snapshot cluster.json [--max-limit N]
            [--exclude-nodes a,b] [--default-config cfg.yaml] [--verbose] [-o json|yaml] [--kubeconfig KUBECONFIG]
     (--podspec may be repeated or name a directory: several podspecs are simulated round-robin, e.g. the genpod output of 64 namespaces;
-     with --each every podspec is analysed on its own, as if `cluster-capacity --podspec <file>` ran once per file)
+     with --each every podspec is analysed on its own, as if `cluster-capacity --podspec <file>` ran once per file, hard topology
+     spread, required pod (anti-)affinity and hostPorts included)
 
 The analysis needs the LISTed Node/Pod/Namespace objects. `--snapshot` takes a JSON/YAML file
 {"nodes": [...], "pods": [...], "namespaces": [...]} (or a directory with nodes.json / pods.json / namespaces.json);
@@ -127,7 +128,8 @@ def main(argv=None):
     ap.add_argument("--snapshot", default="", help="Node/Pod/Namespace lists as a file or directory (instead of a live API server)")
     ap.add_argument("--each", action="store_true",
                     help="Analyse every podspec of --podspec on its own against the same snapshot (one review per podspec, in order; "
-                         "-o json prints them as one JSON array, -o yaml separates them by ---).")
+                         "-o json prints them as one JSON array, -o yaml separates them by ---). Podspecs may carry hard topology spread, "
+                         "required pod (anti-)affinity and hostPorts; normalised soft scorers are refused.")
     ap.add_argument("--device", type=int, default=0)
     a = ap.parse_args(argv)
     if not a.podspec:
@@ -144,9 +146,12 @@ def main(argv=None):
             else:
                 files.append(path)
         pods = [parse_api_spec(f) for f in files]
-        pod = pods if a.each else (pods[0] if len(pods) == 1 else pods)
         objs = load_snapshot(a.snapshot) if a.snapshot else list_from_cluster(a.kubeconfig)
-        cc = fw.New(load_scheduler_config(a.default_config), None, pod, a.max_limit, [x for x in a.exclude_nodes.split(",") if x], device=a.device)
+        excl = [x for x in a.exclude_nodes.split(",") if x]
+        if a.each:
+            cc = fw.NewEach(load_scheduler_config(a.default_config), None, pods, a.max_limit, excl, device=a.device)
+        else:
+            cc = fw.New(load_scheduler_config(a.default_config), None, pods[0] if len(pods) == 1 else pods, a.max_limit, excl, device=a.device)
         cc.SyncWithClient(fw.ListClient(objs["nodes"], objs["pods"], objs["namespaces"], objs["services"], objs["replicationcontrollers"],
                                         objs["replicasets"], objs["statefulsets"]))
         for w in cc.Warnings():

@@ -229,8 +229,16 @@ struct Tile {
 
 // one thread: fold template t into FilterConsts. topo_ptr[k] / cnt_ptr[j] are the (pre-offset) bases of topology
 // column k and of counter j as this CTA sees them.
-__device__ void build_filter_consts(const DevParams &p, const ccsim_template &t, int32_t ti, const int32_t *const *topo_ptr,
-                                    int32_t *const *cnt_ptr, const int32_t *ptsmin, long long aff_total, FilterConsts &fc) {
+// PodTopologySpread's Filter bound for a domain count (filtering.go:341-351): reject when cnt > maxSkew - selfMatch + globalMin
+__device__ __forceinline__ int32_t pts_limit(const ccsim_pts &pc, int32_t ptsmin) {
+  const long long lim = (long long)pc.max_skew - pc.self_match + (long long)ptsmin;
+  return lim > INT32_MAX ? INT32_MAX : (lim < INT32_MIN ? INT32_MIN : (int32_t)lim);
+}
+
+// counters: the counter table t's indexes refer to (p.counters, or a per-analysis table of ccsim_run_each)
+__device__ void build_filter_consts(const DevParams &p, const DevCounter *counters, const ccsim_template &t, int32_t ti,
+                                    const int32_t *const *topo_ptr, int32_t *const *cnt_ptr, const int32_t *ptsmin, long long aff_total,
+                                    FilterConsts &fc) {
   const uint32_t fe = t.filter_enable, fl = t.flags;
   fc.tmpl_index = ti;
   unsigned long long tb = 0ull;
@@ -262,26 +270,29 @@ __device__ void build_filter_consts(const DevParams &p, const ccsim_template &t,
   fc.extras = x;
   fc.n_pts = (fe & CCSIM_PL_POD_TOPOLOGY_SPREAD) ? t.n_pts : 0;
   for (int c = 0; c < fc.n_pts; c++) {
-    const DevCounter &dc = p.counters[t.pts[c].counter];
+    const DevCounter &dc = counters[t.pts[c].counter];
     fc.pts[c].col = dc.topo_col < 0 ? nullptr : topo_ptr[dc.topo_col];
     fc.pts[c].cnt = cnt_ptr[t.pts[c].counter];
-    const long long lim = (long long)t.pts[c].max_skew - t.pts[c].self_match + (long long)ptsmin[c];
-    fc.pts_lim[c] = lim > INT32_MAX ? INT32_MAX : (lim < INT32_MIN ? INT32_MIN : (int32_t)lim);
+    fc.pts_lim[c] = pts_limit(t.pts[c], ptsmin[c]);
   }
   const bool ipa = (fe & CCSIM_PL_INTER_POD_AFFINITY) != 0;
   fc.n_aff = ipa ? t.n_aff : 0;
   fc.n_anti = ipa ? t.n_anti : 0;
   for (int a = 0; a < fc.n_aff; a++) {
-    const DevCounter &dc = p.counters[t.aff_counter[a]];
+    const DevCounter &dc = counters[t.aff_counter[a]];
     fc.aff[a].col = dc.topo_col < 0 ? nullptr : topo_ptr[dc.topo_col];
     fc.aff[a].cnt = cnt_ptr[t.aff_counter[a]];
   }
   for (int a = 0; a < fc.n_anti; a++) {
-    const DevCounter &dc = p.counters[t.anti_counter[a]];
+    const DevCounter &dc = counters[t.anti_counter[a]];
     fc.anti[a].col = dc.topo_col < 0 ? nullptr : topo_ptr[dc.topo_col];
     fc.anti[a].cnt = cnt_ptr[t.anti_counter[a]];
   }
   fc.aff_bypass = (aff_total == 0 && (fl & CCSIM_TF_AFF_SELF_MATCH_ALL)) ? 1 : 0;
+}
+__device__ __forceinline__ void build_filter_consts(const DevParams &p, const ccsim_template &t, int32_t ti, const int32_t *const *topo_ptr,
+                                                    int32_t *const *cnt_ptr, const int32_t *ptsmin, long long aff_total, FilterConsts &fc) {
+  build_filter_consts(p, p.counters, t, ti, topo_ptr, cnt_ptr, ptsmin, aff_total, fc);
 }
 
 // status codes for the diagnosis pass
@@ -362,6 +373,36 @@ __device__ __forceinline__ HotConsts load_hot(const FilterConsts &fc) {
   return h;
 }
 
+// The coupled Filter terms of node i, ANDed into ok: PodTopologySpread hard constraints (podtopologyspread/filtering.go:311-356) and
+// InterPodAffinity required terms (interpodaffinity/filtering.go:367-432). sel picks the terms: bit c spread constraint c, bit 8 + a
+// affinity key a, bit 16 + a anti-affinity key a; ALL: every term, sel unused (filter_node). The affinity test splits exactly over the
+// terms: with the bypass every selected key must be present, without it every selected key must also count a pod.
+#define COUPLED_AFF_SEL(a) (1u << (8 + (a)))
+#define COUPLED_ANTI_SEL(a) (1u << (16 + (a)))
+template <bool ALL>
+__device__ __forceinline__ void coupled_ok(const FilterConsts &fc, int n_pts, int n_aff, int n_anti, int32_t i, uint32_t sel, bool &ok) {
+  for (int c = 0; c < n_pts; c++) {
+    if (!ALL && !((sel >> c) & 1u)) continue;
+    const int32_t dom = fc.pts[c].col ? fc.pts[c].col[i] : i;
+    ok &= (dom >= 0) && !(fc.pts[c].cnt[dom < 0 ? 0 : dom] > fc.pts_lim[c]);
+  }
+  if (n_aff) {
+    bool pods_exist = true, missing = false;
+    for (int a = 0; a < n_aff; a++) {
+      if (!ALL && !(sel & COUPLED_AFF_SEL(a))) continue;
+      const int32_t dom = fc.aff[a].col ? fc.aff[a].col[i] : i;
+      missing |= (dom < 0);
+      pods_exist &= (dom >= 0) && (fc.aff[a].cnt[dom < 0 ? 0 : dom] > 0);
+    }
+    ok &= !(missing || (!pods_exist && !fc.aff_bypass));
+  }
+  for (int a = 0; a < n_anti; a++) {
+    if (!ALL && !(sel & COUPLED_ANTI_SEL(a))) continue;
+    const int32_t dom = fc.anti[a].col ? fc.anti[a].col[i] : i;
+    ok &= !((dom >= 0) && (fc.anti[a].cnt[dom < 0 ? 0 : dom] > 0));
+  }
+}
+
 // Hot path: the fused Filter pass for node i (shard-local index). One predicate-eval.
 // Plugin order does not matter for feasibility (the AND of all enabled plugins); the order only matters for the
 // FitError reasons, which the terminal diagnosis kernel reproduces.
@@ -387,25 +428,7 @@ __device__ __forceinline__ bool filter_node(const DevParams &p, const HotConsts 
     const unsigned long long sw = tl.static0[i];
     ok &= ((~sw & hc.sel0) | (sw & hc.forbid0)) == 0ull;
   }
-  // PodTopologySpread hard constraints (podtopologyspread/filtering.go:311-356)
-  for (int c = 0; c < hc.n_pts; c++) {
-    const int32_t dom = fc.pts[c].col ? fc.pts[c].col[i] : i;
-    ok &= (dom >= 0) && !(fc.pts[c].cnt[dom < 0 ? 0 : dom] > fc.pts_lim[c]);
-  }
-  // InterPodAffinity required terms (interpodaffinity/filtering.go:367-432)
-  if (hc.n_aff) {
-    bool pods_exist = true, missing = false;
-    for (int a = 0; a < hc.n_aff; a++) {
-      const int32_t dom = fc.aff[a].col ? fc.aff[a].col[i] : i;
-      missing |= (dom < 0);
-      pods_exist &= (dom >= 0) && (fc.aff[a].cnt[dom < 0 ? 0 : dom] > 0);
-    }
-    ok &= !(missing || (!pods_exist && !fc.aff_bypass));
-  }
-  for (int a = 0; a < hc.n_anti; a++) {
-    const int32_t dom = fc.anti[a].col ? fc.anti[a].col[i] : i;
-    ok &= !((dom >= 0) && (fc.anti[a].cnt[dom < 0 ? 0 : dom] > 0));
-  }
+  coupled_ok<true>(fc, hc.n_pts, hc.n_aff, hc.n_anti, i, 0u, ok);
   if (hc.extras && ok) ok = filter_extras(p.self, fc.tmpl_index, hc.extras, i);
   if ((hc.extras & CCSIM_X_TAINT_WORDS) && ok) raw += prefer_count_hi(p.self, fc.tmpl_index, i);
   return ok;

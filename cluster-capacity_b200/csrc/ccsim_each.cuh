@@ -1,15 +1,22 @@
 // ccsim_each.cuh — per-analysis runs (ccsim_run_each): every template of the handle is analysed on its own against the loaded
 // snapshot, one CTA per analysis, all analyses in one launch (DESIGN.md §4.1g).
 //
-// Only node-local templates run here (no per-domain counters, no normalised soft scorer, no hostPorts): placing a clone on node i
-// then changes node i's feasibility and score only, and node i's state after k clones is its snapshot row plus k times the
-// template's request. An analysis therefore keeps a clone count k[i] per node and a 32-ary max-tree over per-node keys (pack_key
-// body, 0 = infeasible): a placement reads the root, commits the winner, re-evaluates that one node and re-reduces O(log N) entries.
+// For a node-local template (no per-domain counters, no normalised soft scorer, no hostPorts) placing a clone on node i changes node
+// i's feasibility and score only, and node i's state after k clones is its snapshot row plus k times the template's request. An
+// analysis therefore keeps a clone count k[i] per node and a 32-ary max-tree over per-node keys (pack_key body, 0 = infeasible): a
+// placement reads the root, commits the winner, re-evaluates that one node and re-reduces O(log N) entries.
 //
-// One tree per normalisation class (untolerated PreferNoSchedule taints, static per template and node): the class trees cover a
+// One tree segment per normalisation class (untolerated PreferNoSchedule taints, static per template and node): the segments cover a
 // stable partition of the nodes by class, and their roots go through select_host_over_classes like the class winners of the wave
 // kernels. Level 0 (the leaves) and the upper levels that do not fit in shared memory live in global memory; the host chooses the
 // split (EachParams::split).
+//
+// Templates with coupled terms (ccsim_set_analyses: hard spread, required pod (anti-)affinity, hostPorts) keep their counters per
+// analysis (EachTerms). A term whose domains hold one node each (node-local counters, hostname columns) and the hostPort self-conflict
+// (k > 0) depend on the node's own clones only: they fold into the leaf. The other terms split the nodes into domain groups (class,
+// domain in each of their columns), partitioned on the host; each group is a segment, and a placement takes a group's root only when
+// the group's domains pass those terms (coupled_ok on one of its nodes, the code filter_node runs). When a leaf-folded term changes
+// on every node at once (a folded spread minimum moves, the affinity bypass ends) the leaves and levels are rebuilt.
 #pragma once
 
 #define EACH_THREADS 512
@@ -19,6 +26,20 @@ struct EachOut {
   long long placed;
   int32_t stop_code;
   int32_t error;        // 1: the sequence buffer would overflow (cannot happen: the host sizes it from the run's bound)
+  long long rebuilds;   // leaf and level rebuilds after a folded term changed on every node
+};
+
+struct EachTerms {      // one analysis's coupled terms (ccsim_set_analyses), device memory
+  DevCounter counters[CCSIM_MAX_COUNTERS];   // work: the analysis's working counts (initialised from init at kernel start)
+  const int32_t *topo[CCSIM_MAX_TOPO_COLS];  // the analysis's topology columns
+  int32_t n_counters;
+  int32_t n_seg;        // domain groups = tree segments
+  uint32_t leaf_sel;    // coupled_ok selection of the terms folded into the leaf
+  uint32_t group_sel;   // the terms tested per group
+  const long long *cof; // [(L + 1) * (n_seg + 1)]: group s's entries of level l are [cof[l * (n_seg + 1) + s], cof[... + s + 1])
+  const int32_t *seg_rep;   // [n_seg] a node of group s (its domains in the group columns are the group's)
+  const int32_t *seg_cls;   // [n_seg] the group's normalisation class
+  int32_t *pos;             // [n] leaf position of each node
 };
 
 struct EachParams {
@@ -34,6 +55,8 @@ struct EachParams {
   unsigned long long *glev;     // [T][glev_stride]
   int32_t *seq;                 // [T][seq_cap] node of clone k
   EachOut *out;                 // [T]
+  const EachTerms *terms;       // [T] (ccsim_set_analyses), nullptr: node-local templates, partitioned by class here
+  DevOut *diag;                 // [T] the diagnosis's outputs: final spread minima and affinity total
   // the snapshot rows a node's state is computed from
   const int64_t *s_req_cpu, *s_req_mem, *s_req_eph, *s_nz_cpu, *s_nz_mem;
   const int32_t *s_npods;
@@ -48,8 +71,50 @@ struct __align__(16) EachShared {
   int32_t wcnt[EACH_THREADS / 32][CCSIM_MAX_CLASSES];   // partition: nodes of each class per warp in the current chunk
   int32_t crun[CCSIM_MAX_CLASSES];                       // partition: next position of each class
   long long coff[EACH_MAX_LEVELS + 1][CCSIM_MAX_CLASSES + 1];   // class c's entries of level l: [coff[l][c], coff[l][c+1])
+  const long long *cof;   // segment offsets: es.coff (classes) or the analysis's group table
+  int32_t cstride, nseg;  // entries per level of cof, segments
+  int32_t grouped;        // segments are domain groups: a placement tests each group's terms and takes the maximum per class
+  int32_t coupled;        // the analysis has counters or hostPorts
+  int32_t port_self;      // a clone's hostPorts conflict with the next clone's
+  uint32_t leaf_sel, group_sel;
+  const int32_t *topo_ptr[CCSIM_MAX_TOPO_COLS];
+  int32_t *cnt_ptr[CCSIM_MAX_COUNTERS];
+  CommitInfo cinfo[CCSIM_MAX_COUNTERS];
+  int32_t ptsmin[CCSIM_MAX_PTS], ptsnum[CCSIM_MAX_PTS];
+  unsigned long long aff_total;
 };
 __shared__ EachShared es;
+// G: the analyses have ccsim_set_analyses terms (segments from the host's table); else class segments in es.coff, read directly
+// (the node-local path's per-placement loads stay plain shared-memory loads)
+template <bool G> __device__ __forceinline__ long long cof(int l, int s) {
+  return G ? es.cof[(long long)l * es.cstride + s] : es.coff[l][s];
+}
+
+// the segment holding entry e of level l: the last s with cof(l, s) <= e
+template <bool G> __device__ __forceinline__ int each_seg_of(int l, long long e) {
+  if (!G) { int c = 0; while (e >= es.coff[l][c + 1]) c++; return c; }
+  int lo = 0, hi = es.nseg;   // cof(l, lo) <= e < cof(l, hi)
+  while (hi - lo > 1) { const int mid = (lo + hi) >> 1; if (cof<G>(l, mid) <= e) lo = mid; else hi = mid; }
+  return lo;
+}
+
+// spread constraint c's global minimum (filtering.go:56-69) and how many domains hold it, recounted by one warp
+__device__ void each_pts_recount(int c, int lane) {
+  const ccsim_pts &pc = es.tmpl.pts[c];
+  const int32_t *cnt = es.cnt_ptr[pc.counter];
+  const int32_t np = es.cinfo[pc.counter].n_present;
+  int32_t m = INT32_MAX, s = 0;
+  for (int d = lane; d < np; d += 32) m = min(m, cnt[d]);
+  m = __reduce_min_sync(0xffffffffu, m);
+  for (int d = lane; d < np; d += 32) s += (cnt[d] == m);
+  s = __reduce_add_sync(0xffffffffu, s);
+  if (lane == 0) {
+    es.ptsmin[c] = pc.min_zero ? 0 : m;
+    es.ptsnum[c] = s;
+    es.fc.pts_lim[c] = pts_limit(pc, es.ptsmin[c]);
+  }
+  __syncwarp();
+}
 
 // x + k * r with the wrap of k repeated int64 additions (the wave kernels' commit)
 __device__ __forceinline__ long long each_add(int64_t x, uint32_t k, int64_t r) {
@@ -63,6 +128,7 @@ __device__ __forceinline__ int each_class(const DevParams &p, int32_t ti, int32_
 
 // leaf key of node i after kk clones of the analysis's template: filter_node's Filter and the wave kernel's score on the computed
 // state (snapshot row + kk * request); 0 when infeasible
+template <bool G>
 __device__ unsigned long long each_leaf(const DevParams &p, const EachParams &ep, int32_t ti, int32_t i, uint32_t kk) {
   const ccsim_template &t = es.tmpl;
   const FilterConsts &fc = es.fc;
@@ -82,6 +148,10 @@ __device__ unsigned long long each_leaf(const DevParams &p, const EachParams &ep
       if (t.req_scalar[q] != 0) ok &= !(t.req_scalar[q] > p.alloc_scalar[q][i] - each_add(ep.s_req_scalar[q][i], kk, t.req_scalar[q]));
   const uint32_t ext = fc.extras & ~(CCSIM_X_EPH | CCSIM_X_SCALARS);
   if (ok && ext) ok = filter_extras(p.self, ti, ext, i);
+  if (G && es.coupled) {   // the terms of the node's own domain: its clones' hostPorts, node-local counters and one-node domains
+    ok &= !(es.port_self && kk > 0u);
+    if (ok && es.leaf_sel) coupled_ok<false>(fc, fc.n_pts, fc.n_aff, fc.n_anti, i, es.leaf_sel, ok);
+  }
   if (!ok) return 0ull;
   int32_t sc = score_node(p.alloc_cpu[i], p.alloc_mem[i], each_add(ep.s_nz_cpu[i], kk, t.nz_cpu) + t.least_cpu,
                           each_add(ep.s_nz_mem[i], kk, t.nz_mem) + t.least_mem, rc + t.bal_cpu, rm + t.bal_mem, es.sw);
@@ -95,157 +165,265 @@ __device__ __forceinline__ unsigned long long *each_level(const EachParams &ep, 
   return l == 0 ? leaf : (l < ep.split ? glev : slev) + ep.lev_off[l];
 }
 
+// every leaf at its node's position, evaluated after its current clones (at kernel start: none), by threads t0, t0 + nt, ...
+__device__ void each_leaves(const DevParams &p, const EachParams &ep, int32_t ti, int32_t *kcol, unsigned long long *leaf,
+                            const int32_t *pos, bool start, int t0, int nt) {
+  for (int32_t i = t0; i < p.n; i += nt) {
+    if (start) kcol[i] = 0;
+    leaf[pos[i]] = each_leaf<true>(p, ep, ti, i, start ? 0u : (uint32_t)kcol[i]);
+  }
+}
+
+// upper levels, bottom up: one warp per entry, its 32 children in one coalesced load. BLOCK: the whole CTA (kernel start), else warp 0
+template <bool G, bool BLOCK>
+__device__ void each_levels(const EachParams &ep, unsigned long long *leaf, unsigned long long *glev, unsigned long long *slev,
+                            int nseg, int w0, int nw, int lane) {
+  for (int l = 1; l <= ep.n_levels; l++) {
+    const unsigned long long *lo = each_level(ep, leaf, glev, slev, l - 1);
+    unsigned long long *up = each_level(ep, leaf, glev, slev, l);
+    const long long ne = cof<G>(l, nseg);
+    for (long long g = w0; g < ne; g += nw) {
+      const int c = each_seg_of<G>(l, g);
+      const long long child = cof<G>(l - 1, c) + 32 * (g - cof<G>(l, c)) + lane;
+      const unsigned long long v = warp_max_u64(child < cof<G>(l - 1, c + 1) ? lo[child] : 0ull);
+      if (lane == 0) up[g] = v;
+    }
+    if (BLOCK) __syncthreads(); else __syncwarp();
+  }
+}
+
+// G: the analyses of ccsim_set_analyses (coupled terms, host-made groups); else node-local templates, partitioned by class here. Two
+// instantiations, so that the node-local one is compiled and register-allocated on its own
+template <bool G>
 __global__ void __launch_bounds__(EACH_THREADS, 1) ccsim_each_kernel(const DevParams p, const EachParams ep) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   unsigned long long *slev = reinterpret_cast<unsigned long long *>(smem_raw);
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nw = blockDim.x >> 5;
   const int32_t ti = blockIdx.x, n = p.n;
   const int ncls = p.n_classes, L = ep.n_levels;
+  const EachTerms *et = G ? ep.terms + ti : nullptr;
   int32_t *kcol = ep.k + (size_t)ti * n;
   unsigned long long *leaf = ep.leaf + (size_t)ti * n;
-  int32_t *pos = ep.pos ? ep.pos + (size_t)ti * n : nullptr;
+  int32_t *pos = et ? et->pos : (ep.pos ? ep.pos + (size_t)ti * n : nullptr);
   unsigned long long *glev = ep.glev + (size_t)ti * ep.glev_stride;
   int32_t *seq = ep.seq + (size_t)ti * ep.seq_cap;
 
-  // ---- template, folded Filter constants, score configuration ----
+  // ---- template, the analysis's working counters, folded Filter constants, score configuration ----
   for (int q = tid; q < (int)(sizeof(ccsim_template) / 8); q += blockDim.x)
     reinterpret_cast<unsigned long long *>(&es.tmpl)[q] = reinterpret_cast<const unsigned long long *>(&p.templates[ti])[q];
   if (tid < CCSIM_MAX_CLASSES) es.crun[tid] = 0;
+  const int ncnt = et ? et->n_counters : 0;
+  for (int j = 0; j < ncnt; j++) {
+    const DevCounter &dc = et->counters[j];
+    for (int d = tid; d < dc.n_domains; d += blockDim.x) dc.work[d] = dc.init[d];
+  }
   __syncthreads();
   if (tid == 0) {
     const ccsim_template &t = es.tmpl;
-    const int32_t *no_topo[CCSIM_MAX_TOPO_COLS] = {};
-    int32_t *no_cnt[CCSIM_MAX_COUNTERS] = {};
-    const int32_t no_min[CCSIM_MAX_PTS] = {};
-    build_filter_consts(p, t, ti, no_topo, no_cnt, no_min, t.aff_total_init, es.fc);
+    es.aff_total = (unsigned long long)t.aff_total_init;
+    es.leaf_sel = et ? et->leaf_sel : 0u; es.group_sel = et ? et->group_sel : 0u;
+    es.grouped = et && et->group_sel ? 1 : 0;
+    es.port_self = et && (t.filter_enable & CCSIM_PL_NODE_PORTS) && (t.flags & CCSIM_TF_HAS_HOST_PORTS) && ((t.port_tmpl_conflict >> ti) & 1ull);
+    es.coupled = ncnt > 0 || es.port_self;
+    if (et) { es.cof = et->cof; es.cstride = et->n_seg + 1; es.nseg = et->n_seg; }
+    else { es.cof = &es.coff[0][0]; es.cstride = CCSIM_MAX_CLASSES + 1; es.nseg = ncls; }
+    for (int k = 0; k < CCSIM_MAX_TOPO_COLS; k++) es.topo_ptr[k] = et ? et->topo[k] : nullptr;
+    for (int j = 0; j < CCSIM_MAX_COUNTERS; j++) es.cnt_ptr[j] = j < ncnt ? et->counters[j].work : nullptr;
+    for (int j = 0; j < ncnt; j++) {   // what a commit does to each counter (the generic wave kernel's CommitInfo)
+      const DevCounter &dc = et->counters[j];
+      CommitInfo &ci = es.cinfo[j];
+      const bool skip = (dc.inc == 0) || (dc.is_aff && !(t.flags & CCSIM_TF_AFF_SELF_MATCH_ALL));
+      ci.inc = skip ? 0 : dc.inc;
+      ci.local = dc.topo_col < 0; ci.is_aff = dc.is_aff; ci.n_present = dc.n_present; ci.elig_bit = dc.elig_bit;
+      ci.gtopo = ci.ltopo = dc.topo_col < 0 ? nullptr : et->topo[dc.topo_col];
+      ci.pts_idx = -1;
+      for (int c = 0; c < t.n_pts; c++) if (t.pts[c].counter == j && !t.pts[c].min_zero) ci.pts_idx = c;
+    }
+    for (int c = 0; c < CCSIM_MAX_PTS; c++) { es.ptsmin[c] = 0; es.ptsnum[c] = 0; }
+  }
+  __syncthreads();
+  if (tid == 0) {
+    const ccsim_template &t = es.tmpl;
+    build_filter_consts(p, et ? et->counters : p.counters, t, ti, es.topo_ptr, es.cnt_ptr, es.ptsmin, (long long)es.aff_total, es.fc);
+    es.fc.extras &= ~CCSIM_X_PLACED;   // hostPorts against the analysis's own clones: k > 0 in the leaf
     es.sw.w_fit = (t.score_enable & CCSIM_PL_FIT) ? t.w_fit : 0;
     es.sw.w_balanced = ((t.score_enable & CCSIM_PL_BALANCED) && !(t.flags & CCSIM_TF_BALANCED_SKIP)) ? t.w_balanced : 0;
     es.sw.least_w_cpu = t.least_w_cpu; es.sw.least_w_mem = t.least_w_mem;
     es.w_image = ((t.score_enable & CCSIM_PL_IMAGE_LOCALITY) && t.image_score) ? t.w_image : 0;
   }
   __syncthreads();
-
-  // ---- class sizes (several classes only): class c's leaves are positions [coff[0][c], coff[0][c+1]) ----
-  if (ncls > 1) {
-    int cnt[CCSIM_MAX_CLASSES] = {};
-    for (int32_t i = tid; i < n; i += blockDim.x) {
-      const int c = each_class(p, ti, i);
-      #pragma unroll
-      for (int q = 0; q < CCSIM_MAX_CLASSES; q++) cnt[q] += (q == c);
-    }
-    #pragma unroll
-    for (int q = 0; q < CCSIM_MAX_CLASSES; q++) {
-      const int v = __reduce_add_sync(0xffffffffu, cnt[q]);
-      if (lane == 0 && v) atomicAdd(&es.crun[q], v);
-    }
-  } else if (tid == 0) es.crun[0] = n;
-  __syncthreads();
-  if (tid == 0) {   // entries per class and level: ceil(size / 32^l); crun becomes the partition's running position
-    long long run = 0;
-    for (int c = 0; c < ncls; c++) { const long long sz = es.crun[c]; es.crun[c] = (int32_t)run; es.coff[0][c] = run; run += sz; }
-    es.coff[0][ncls] = run;
-    for (int l = 1; l <= L; l++) {
-      long long acc = 0;
-      for (int c = 0; c < ncls; c++) {
-        const long long sz = es.coff[l - 1][c + 1] - es.coff[l - 1][c];
-        es.coff[l][c] = acc; acc += (sz + 31) >> 5;
-      }
-      es.coff[l][ncls] = acc;
-    }
-  }
+  if (warp == 0) for (int c = 0; c < es.fc.n_pts; c++) each_pts_recount(c, lane);   // the spread minima and their limits
   __syncthreads();
 
-  // ---- leaves: stable partition by class (node order inside a class), every node evaluated with no clone placed ----
-  for (int32_t base = 0; base < n; base += blockDim.x) {
-    const int32_t i = base + tid;
-    int32_t at = i;
+  if (G) {
+    // ---- leaves at the host's positions (partition by domain group) ----
+    each_leaves(p, ep, ti, kcol, leaf, pos, true, tid, blockDim.x);
+  } else {
+    // ---- class sizes (several classes only): class c's leaves are positions [coff[0][c], coff[0][c+1]) ----
     if (ncls > 1) {
-      const int c = i < n ? each_class(p, ti, i) : -1;
-      int rank = 0;
-      for (int q = 0; q < ncls; q++) {
-        const unsigned b = __ballot_sync(0xffffffffu, c == q);
-        if (c == q) rank = __popc(b & ((1u << lane) - 1u));
-        if (lane == 0) es.wcnt[warp][q] = __popc(b);
+      int cnt[CCSIM_MAX_CLASSES] = {};
+      for (int32_t i = tid; i < n; i += blockDim.x) {
+        const int c = each_class(p, ti, i);
+        #pragma unroll
+        for (int q = 0; q < CCSIM_MAX_CLASSES; q++) cnt[q] += (q == c);
       }
-      __syncthreads();
-      if (c >= 0) {
-        at = es.crun[c] + rank;
-        for (int w = 0; w < warp; w++) at += es.wcnt[w][c];
+      #pragma unroll
+      for (int q = 0; q < CCSIM_MAX_CLASSES; q++) {
+        const int v = __reduce_add_sync(0xffffffffu, cnt[q]);
+        if (lane == 0 && v) atomicAdd(&es.crun[q], v);
       }
-      __syncthreads();
-      if (tid < ncls) { int s = 0; for (int w = 0; w < nw; w++) s += es.wcnt[w][tid]; es.crun[tid] += s; }
-      __syncthreads();
-    }
-    if (i < n) {
-      kcol[i] = 0;
-      if (pos) pos[i] = at;
-      leaf[at] = each_leaf(p, ep, ti, i, 0u);
-    }
-  }
-  __syncthreads();
-
-  // ---- upper levels, bottom up: one warp per entry, its 32 children in one coalesced load ----
-  for (int l = 1; l <= L; l++) {
-    const unsigned long long *lo = each_level(ep, leaf, glev, slev, l - 1);
-    unsigned long long *up = each_level(ep, leaf, glev, slev, l);
-    for (long long g = warp; g < es.coff[l][ncls]; g += nw) {
-      int c = 0;
-      while (g >= es.coff[l][c + 1]) c++;
-      const long long child = es.coff[l - 1][c] + 32 * (g - es.coff[l][c]) + lane;
-      const unsigned long long v = warp_max_u64(child < es.coff[l - 1][c + 1] ? lo[child] : 0ull);
-      if (lane == 0) up[g] = v;
+    } else if (tid == 0) es.crun[0] = n;
+    __syncthreads();
+    if (tid == 0) {   // entries per class and level: ceil(size / 32^l); crun becomes the partition's running position
+      long long run = 0;
+      for (int c = 0; c < ncls; c++) { const long long sz = es.crun[c]; es.crun[c] = (int32_t)run; es.coff[0][c] = run; run += sz; }
+      es.coff[0][ncls] = run;
+      for (int l = 1; l <= L; l++) {
+        long long acc = 0;
+        for (int c = 0; c < ncls; c++) {
+          const long long sz = es.coff[l - 1][c + 1] - es.coff[l - 1][c];
+          es.coff[l][c] = acc; acc += (sz + 31) >> 5;
+        }
+        es.coff[l][ncls] = acc;
+      }
     }
     __syncthreads();
+
+    // ---- leaves: stable partition by class (node order inside a class), every node evaluated with no clone placed ----
+    for (int32_t base = 0; base < n; base += blockDim.x) {
+      const int32_t i = base + tid;
+      int32_t at = i;
+      if (ncls > 1) {
+        const int c = i < n ? each_class(p, ti, i) : -1;
+        int rank = 0;
+        for (int q = 0; q < ncls; q++) {
+          const unsigned b = __ballot_sync(0xffffffffu, c == q);
+          if (c == q) rank = __popc(b & ((1u << lane) - 1u));
+          if (lane == 0) es.wcnt[warp][q] = __popc(b);
+        }
+        __syncthreads();
+        if (c >= 0) {
+          at = es.crun[c] + rank;
+          for (int w = 0; w < warp; w++) at += es.wcnt[w][c];
+        }
+        __syncthreads();
+        if (tid < ncls) { int s = 0; for (int w = 0; w < nw; w++) s += es.wcnt[w][tid]; es.crun[tid] += s; }
+        __syncthreads();
+      }
+      if (i < n) {
+        kcol[i] = 0;
+        if (pos) pos[i] = at;
+        leaf[at] = each_leaf<false>(p, ep, ti, i, 0u);
+      }
+    }
   }
+  __syncthreads();
+  each_levels<G, true>(ep, leaf, glev, slev, G ? es.nseg : ncls, warp, nw, lane);
 
   // ---- placements: warp 0 alone ----
   if (warp != 0) return;
   const ccsim_template &t = es.tmpl;
   unsigned long long *top = each_level(ep, leaf, glev, slev, L);
   unsigned long long *lv1 = L >= 2 ? each_level(ep, leaf, glev, slev, 1) : nullptr;
-  long long k = 0;
+  long long k = 0, rebuilds = 0;
   bool limit_hit = false;
   int error = 0;
   for (;; k++) {
     if (ep.max_pods > 0 && k >= ep.max_pods) { limit_hit = true; break; }   // postBindHook limit (simulator.go:300-305)
     if (k >= ep.seq_cap) { error = 1; break; }
     // prioritizeNodes + selectHost over the class roots (schedule_one.go:776-941)
-    const unsigned long long r = (lane < ncls && es.coff[L][lane + 1] > es.coff[L][lane]) ? top[es.coff[L][lane]] : 0ull;
     unsigned long long cbest[CCSIM_MAX_CLASSES];
-    #pragma unroll
-    for (int c = 0; c < CCSIM_MAX_CLASSES; c++) cbest[c] = __shfl_sync(0xffffffffu, r, c);
+    if (!G || !es.grouped) {   // one segment per class
+      const unsigned long long r = (lane < ncls && cof<G>(L, lane + 1) > cof<G>(L, lane)) ? top[cof<G>(L, lane)] : 0ull;
+      #pragma unroll
+      for (int c = 0; c < CCSIM_MAX_CLASSES; c++) cbest[c] = __shfl_sync(0xffffffffu, r, c);
+    } else {             // a group's root counts when its domains pass the group terms; the best open group per class
+      unsigned long long mine[CCSIM_MAX_CLASSES];
+      #pragma unroll
+      for (int c = 0; c < CCSIM_MAX_CLASSES; c++) mine[c] = 0ull;
+      for (int s = lane; s < es.nseg; s += 32) {
+        const long long e = cof<G>(L, s);
+        if (cof<G>(L, s + 1) == e) continue;
+        bool ok = true;
+        coupled_ok<false>(es.fc, es.fc.n_pts, es.fc.n_aff, es.fc.n_anti, et->seg_rep[s], es.group_sel, ok);
+        if (!ok) continue;
+        const unsigned long long v = top[e];
+        const int cl = et->seg_cls[s];
+        #pragma unroll
+        for (int c = 0; c < CCSIM_MAX_CLASSES; c++) if (c == cl && v > mine[c]) mine[c] = v;
+      }
+      #pragma unroll
+      for (int c = 0; c < CCSIM_MAX_CLASSES; c++) cbest[c] = c < ncls ? warp_max_u64(mine[c]) : 0ull;
+    }
     const unsigned long long wkey = select_host_over_classes(cbest, ncls, t);
     if (wkey == 0ull) break;                                                // Unschedulable
     const int32_t i = (int32_t)key_index(wkey);
     const long long at = pos ? pos[i] : i;
-    int c = 0;
-    while (at >= es.coff[0][c + 1]) c++;
-    // the winner's group of 32 on level 0 and on level 1, loaded while lane 0 re-evaluates the winner
-    const long long e0 = at - es.coff[0][c], e1 = e0 >> 5;
-    const long long g0 = es.coff[0][c] + (e0 & ~31ll) + lane;
-    unsigned long long v0 = g0 < es.coff[0][c + 1] ? leaf[g0] : 0ull, v1 = 0ull;
-    if (lv1) { const long long g1 = es.coff[1][c] + (e1 & ~31ll) + lane; v1 = g1 < es.coff[1][c + 1] ? lv1[g1] : 0ull; }
-    unsigned long long nv = 0ull;
+    const int c = each_seg_of<G>(0, at);
+    // the winner's group of 32 on level 0 and on level 1, loaded while lane 0 commits the winner
+    const long long e0 = at - cof<G>(0, c), e1 = e0 >> 5;
+    const long long g0 = cof<G>(0, c) + (e0 & ~31ll) + lane;
+    unsigned long long v0 = g0 < cof<G>(0, c + 1) ? leaf[g0] : 0ull, v1 = 0ull;
+    if (lv1) { const long long g1 = cof<G>(1, c) + (e1 & ~31ll) + lane; v1 = g1 < cof<G>(1, c + 1) ? lv1[g1] : 0ull; }
+    uint32_t kk = 0u;
     if (lane == 0) {
-      const uint32_t kk = (uint32_t)kcol[i] + 1u;                          // ClusterCapacityBinder commit: one more clone on i
+      kk = (uint32_t)kcol[i] + 1u;                                          // ClusterCapacityBinder commit: one more clone on i
       kcol[i] = (int32_t)kk;
       seq[k] = i;
-      nv = each_leaf(p, ep, ti, i, kk);
     }
+    bool rebuild = false;
+    if (G && es.coupled) {
+      // the counters of the winner's domains, one lane per counter (the generic wave kernel's commit)
+      if (lane < ncnt) {
+        const CommitInfo &ci = es.cinfo[lane];
+        if (ci.inc && !(ci.elig_bit >= 0 && !static_bit(p, i, ci.elig_bit))) {
+          const int32_t dom = ci.local ? i : ci.ltopo[i];
+          if (dom >= 0) {
+            int32_t *cnt = es.cnt_ptr[lane];
+            const int32_t old = cnt[dom];
+            cnt[dom] = old + ci.inc;
+            if (ci.is_aff) atomicAdd(&es.aff_total, (unsigned long long)(long long)ci.inc);
+            if (ci.pts_idx >= 0 && dom < ci.n_present && old == es.ptsmin[ci.pts_idx]) atomicSub(&es.ptsnum[ci.pts_idx], 1);
+          }
+        }
+      }
+      __syncwarp();
+      // a spread minimum whose last domain moved up: recount; a folded constraint's limit then changed on every node
+      for (int q = 0; q < es.fc.n_pts; q++)
+        if (!t.pts[q].min_zero && es.ptsnum[q] <= 0 && es.cinfo[t.pts[q].counter].n_present > 0) {
+          each_pts_recount(q, lane);
+          rebuild |= (es.leaf_sel >> q) & 1u;
+        }
+      if (es.fc.aff_bypass && es.aff_total != 0ull) {   // the first matching pod ends the bypass (filtering.go:396-405)
+        __syncwarp();
+        if (lane == 0) es.fc.aff_bypass = 0;
+        rebuild = true;
+      }
+      __syncwarp();
+    }
+    if (G && rebuild) {   // every leaf and level again, with the code of the kernel start
+      each_leaves(p, ep, ti, kcol, leaf, pos, false, lane, 32);
+      __syncwarp();
+      each_levels<G, false>(ep, leaf, glev, slev, es.nseg, 0, 1, lane);
+      rebuilds++;
+      continue;
+    }
+    unsigned long long nv = 0ull;
+    if (lane == 0) nv = each_leaf<G>(p, ep, ti, i, kk);
     nv = __shfl_sync(0xffffffffu, nv, 0);
-    // level l's entry e (within class c's segment) gets nv; its group's maximum becomes level l + 1's entry e >> 5
+    // level l's entry e (within segment c) gets nv; its group's maximum becomes level l + 1's entry e >> 5
     long long e = e0;
     for (int l = 0; l < L; l++) {
-      unsigned long long *lv = each_level(ep, leaf, glev, slev, l) + es.coff[l][c];
+      unsigned long long *lv = each_level(ep, leaf, glev, slev, l) + cof<G>(l, c);
       unsigned long long v;
       if (l == 0) v = v0;
       else if (l == 1) v = v1;
-      else { const long long g = (e & ~31ll) + lane; v = g < es.coff[l][c + 1] - es.coff[l][c] ? lv[g] : 0ull; }
+      else { const long long g = (e & ~31ll) + lane; v = g < cof<G>(l, c + 1) - cof<G>(l, c) ? lv[g] : 0ull; }
       if (lane == (int)(e & 31)) { v = nv; lv[e] = nv; }
       nv = warp_max_u64(v);
       e >>= 5;
     }
-    if (lane == 0) top[es.coff[L][c]] = nv;
+    if (lane == 0) top[cof<G>(L, c)] = nv;
     __syncwarp();
   }
   if (lane == 0) {
@@ -253,11 +431,18 @@ __global__ void __launch_bounds__(EACH_THREADS, 1) ccsim_each_kernel(const DevPa
     o.placed = k;
     o.stop_code = limit_hit ? CCSIM_STOP_LIMIT_REACHED : CCSIM_STOP_UNSCHEDULABLE;
     o.error = error;
+    o.rebuilds = rebuilds;
     ep.out[ti] = o;
+    if (G) {   // what the diagnosis reads besides the counters
+      for (int q = 0; q < CCSIM_MAX_PTS; q++) ep.diag[ti].ptsmin[q] = es.ptsmin[q];
+      ep.diag[ti].aff_total = (long long)es.aff_total;
+    }
   }
 }
 
-// Analysis t's final node state into the working columns, for the terminal diagnosis (ccsim_diag_kernel)
+
+// Analysis t's final node state into the working columns, for the terminal diagnosis (ccsim_diag_kernel); its counters are read
+// where the run left them (EachTerms::counters[].work)
 __global__ void ccsim_each_scatter_kernel(const DevParams p, const EachParams ep, int32_t ti) {
   const ccsim_template &t = p.templates[ti];
   const int32_t *kcol = ep.k + (size_t)ti * p.n;
@@ -270,5 +455,6 @@ __global__ void ccsim_each_scatter_kernel(const DevParams p, const EachParams ep
     p.nz_mem[i] = each_add(ep.s_nz_mem[i], kk, t.nz_mem);
     p.npods[i] = (int32_t)((uint32_t)ep.s_npods[i] + kk);
     for (int q = 0; q < p.n_scalars; q++) p.req_scalar[q][i] = each_add(ep.s_req_scalar[q][i], kk, t.req_scalar[q]);
+    if (p.placed_mask) p.placed_mask[i] = kk > 0u ? 1ull << ti : 0ull;   // hostPorts: the analysis's own clones
   }
 }

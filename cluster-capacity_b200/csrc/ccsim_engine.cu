@@ -193,10 +193,12 @@ static const WaveKernel WAVE_KERNELS[] = {
   {(const void *)ccsim_wave_stream_kernel<0>, "stream<0>", ENG_STREAM, STREAM_BLOCK, sizeof(StreamShared), stream_smem_bytes(0, 0)},
   {(const void *)ccsim_wave_stream_kernel<1>, "stream<1>", ENG_STREAM, STREAM_BLOCK, sizeof(StreamShared), stream_smem_bytes(1, 0)},
   {(const void *)ccsim_wave_stream_kernel<2>, "stream<2>", ENG_STREAM, STREAM_BLOCK, sizeof(StreamShared), 0},
-  {(const void *)ccsim_each_kernel, "each", ENG_EACH, EACH_THREADS, sizeof(EachShared), 0},     // ccsim_run_each only
+  {(const void *)ccsim_each_kernel<false>, "each", ENG_EACH, EACH_THREADS, sizeof(EachShared), 0},   // ccsim_run_each only
+  {(const void *)ccsim_each_kernel<true>, "each", ENG_EACH, EACH_THREADS, sizeof(EachShared), 0},    // ... after ccsim_set_analyses
 };
-enum { WK_WAVE, WK_WAVE_STREAMED, WK_LEAN, WK_LEAN_SAMPLING, WK_BATCHED, WK_MULTI, WK_MULTI_SHARDED, WK_STREAM /* + mode */, WK_EACH = WK_STREAM + 3 };
-static_assert(sizeof(WAVE_KERNELS) / sizeof(WAVE_KERNELS[0]) == WK_EACH + 1, "one WAVE_KERNELS entry per WK_* index");
+enum { WK_WAVE, WK_WAVE_STREAMED, WK_LEAN, WK_LEAN_SAMPLING, WK_BATCHED, WK_MULTI, WK_MULTI_SHARDED, WK_STREAM /* + mode */,
+       WK_EACH = WK_STREAM + 3, WK_EACH_TERMS };
+static_assert(sizeof(WAVE_KERNELS) / sizeof(WAVE_KERNELS[0]) == WK_EACH_TERMS + 1, "one WAVE_KERNELS entry per WK_* index");
 
 struct RunPlan {      // what run_prepare decided, consumed by the launch
   bool valid = false, empty = false;
@@ -208,6 +210,20 @@ struct RunPlan {      // what run_prepare decided, consumed by the launch
 // Template facts of the engine choice (ccsim_set_templates): a template without NodeResourcesFit's Filter (no "Too many pods" bound);
 // normalised soft scorers; the lean and streaming kernels cover every template (no soft scorer, ImageLocality or needs_extras; one taint word, <= 1 static word)
 struct TemplateFacts { bool fit_off, has_soft, lean_filter; };
+
+// the most placements after which every domain of a counter is still exact, with NodeResourcesFit bounding each domain by its free
+// pod slots (lim_fit) or not (lim_any), and the domain that sets each bound
+struct CounterRange { int64_t lim_fit, lim_any; int32_t dom_fit, dom_any, init_fit, init_any; };
+
+// ccsim_set_analyses: one analysis's terms as the host keeps them
+struct AnalysisState {
+  EachTerms terms;                            // its device copy is d_terms[t]
+  int32_t n_topo = 0;
+  int32_t final_off[CCSIM_MAX_COUNTERS] = {};  // counter j's working counts: terms.counters[j].work = work + final_off[j]
+  int32_t *work = nullptr;
+  CounterRange range[CCSIM_MAX_COUNTERS];
+  std::vector<int64_t> dom_slots[CCSIM_MAX_TOPO_COLS];
+};
 
 struct ccsim_handle {
   ccsim_config cfg;
@@ -260,7 +276,7 @@ struct ccsim_handle {
   // (ccsim_set_templates), with NodeResourcesFit bounding each domain by its slots (lim_fit) or not (lim_any)
   std::vector<int32_t> node_slots;
   std::vector<int64_t> dom_slots[CCSIM_MAX_TOPO_COLS];
-  struct CounterRange { int64_t lim_fit, lim_any; int32_t dom_fit, dom_any, init_fit, init_any; } cnt_range[CCSIM_MAX_COUNTERS];
+  CounterRange cnt_range[CCSIM_MAX_COUNTERS];
   int32_t smem_cnt_ints = 0;
   // run state
   int grid = 0;
@@ -287,6 +303,12 @@ struct ccsim_handle {
   int32_t *d_each_seq = nullptr; int64_t each_seq_cap = 0;
   std::vector<int64_t> each_placed;
   std::vector<std::vector<int32_t>> each_seq;
+  // ccsim_set_analyses: every analysis's own counters, columns and domain groups (until the next ccsim_set_templates)
+  bool analyses = false;
+  std::vector<AnalysisState> an;
+  EachTerms *d_terms = nullptr;
+  int32_t max_seg = 0;                        // most tree segments of an analysis
+  std::vector<uint64_t> h_taint;              // the loaded taint masks (word-major): the normalisation class of each node
 };
 
 static std::string g_create_err;
@@ -497,6 +519,7 @@ extern "C" int ccsim_load_nodes(ccsim_handle *h, const ccsim_nodes *nd) {
     }
   h->taint_or0 = 0;
   for (int32_t i = 0; i < N; i++) h->taint_or0 |= nd->taint_mask[i];
+  h->h_taint.assign(nd->taint_mask, nd->taint_mask + (size_t)nd->taint_words * N);
   CK(cudaStreamSynchronize(h->stream));
   h->have_nodes = true;
   return CCSIM_OK;
@@ -515,62 +538,72 @@ static bool needs_extras(const ccsim_handle *h, const ccsim_template &T) {
   return false;
 }
 
-extern "C" int ccsim_set_templates(ccsim_handle *h, int32_t n_templates, const ccsim_template *templates,
-                                   int32_t n_counters, const ccsim_counter *counters) {
-  if (!h || !templates) return fail(h, CCSIM_EINVAL, "null argument");
-  if (!h->have_nodes) return fail(h, CCSIM_ESTATE, "ccsim_load_nodes must come first");
-  if (n_templates < 1 || n_templates > CCSIM_MAX_TEMPLATES) return fail(h, CCSIM_EINVAL, "n_templates out of range");
-  if (n_counters < 0 || n_counters > CCSIM_MAX_COUNTERS || (n_counters && !counters)) return fail(h, CCSIM_EINVAL, "n_counters out of range");
-  if (n_templates > 1 && n_counters > 0)
-    return fail(h, CCSIM_EUNSUPPORTED, "PodTopologySpread/InterPodAffinity templates are single-template only");
-  CK(cudaSetDevice(h->cfg.device));
-  free_pool(h, h->tmpl_allocs);
-  h->have_templates = false; h->plan.valid = false; h->each_ran = false;
+// One template's index ranges against its counter table (CCSIM_EINVAL) and its score weights (CCSIM_EUNSUPPORTED)
+static int check_template(ccsim_handle *h, int t, const ccsim_template &T, int32_t n_counters, const ccsim_counter *counters) {
   const ccsim_nodes &nd = h->meta;
-  for (int t = 0; t < n_templates; t++) {
-    const ccsim_template &T = templates[t];
-    if (T.n_pref_terms < 0 || T.n_pref_terms > CCSIM_MAX_AFF_TERMS) return fail(h, CCSIM_EINVAL, "template %d: n_pref_terms", t);
-    if (T.n_pts < 0 || T.n_pts > CCSIM_MAX_PTS || T.n_aff < 0 || T.n_aff > CCSIM_MAX_IPA || T.n_anti < 0 || T.n_anti > CCSIM_MAX_IPA ||
-        T.n_aff_terms < 0 || T.n_aff_terms > CCSIM_MAX_AFF_TERMS)
-      return fail(h, CCSIM_EINVAL, "template %d: term counts out of range", t);
-    for (int c = 0; c < T.n_pts; c++) {
-      if (T.pts[c].counter < 0 || T.pts[c].counter >= n_counters) return fail(h, CCSIM_EINVAL, "template %d: pts counter index", t);
-      if (counters[T.pts[c].counter].topo_col < 0)
-        return fail(h, CCSIM_EUNSUPPORTED, "topology spread over a node-local (hostname) domain is not supported yet");
-    }
-    for (int a = 0; a < T.n_aff; a++) if (T.aff_counter[a] < 0 || T.aff_counter[a] >= n_counters) return fail(h, CCSIM_EINVAL, "aff counter index");
-    for (int a = 0; a < T.n_anti; a++) if (T.anti_counter[a] < 0 || T.anti_counter[a] >= n_counters) return fail(h, CCSIM_EINVAL, "anti counter index");
-    if ((T.flags & CCSIM_TF_PREFILTER_NODES) && (T.prefilter_bit < 0 || T.prefilter_bit >= 64 * nd.static_words))
-      return fail(h, CCSIM_EINVAL, "template %d: prefilter_bit", t);
-    if (T.n_spts < 0 || T.n_spts > CCSIM_MAX_PTS || T.n_ipa_score < 0 || T.n_ipa_score > CCSIM_MAX_IPA)
-      return fail(h, CCSIM_EINVAL, "template %d: soft term counts out of range", t);
-    if (T.spts_ignored_bit >= 64 * nd.static_words) return fail(h, CCSIM_EINVAL, "template %d: spts_ignored_bit", t);
-    for (int c = 0; c < T.n_spts; c++) {
-      const ccsim_spts &sc = T.spts[c];
-      if (sc.counter < 0 || sc.counter >= n_counters) return fail(h, CCSIM_EINVAL, "template %d: spts counter index", t);
-      if ((sc.hostname != 0) != (counters[sc.counter].topo_col < 0)) return fail(h, CCSIM_EINVAL, "template %d: spts %d: hostname constraints use node-local counters (and only they)", t, c);
-      if (sc.has_key_bit >= 64 * nd.static_words) return fail(h, CCSIM_EINVAL, "template %d: spts has_key_bit", t);
-    }
-    for (int a = 0; a < T.n_ipa_score; a++) if (T.ipa_score_counter[a] < 0 || T.ipa_score_counter[a] >= n_counters) return fail(h, CCSIM_EINVAL, "ipa score counter index");
+  if (T.n_pref_terms < 0 || T.n_pref_terms > CCSIM_MAX_AFF_TERMS) return fail(h, CCSIM_EINVAL, "template %d: n_pref_terms", t);
+  if (T.n_pts < 0 || T.n_pts > CCSIM_MAX_PTS || T.n_aff < 0 || T.n_aff > CCSIM_MAX_IPA || T.n_anti < 0 || T.n_anti > CCSIM_MAX_IPA ||
+      T.n_aff_terms < 0 || T.n_aff_terms > CCSIM_MAX_AFF_TERMS)
+    return fail(h, CCSIM_EINVAL, "template %d: term counts out of range", t);
+  for (int c = 0; c < T.n_pts; c++) {
+    if (T.pts[c].counter < 0 || T.pts[c].counter >= n_counters) return fail(h, CCSIM_EINVAL, "template %d: pts counter index", t);
+    if (counters[T.pts[c].counter].topo_col < 0)
+      return fail(h, CCSIM_EUNSUPPORTED, "topology spread over a node-local (hostname) domain is not supported yet");
   }
-  for (int j = 0; j < n_counters; j++) if (counters[j].elig_bit >= 64 * nd.static_words) return fail(h, CCSIM_EINVAL, "counter %d: elig_bit", j);
-  for (int t = 0; t < n_templates; t++) {
-    const ccsim_template &T = templates[t];
-    // a negative weight can make a total negative, and score + 1 <= 0 sets the key's tag bits; the reference's plugin weights
-    // are never negative (framework.go:487-497) and its resource weights are validated to [1, 100] (validation_pluginargs.go)
-    const int32_t w[7] = {T.w_taint, T.w_node_affinity, T.w_fit, T.w_pts, T.w_ipa, T.w_balanced, T.w_image};
-    const char *wname[7] = {"TaintToleration", "NodeAffinity", "NodeResourcesFit", "PodTopologySpread", "InterPodAffinity",
-                            "NodeResourcesBalancedAllocation", "ImageLocality"};
-    for (int q = 0; q < 7; q++)
-      if (w[q] < 0) return fail(h, CCSIM_EUNSUPPORTED, "template %d: %s score weight %d is negative", t, wname[q], w[q]);
-    if (T.least_w_cpu < 1 || T.least_w_cpu > 100 || T.least_w_mem < 1 || T.least_w_mem > 100)
-      return fail(h, CCSIM_EUNSUPPORTED, "template %d: NodeResourcesFit resource weights cpu %d / memory %d outside [1, 100]", t, T.least_w_cpu, T.least_w_mem);
-    long long wsum = 0;
-    for (int q = 0; q < 7; q++) wsum += w[q];
-    if (wsum * 100 >= 4095) return fail(h, CCSIM_EUNSUPPORTED, "template %d: sum of score weights %lld too large for the packed key", t, wsum);
+  for (int a = 0; a < T.n_aff; a++) if (T.aff_counter[a] < 0 || T.aff_counter[a] >= n_counters) return fail(h, CCSIM_EINVAL, "aff counter index");
+  for (int a = 0; a < T.n_anti; a++) if (T.anti_counter[a] < 0 || T.anti_counter[a] >= n_counters) return fail(h, CCSIM_EINVAL, "anti counter index");
+  if ((T.flags & CCSIM_TF_PREFILTER_NODES) && (T.prefilter_bit < 0 || T.prefilter_bit >= 64 * nd.static_words))
+    return fail(h, CCSIM_EINVAL, "template %d: prefilter_bit", t);
+  if (T.n_spts < 0 || T.n_spts > CCSIM_MAX_PTS || T.n_ipa_score < 0 || T.n_ipa_score > CCSIM_MAX_IPA)
+    return fail(h, CCSIM_EINVAL, "template %d: soft term counts out of range", t);
+  if (T.spts_ignored_bit >= 64 * nd.static_words) return fail(h, CCSIM_EINVAL, "template %d: spts_ignored_bit", t);
+  for (int c = 0; c < T.n_spts; c++) {
+    const ccsim_spts &sc = T.spts[c];
+    if (sc.counter < 0 || sc.counter >= n_counters) return fail(h, CCSIM_EINVAL, "template %d: spts counter index", t);
+    if ((sc.hostname != 0) != (counters[sc.counter].topo_col < 0)) return fail(h, CCSIM_EINVAL, "template %d: spts %d: hostname constraints use node-local counters (and only they)", t, c);
+    if (sc.has_key_bit >= 64 * nd.static_words) return fail(h, CCSIM_EINVAL, "template %d: spts has_key_bit", t);
   }
-  if (h->max_prefer_pop + 1 > CCSIM_MAX_CLASSES)
-    return fail(h, CCSIM_EUNSUPPORTED, "a node carries %d PreferNoSchedule taints (max %d)", h->max_prefer_pop, CCSIM_MAX_CLASSES - 1);
+  for (int a = 0; a < T.n_ipa_score; a++) if (T.ipa_score_counter[a] < 0 || T.ipa_score_counter[a] >= n_counters) return fail(h, CCSIM_EINVAL, "ipa score counter index");
+  return CCSIM_OK;
+}
+
+static int check_weights(ccsim_handle *h, int t, const ccsim_template &T) {
+  // a negative weight can make a total negative, and score + 1 <= 0 sets the key's tag bits; the reference's plugin weights
+  // are never negative (framework.go:487-497) and its resource weights are validated to [1, 100] (validation_pluginargs.go)
+  const int32_t w[7] = {T.w_taint, T.w_node_affinity, T.w_fit, T.w_pts, T.w_ipa, T.w_balanced, T.w_image};
+  const char *wname[7] = {"TaintToleration", "NodeAffinity", "NodeResourcesFit", "PodTopologySpread", "InterPodAffinity",
+                          "NodeResourcesBalancedAllocation", "ImageLocality"};
+  for (int q = 0; q < 7; q++)
+    if (w[q] < 0) return fail(h, CCSIM_EUNSUPPORTED, "template %d: %s score weight %d is negative", t, wname[q], w[q]);
+  if (T.least_w_cpu < 1 || T.least_w_cpu > 100 || T.least_w_mem < 1 || T.least_w_mem > 100)
+    return fail(h, CCSIM_EUNSUPPORTED, "template %d: NodeResourcesFit resource weights cpu %d / memory %d outside [1, 100]", t, T.least_w_cpu, T.least_w_mem);
+  long long wsum = 0;
+  for (int q = 0; q < 7; q++) wsum += w[q];
+  if (wsum * 100 >= 4095) return fail(h, CCSIM_EUNSUPPORTED, "template %d: sum of score weights %lld too large for the packed key", t, wsum);
+  return CCSIM_OK;
+}
+
+// Counter c's int32 range (check_run_bounds). dom_slots: the free pod slots of each domain of its column (nullptr: node-local)
+static CounterRange counter_range(const ccsim_handle *h, const ccsim_counter &c, const std::vector<int64_t> *dom_slots) {
+  // domain d stays exact for m placements into it while |init_d| + m * |inc| <= INT32_MAX, i.e. m <= room_d; it receives at
+  // most min(placements, its free slots) of them while NodeResourcesFit filters, at most `placements` otherwise
+  CounterRange r;
+  r.lim_fit = r.lim_any = INT64_MAX; r.dom_fit = r.dom_any = -1; r.init_fit = r.init_any = 0;
+  const int64_t inc = std::llabs((long long)c.inc);
+  for (int32_t d = 0; inc > 0 && d < c.n_domains; d++) {
+    const int64_t room = std::max<int64_t>(0, ((int64_t)INT32_MAX - std::llabs((long long)c.init[d])) / inc);
+    const int64_t slots = !dom_slots ? (d < (int32_t)h->node_slots.size() ? h->node_slots[d] : 0)
+                                     : ((size_t)d < dom_slots->size() ? (*dom_slots)[d] : 0);
+    if (room < r.lim_any) { r.lim_any = room; r.dom_any = d; r.init_any = c.init[d]; }
+    if (slots > room && room < r.lim_fit) { r.lim_fit = room; r.dom_fit = d; r.init_fit = c.init[d]; }
+  }
+  return r;
+}
+
+// The facts and the device copy of the templates (ImageLocality columns: this shard's slice goes to the device, the device copy of
+// the template points at it)
+static int upload_templates(ccsim_handle *h, int32_t n_templates, const ccsim_template *templates, int32_t n_counters, const ccsim_counter *counters) {
+  const ccsim_nodes &nd = h->meta;
   h->h_templates.assign(templates, templates + n_templates);
   TemplateFacts &tf = h->tf;
   tf = TemplateFacts{false, false, nd.taint_words == 1 && nd.static_words <= 1};
@@ -584,18 +617,37 @@ extern "C" int ccsim_set_templates(ccsim_handle *h, int32_t n_templates, const c
   for (int j = 0; j < n_counters; j++) if (counters[j].elig_bit >= 0) tf.has_soft = true;
   if (tf.has_soft) tf.lean_filter = false;
   int rc;
-  {
-    // ImageLocality columns: this shard's slice goes to the device, the device copy of the template points at it
-    std::vector<ccsim_template> dev_t(templates, templates + n_templates);
-    for (int t = 0; t < n_templates; t++)
-      if (templates[t].image_score) {
-        uint8_t *d = nullptr;
-        if ((rc = dev_upload<uint8_t>(h, h->tmpl_allocs, &d, templates[t].image_score + h->node_base, (size_t)h->n))) return rc;
-        dev_t[t].image_score = d;
-      }
-    if ((rc = dev_upload<ccsim_template>(h, h->tmpl_allocs, &h->d_templates, dev_t.data(), (size_t)n_templates))) return rc;
-    CK(cudaStreamSynchronize(h->stream));   // dev_t is about to go out of scope
-  }
+  std::vector<ccsim_template> dev_t(templates, templates + n_templates);
+  for (int t = 0; t < n_templates; t++)
+    if (templates[t].image_score) {
+      uint8_t *d = nullptr;
+      if ((rc = dev_upload<uint8_t>(h, h->tmpl_allocs, &d, templates[t].image_score + h->node_base, (size_t)h->n))) return rc;
+      dev_t[t].image_score = d;
+    }
+  if ((rc = dev_upload<ccsim_template>(h, h->tmpl_allocs, &h->d_templates, dev_t.data(), (size_t)n_templates))) return rc;
+  CK(cudaStreamSynchronize(h->stream));   // dev_t is about to go out of scope
+  return CCSIM_OK;
+}
+
+extern "C" int ccsim_set_templates(ccsim_handle *h, int32_t n_templates, const ccsim_template *templates,
+                                   int32_t n_counters, const ccsim_counter *counters) {
+  if (!h || !templates) return fail(h, CCSIM_EINVAL, "null argument");
+  if (!h->have_nodes) return fail(h, CCSIM_ESTATE, "ccsim_load_nodes must come first");
+  if (n_templates < 1 || n_templates > CCSIM_MAX_TEMPLATES) return fail(h, CCSIM_EINVAL, "n_templates out of range");
+  if (n_counters < 0 || n_counters > CCSIM_MAX_COUNTERS || (n_counters && !counters)) return fail(h, CCSIM_EINVAL, "n_counters out of range");
+  if (n_templates > 1 && n_counters > 0)
+    return fail(h, CCSIM_EUNSUPPORTED, "PodTopologySpread/InterPodAffinity templates are single-template only");
+  CK(cudaSetDevice(h->cfg.device));
+  free_pool(h, h->tmpl_allocs);
+  h->have_templates = false; h->plan.valid = false; h->each_ran = false; h->analyses = false;
+  const ccsim_nodes &nd = h->meta;
+  int rc;
+  for (int t = 0; t < n_templates; t++) if ((rc = check_template(h, t, templates[t], n_counters, counters))) return rc;
+  for (int j = 0; j < n_counters; j++) if (counters[j].elig_bit >= 64 * nd.static_words) return fail(h, CCSIM_EINVAL, "counter %d: elig_bit", j);
+  for (int t = 0; t < n_templates; t++) if ((rc = check_weights(h, t, templates[t]))) return rc;
+  if (h->max_prefer_pop + 1 > CCSIM_MAX_CLASSES)
+    return fail(h, CCSIM_EUNSUPPORTED, "a node carries %d PreferNoSchedule taints (max %d)", h->max_prefer_pop, CCSIM_MAX_CLASSES - 1);
+  if ((rc = upload_templates(h, n_templates, templates, n_counters, counters))) return rc;
   for (int c = 0; c < CCSIM_MAX_PTS; c++) { h->d_stamp[c] = nullptr; h->stamp_len[c] = 0; }
   for (int c = 0; c < templates[0].n_spts; c++)
     if (!templates[0].spts[c].hostname) {
@@ -611,21 +663,7 @@ extern "C" int ccsim_set_templates(ccsim_handle *h, int32_t n_templates, const c
     d.topo_col = c.topo_col; d.inc = c.inc; d.n_present = c.n_present; d.is_aff = 0; d.smem_off = -1; d.work = nullptr; d.elig_bit = c.elig_bit; d.pad = 0;
     for (int a = 0; a < templates[0].n_aff; a++) if (templates[0].aff_counter[a] == j) d.is_aff = 1;
     if (c.topo_col >= nd.n_topo_cols) return fail(h, CCSIM_EINVAL, "counter %d: topo_col", j);
-    {
-      // domain d stays exact for m placements into it while |init_d| + m * |inc| <= INT32_MAX, i.e. m <= room_d; it receives at
-      // most min(placements, its free slots) of them while NodeResourcesFit filters, at most `placements` otherwise
-      auto &r = h->cnt_range[j];
-      r.lim_fit = r.lim_any = INT64_MAX; r.dom_fit = r.dom_any = -1; r.init_fit = r.init_any = 0;
-      const int64_t inc = std::llabs((long long)c.inc);
-      const bool local = c.topo_col < 0;
-      for (int32_t d = 0; inc > 0 && d < c.n_domains; d++) {
-        const int64_t room = std::max<int64_t>(0, ((int64_t)INT32_MAX - std::llabs((long long)c.init[d])) / inc);
-        const int64_t slots = local ? (d < (int32_t)h->node_slots.size() ? h->node_slots[d] : 0)
-                                    : ((size_t)d < h->dom_slots[c.topo_col].size() ? h->dom_slots[c.topo_col][d] : 0);
-        if (room < r.lim_any) { r.lim_any = room; r.dom_any = d; r.init_any = c.init[d]; }
-        if (slots > room && room < r.lim_fit) { r.lim_fit = room; r.dom_fit = d; r.init_fit = c.init[d]; }
-      }
-    }
+    h->cnt_range[j] = counter_range(h, c, c.topo_col < 0 ? nullptr : &h->dom_slots[c.topo_col]);
     if (c.topo_col < 0) {
       // node-local: init is a whole-cluster column; keep this shard's slice
       if (c.n_domains != h->n_global) return fail(h, CCSIM_EINVAL, "counter %d: node-local counter needs n_domains == n_nodes", j);
@@ -648,6 +686,189 @@ extern "C" int ccsim_set_templates(ccsim_handle *h, int32_t n_templates, const c
   return CCSIM_OK;
 }
 
+// Tree levels of the per-analysis kernel: roots on level L, 32^L >= n
+static int each_tree_levels(int32_t n) {
+  int L = 0;
+  while (n > 0 && (1ll << (5 * L)) < n) L++;
+  return L;
+}
+
+extern "C" int ccsim_set_analyses(ccsim_handle *h, int32_t n_templates, const ccsim_template *templates, const ccsim_analysis_terms *terms) {
+  if (!h || !templates || !terms) return fail(h, CCSIM_EINVAL, "null argument");
+  if (!h->have_nodes) return fail(h, CCSIM_ESTATE, "ccsim_load_nodes must come first");
+  if (n_templates < 1 || n_templates > CCSIM_MAX_TEMPLATES) return fail(h, CCSIM_EINVAL, "n_templates out of range");
+  CK(cudaSetDevice(h->cfg.device));
+  free_pool(h, h->tmpl_allocs);
+  h->have_templates = false; h->plan.valid = false; h->each_ran = false; h->analyses = false;
+  const ccsim_nodes &nd = h->meta;
+  const int32_t n = h->n;
+  if (h->cfg.world > 1) return fail(h, CCSIM_EUNSUPPORTED, "per-analysis runs: node-sharded runs (world %d) are not supported", h->cfg.world);
+  int rc;
+  for (int t = 0; t < n_templates; t++) {   // every analysis validated as ccsim_set_templates validates its template alone
+    const ccsim_analysis_terms &A = terms[t];
+    if (A.n_counters < 0 || A.n_counters > CCSIM_MAX_COUNTERS || (A.n_counters && !A.counters))
+      return fail(h, CCSIM_EINVAL, "analysis %d: n_counters out of range", t);
+    if (A.n_topo_cols < 0 || A.n_topo_cols > CCSIM_MAX_TOPO_COLS) return fail(h, CCSIM_EINVAL, "analysis %d: n_topo_cols out of range", t);
+    for (int k = 0; k < A.n_topo_cols; k++) if (!A.topo[k] && n > 0) return fail(h, CCSIM_EINVAL, "analysis %d: null topo column %d", t, k);
+    if ((rc = check_template(h, t, templates[t], A.n_counters, A.counters))) return rc;
+    for (int j = 0; j < A.n_counters; j++) {
+      const ccsim_counter &c = A.counters[j];
+      if (c.elig_bit >= 64 * nd.static_words) return fail(h, CCSIM_EINVAL, "analysis %d: counter %d: elig_bit", t, j);
+      if (c.topo_col >= A.n_topo_cols) return fail(h, CCSIM_EINVAL, "analysis %d: counter %d: topo_col", t, j);
+      if (c.topo_col < 0 ? c.n_domains != n : (c.n_domains < 0 || c.n_present < 0 || c.n_present > c.n_domains))
+        return fail(h, CCSIM_EINVAL, "analysis %d: counter %d: domains", t, j);
+      if (c.n_domains > 0 && !c.init) return fail(h, CCSIM_EINVAL, "analysis %d: counter %d: null init", t, j);
+      if (c.topo_col >= 0)
+        for (int32_t i = 0; i < n; i++)
+          if (A.topo[c.topo_col][i] >= c.n_domains) return fail(h, CCSIM_EINVAL, "analysis %d: counter %d: node %d's domain out of range", t, j, i);
+    }
+  }
+  for (int t = 0; t < n_templates; t++) if ((rc = check_weights(h, t, templates[t]))) return rc;
+  if (h->max_prefer_pop + 1 > CCSIM_MAX_CLASSES)
+    return fail(h, CCSIM_EUNSUPPORTED, "a node carries %d PreferNoSchedule taints (max %d)", h->max_prefer_pop, CCSIM_MAX_CLASSES - 1);
+  if ((rc = upload_templates(h, n_templates, templates, 0, nullptr))) return rc;
+  const int ncls = h->max_prefer_pop + 1, L = each_tree_levels(n);
+  h->an.assign((size_t)n_templates, AnalysisState());
+  std::vector<EachTerms> dev_terms((size_t)n_templates);
+  h->max_seg = ncls;
+  for (int t = 0; t < n_templates; t++) {
+    const ccsim_template &T = templates[t];
+    const ccsim_analysis_terms &A = terms[t];
+    AnalysisState &S = h->an[t];
+    EachTerms &E = S.terms;
+    memset(&E, 0, sizeof(E));
+    S.n_topo = A.n_topo_cols;
+    // the columns, and whether a column's domains hold one node each
+    bool single[CCSIM_MAX_TOPO_COLS] = {};
+    for (int k = 0; k < A.n_topo_cols; k++) {
+      int32_t *d = nullptr;
+      if ((rc = dev_upload<int32_t>(h, h->tmpl_allocs, &d, A.topo[k], (size_t)n))) return rc;
+      E.topo[k] = d;
+      std::vector<int64_t> &slots = S.dom_slots[k];
+      std::vector<int32_t> members;
+      for (int32_t i = 0; i < n; i++) {
+        const int32_t dd = A.topo[k][i];
+        if (dd < 0) continue;
+        if ((size_t)dd >= slots.size()) { slots.resize((size_t)dd + 1, 0); members.resize((size_t)dd + 1, 0); }
+        slots[dd] += h->node_slots[i];
+        members[dd]++;
+      }
+      single[k] = std::all_of(members.begin(), members.end(), [](int32_t m) { return m <= 1; });
+    }
+    // the counters: their initial counts, one block of working counts, the int32 range of each
+    int32_t total = 0;
+    for (int j = 0; j < A.n_counters; j++) { S.final_off[j] = total; total += A.counters[j].n_domains; }
+    if ((rc = dev_alloc<int32_t>(h, h->tmpl_allocs, &S.work, (size_t)std::max(total, 1)))) return rc;
+    E.n_counters = A.n_counters;
+    for (int j = 0; j < A.n_counters; j++) {
+      const ccsim_counter &c = A.counters[j];
+      DevCounter &d = E.counters[j];
+      d.topo_col = c.topo_col; d.n_domains = c.n_domains; d.n_present = c.n_present; d.inc = c.inc; d.smem_off = -1; d.elig_bit = c.elig_bit;
+      for (int a = 0; a < T.n_aff; a++) if (T.aff_counter[a] == j) d.is_aff = 1;
+      int32_t *init = nullptr;
+      if ((rc = dev_upload<int32_t>(h, h->tmpl_allocs, &init, c.init, (size_t)c.n_domains))) return rc;
+      d.init = init; d.work = S.work + S.final_off[j];
+      S.range[j] = counter_range(h, c, c.topo_col < 0 ? nullptr : &S.dom_slots[c.topo_col]);
+    }
+    // the terms: folded into the leaf when their domains hold one node each, else tested per domain group
+    const uint32_t fe = T.filter_enable;
+    bool group_col[CCSIM_MAX_TOPO_COLS] = {};
+    auto place = [&](int counter, uint32_t bit) {
+      const int32_t col = A.counters[counter].topo_col;
+      if (col < 0 || single[col]) E.leaf_sel |= bit;
+      else { E.group_sel |= bit; group_col[col] = true; }
+    };
+    if (fe & CCSIM_PL_POD_TOPOLOGY_SPREAD) for (int c = 0; c < T.n_pts; c++) place(T.pts[c].counter, 1u << c);
+    if (fe & CCSIM_PL_INTER_POD_AFFINITY) {
+      for (int a = 0; a < T.n_aff; a++) place(T.aff_counter[a], COUPLED_AFF_SEL(a));
+      for (int a = 0; a < T.n_anti; a++) place(T.anti_counter[a], COUPLED_ANTI_SEL(a));
+    }
+    // domain groups: (class, domain in each group column), a stable partition of the nodes; without group terms one group per class
+    std::vector<int32_t> gcols;
+    for (int k = 0; k < A.n_topo_cols; k++) if (group_col[k]) gcols.push_back(k);
+    const size_t kw = 1 + gcols.size();
+    std::vector<int32_t> key((size_t)n * kw);
+    for (int32_t i = 0; i < n; i++) {
+      int cls = 0;
+      if (T.score_enable & CCSIM_PL_TAINT_TOLERATION)
+        for (int w = 0; w < nd.taint_words; w++) cls += __builtin_popcountll(h->h_taint[(size_t)w * n + i] & nd.taint_prefer[w] & ~T.tol_prefer[w]);
+      key[(size_t)i * kw] = cls;
+      for (size_t q = 0; q < gcols.size(); q++) key[(size_t)i * kw + 1 + q] = A.topo[gcols[q]][i];
+    }
+    std::vector<int32_t> order((size_t)n);
+    for (int32_t i = 0; i < n; i++) order[i] = i;
+    auto less = [&](int32_t x, int32_t y) {
+      return std::lexicographical_compare(&key[(size_t)x * kw], &key[(size_t)x * kw + kw], &key[(size_t)y * kw], &key[(size_t)y * kw + kw]);
+    };
+    std::stable_sort(order.begin(), order.end(), less);
+    std::vector<int32_t> pos((size_t)n), rep, cls;
+    std::vector<long long> start;
+    for (int32_t r = 0; r < n; r++) {
+      const int32_t i = order[r];
+      pos[i] = r;
+      if (E.group_sel && (r == 0 || less(order[r - 1], i))) { start.push_back(r); rep.push_back(i); cls.push_back(key[(size_t)i * kw]); }
+    }
+    if (!E.group_sel)   // segment c = class c (possibly empty), as the class trees of node-local templates
+      for (int c = 0; c < ncls; c++) {
+        start.push_back(std::lower_bound(order.begin(), order.end(), c, [&](int32_t x, int v) { return key[(size_t)x * kw] < v; }) - order.begin());
+        rep.push_back(0); cls.push_back(c);
+      }
+    const int32_t G = (int32_t)start.size();
+    if (G > CCSIM_EACH_MAX_GROUPS)
+      return fail(h, CCSIM_EUNSUPPORTED, "per-analysis runs: analysis %d has %d domain groups (max %d)", t, G, CCSIM_EACH_MAX_GROUPS);
+    std::vector<long long> cof((size_t)(L + 1) * (G + 1));
+    for (int g = 0; g < G; g++) cof[g] = start[g];
+    cof[G] = n;
+    for (int l = 1; l <= L; l++) {
+      long long acc = 0;
+      for (int g = 0; g < G; g++) {
+        const long long sz = cof[(size_t)(l - 1) * (G + 1) + g + 1] - cof[(size_t)(l - 1) * (G + 1) + g];
+        cof[(size_t)l * (G + 1) + g] = acc; acc += (sz + 31) >> 5;
+      }
+      cof[(size_t)l * (G + 1) + G] = acc;
+    }
+    E.n_seg = G;
+    h->max_seg = std::max(h->max_seg, G);
+    long long *d_cof = nullptr; int32_t *d_rep = nullptr, *d_cls = nullptr, *d_pos = nullptr;
+    if ((rc = dev_upload<long long>(h, h->tmpl_allocs, &d_cof, cof.data(), cof.size())) ||
+        (rc = dev_upload<int32_t>(h, h->tmpl_allocs, &d_rep, rep.data(), rep.size())) ||
+        (rc = dev_upload<int32_t>(h, h->tmpl_allocs, &d_cls, cls.data(), cls.size())) ||
+        (rc = dev_upload<int32_t>(h, h->tmpl_allocs, &d_pos, pos.data(), pos.size())))
+      return rc;
+    E.cof = d_cof; E.seg_rep = d_rep; E.seg_cls = d_cls; E.pos = d_pos;
+    CK(cudaStreamSynchronize(h->stream));   // the host vectors go out of scope
+    dev_terms[t] = E;
+  }
+  if ((rc = dev_upload<EachTerms>(h, h->tmpl_allocs, &h->d_terms, dev_terms.data(), (size_t)n_templates))) return rc;
+  CK(cudaStreamSynchronize(h->stream));
+  h->n_templates = n_templates; h->n_counters = 0; h->final_total = 0;
+  h->analyses = true;
+  h->have_templates = true;
+  return CCSIM_OK;
+}
+
+// Counters are int32 here and in the oracle; the reference counts in int64 (podtopologyspread/scoring.go,
+// interpodaffinity/scoring.go). A counter that could leave int32 during the run is refused, never left to wrap: a domain that
+// receives m placements holds init + m' * inc with m' <= m, so |init| + m * |inc| <= INT32_MAX keeps every value exact, and m is
+// at most min(placements, the domain's free pod slots) while NodeResourcesFit filters. `who` prefixes the message.
+static int check_counter_bounds(ccsim_handle *h, int64_t max_pods, bool fit_off, int n_counters, const DevCounter *counters,
+                                const CounterRange *ranges, const std::vector<int64_t> *dom_slots, const char *who) {
+  int64_t placements = h->pod_bound;
+  if (max_pods > 0 && (max_pods < placements || fit_off)) placements = max_pods;
+  for (int j = 0; j < n_counters; j++) {
+    const CounterRange &r = ranges[j];
+    const int64_t lim = fit_off ? r.lim_any : r.lim_fit;
+    const int32_t d = fit_off ? r.dom_any : r.dom_fit;
+    if (placements > lim) {
+      const int32_t tc = counters[j].topo_col;
+      const int64_t m = fit_off ? placements : std::min(placements, tc < 0 ? (int64_t)h->node_slots[d] : dom_slots[tc][d]);
+      return fail(h, CCSIM_EUNSUPPORTED, "%scounter %d, domain %d: |initial count| %lld + %lld placements x |increment| %d can leave int32",
+                  who, j, d, std::llabs((long long)(fit_off ? r.init_any : r.init_fit)), (long long)m, std::abs(counters[j].inc));
+    }
+  }
+  return CCSIM_OK;
+}
+
 // The refusals a run meets before it touches anything: a run that nothing bounds, and counters that could leave int32. `cap`: the
 // output capacity, since no run can place more than sum(max(0, alloc_pods - npods)) pods (fit.go:567-576), or max_pods.
 static int check_run_bounds(ccsim_handle *h, int64_t max_pods, int64_t &cap) {
@@ -658,24 +879,7 @@ static int check_run_bounds(ccsim_handle *h, int64_t max_pods, int64_t &cap) {
     return fail(h, CCSIM_EUNSUPPORTED, "NodeResourcesFit is disabled for a template: the run is unbounded, --max-limit is required");
   cap = h->pod_bound + 1;
   if (max_pods > 0 && (max_pods < cap || fit_off)) cap = max_pods;
-  // Counters are int32 here and in the oracle; the reference counts in int64 (podtopologyspread/scoring.go,
-  // interpodaffinity/scoring.go). A counter that could leave int32 during the run is refused, never left to wrap: a domain that
-  // receives m placements holds init + m' * inc with m' <= m, so |init| + m * |inc| <= INT32_MAX keeps every value exact, and m is
-  // at most min(placements, the domain's free pod slots) while NodeResourcesFit filters.
-  int64_t placements = h->pod_bound;
-  if (max_pods > 0 && (max_pods < placements || fit_off)) placements = max_pods;
-  for (int j = 0; j < h->n_counters; j++) {
-    const auto &r = h->cnt_range[j];
-    const int64_t lim = fit_off ? r.lim_any : r.lim_fit;
-    const int32_t d = fit_off ? r.dom_any : r.dom_fit;
-    if (placements > lim) {
-      const int32_t tc = h->counters[j].topo_col;
-      const int64_t m = fit_off ? placements : std::min(placements, tc < 0 ? (int64_t)h->node_slots[d] : h->dom_slots[tc][d]);
-      return fail(h, CCSIM_EUNSUPPORTED, "counter %d, domain %d: |initial count| %lld + %lld placements x |increment| %d can leave int32",
-                  j, d, std::llabs((long long)(fit_off ? r.init_any : r.init_fit)), (long long)m, std::abs(h->counters[j].inc));
-    }
-  }
-  return CCSIM_OK;
+  return check_counter_bounds(h, max_pods, fit_off, h->n_counters, h->counters, h->cnt_range, h->dom_slots, "");
 }
 
 // The pod -> node buffer grown to `cap`; the working columns restored from the snapshot (a Run never changes the snapshot)
@@ -877,6 +1081,7 @@ static int plan_stream(ccsim_handle *h, RunPlan &pl, const WaveKernel *&k) {
 // process: every rank must be past its allocations before any rank's persistent kernel starts waiting for its peers.
 static int run_prepare(ccsim_handle *h, int64_t max_pods) {
   if (!h->have_nodes || !h->have_templates) return fail(h, CCSIM_ESTATE, "load_nodes and set_templates must come first");
+  if (h->analyses) return fail(h, CCSIM_ESTATE, "templates set by ccsim_set_analyses run with ccsim_run_each only");
   if (h->cfg.world > 1 && !h->peers_ready) return fail(h, CCSIM_ESTATE, "sharded run: ccsim_peer_import must come first");
   CK(cudaSetDevice(h->cfg.device));
   RunPlan &pl = h->plan;
@@ -1032,9 +1237,10 @@ extern "C" int ccsim_run_each(ccsim_handle *h, int64_t max_pods, ccsim_result *o
   // the per-analysis kernel covers node-local templates only: placing a clone must change nothing but its node
   if (h->cfg.world > 1) return fail(h, CCSIM_EUNSUPPORTED, "per-analysis runs: node-sharded runs (world %d) are not supported", h->cfg.world);
   if (h->cfg.sampling == CCSIM_SAMPLING_REFERENCE) return fail(h, CCSIM_EUNSUPPORTED, "per-analysis runs: reference sampling is not supported");
+  // one counter table and one placed mask describe one run; ccsim_set_analyses gives every analysis its own
   if (h->n_counters > 0)
     return fail(h, CCSIM_EUNSUPPORTED, "per-analysis runs: per-domain counters (topology spread, pod (anti-)affinity) are not supported");
-  if (h->w_placed) return fail(h, CCSIM_EUNSUPPORTED, "per-analysis runs: hostPorts (placed mask) are not supported");
+  if (h->w_placed && !h->analyses) return fail(h, CCSIM_EUNSUPPORTED, "per-analysis runs: hostPorts (placed mask) are not supported");
   for (int t = 0; t < T; t++) {
     const ccsim_template &P = h->h_templates[t];
     if ((P.n_pref_terms > 0 && (P.score_enable & CCSIM_PL_NODE_AFFINITY)) || (P.n_spts > 0 && (P.score_enable & CCSIM_PL_POD_TOPOLOGY_SPREAD)) ||
@@ -1050,10 +1256,17 @@ extern "C" int ccsim_run_each(ccsim_handle *h, int64_t max_pods, ccsim_result *o
     int64_t c = h->pod_bound + 1;
     if (max_pods > 0 && (max_pods < c || fit_off)) c = max_pods;
     cap = std::max(cap, c);
+    if (h->analyses) {
+      const AnalysisState &S = h->an[t];
+      char who[32]; snprintf(who, sizeof(who), "analysis %d: ", t);
+      int rc = check_counter_bounds(h, max_pods, fit_off, S.terms.n_counters, S.terms.counters, S.range, S.dom_slots, who);
+      if (rc) return rc;
+    }
   }
   CK(cudaSetDevice(h->cfg.device));
   const int32_t n = h->n;
   const int ncls = h->max_prefer_pop + 1;
+  const int nseg = h->analyses ? h->max_seg : ncls;   // tree segments per analysis: classes, or domain groups
   {
     size_t free_b = 0, total_b = 0;
     CK(cudaMemGetInfo(&free_b, &total_b));
@@ -1067,14 +1280,13 @@ extern "C" int ccsim_run_each(ccsim_handle *h, int64_t max_pods, ccsim_result *o
   memset(out, 0, sizeof(ccsim_result) * (size_t)T);
   // tree shape: roots on level L (32^L >= N); levels [1, split) in global memory, [split, L] in shared memory, the lowest split whose
   // shared levels fit next to the kernel's static structs
-  int L = 0;
-  while (n > 0 && (1ll << (5 * L)) < n) L++;
-  const WaveKernel &kern = WAVE_KERNELS[WK_EACH];
+  const int L = each_tree_levels(n);
+  const WaveKernel &kern = WAVE_KERNELS[h->analyses ? WK_EACH_TERMS : WK_EACH];
   int split = 1;
   size_t smem = 0;
   for (; split <= L + 1; split++) {
     smem = 0;
-    for (int l = split; l <= L; l++) smem += 8 * (size_t)each_level_bound(n, l, ncls);
+    for (int l = split; l <= L; l++) smem += 8 * (size_t)each_level_bound(n, l, nseg);
     if (smem + kern.static_smem + 1024 <= h->smem_optin) break;
   }
   EachParams ep; memset(&ep, 0, sizeof(ep));
@@ -1082,8 +1294,8 @@ extern "C" int ccsim_run_each(ccsim_handle *h, int64_t max_pods, ccsim_result *o
   {
     long long g = 0, s = 0;
     for (int l = 1; l <= L; l++) {
-      if (l < split) { ep.lev_off[l] = g; g += each_level_bound(n, l, ncls); }
-      else { ep.lev_off[l] = s; s += each_level_bound(n, l, ncls); }
+      if (l < split) { ep.lev_off[l] = g; g += each_level_bound(n, l, nseg); }
+      else { ep.lev_off[l] = s; s += each_level_bound(n, l, nseg); }
     }
     ep.glev_stride = g;
   }
@@ -1094,9 +1306,11 @@ extern "C" int ccsim_run_each(ccsim_handle *h, int64_t max_pods, ccsim_result *o
       (rc = dev_alloc<unsigned long long>(h, h->each_allocs, &ep.glev, (size_t)T * ep.glev_stride)) ||
       (rc = dev_alloc<int32_t>(h, h->each_allocs, &ep.seq, (size_t)T * cap)) || (rc = dev_alloc<EachOut>(h, h->each_allocs, &ep.out, (size_t)T)))
     return rc;
-  if (ncls > 1 && (rc = dev_alloc<int32_t>(h, h->each_allocs, &ep.pos, tn))) return rc;
+  if (!h->analyses && ncls > 1 && (rc = dev_alloc<int32_t>(h, h->each_allocs, &ep.pos, tn))) return rc;
   DevOut *d_diag = nullptr;
   if ((rc = dev_alloc<DevOut>(h, h->each_allocs, &d_diag, (size_t)T))) return rc;
+  ep.terms = h->analyses ? h->d_terms : nullptr;
+  ep.diag = d_diag;
   ep.s_req_cpu = h->s_req_cpu; ep.s_req_mem = h->s_req_mem; ep.s_req_eph = h->s_req_eph; ep.s_nz_cpu = h->s_nz_cpu; ep.s_nz_mem = h->s_nz_mem;
   ep.s_npods = h->s_npods;
   for (int q = 0; q < h->meta.n_scalars; q++) ep.s_req_scalar[q] = h->s_req_scalar[q];
@@ -1124,8 +1338,16 @@ extern "C" int ccsim_run_each(ccsim_handle *h, int64_t max_pods, ccsim_result *o
       if (eo[t].stop_code != CCSIM_STOP_UNSCHEDULABLE) continue;
       const int blocks = std::min(4 * h->sm_count, (n + 255) / 256);
       ccsim_each_scatter_kernel<<<blocks, 256, 0, s>>>(p, ep, t);
-      p.out = d_diag + t;
-      ccsim_diag_kernel<<<blocks, 256, 0, s>>>(p, t);
+      DevParams pd = p;
+      if (h->analyses) {   // the analysis's own counters (where the run left them) and columns
+        const AnalysisState &S = h->an[t];
+        pd.n_counters = S.terms.n_counters; pd.n_topo = S.n_topo;
+        for (int j = 0; j < S.terms.n_counters; j++) { pd.counters[j] = S.terms.counters[j]; pd.final_off[j] = S.final_off[j]; }
+        pd.final_cnt = S.work;
+        for (int k = 0; k < CCSIM_MAX_TOPO_COLS; k++) pd.topo[k] = S.terms.topo[k];
+      }
+      pd.out = d_diag + t;
+      ccsim_diag_kernel<<<blocks, 256, 0, s>>>(pd, t);
       h->launches += 2;
       CK(cudaGetLastError());
     }
@@ -1141,9 +1363,10 @@ extern "C" int ccsim_run_each(ccsim_handle *h, int64_t max_pods, ccsim_result *o
     if (eo[t].placed) CK(cudaMemcpyAsync(h->each_seq[t].data(), ep.seq + (size_t)t * cap, (size_t)eo[t].placed * 4, cudaMemcpyDeviceToHost, s));
   }
   CK(cudaStreamSynchronize(s));
-  int64_t waves = 0, placed = 0;
+  int64_t waves = 0, placed = 0, rebuilds = 0;
   for (int t = 0; t < T; t++) {
     ccsim_result &r = out[t];
+    rebuilds += n > 0 ? eo[t].rebuilds : 0;
     const bool unsched = eo[t].stop_code == CCSIM_STOP_UNSCHEDULABLE;
     r.placed = eo[t].placed; r.stop_code = eo[t].stop_code; r.n_nodes = h->n_global;
     r.waves = eo[t].placed + (unsched ? 1 : 0);
@@ -1163,6 +1386,7 @@ extern "C" int ccsim_run_each(ccsim_handle *h, int64_t max_pods, ccsim_result *o
   h->last_stat[0] = ENG_EACH; h->last_stat[1] = waves; h->last_stat[2] = placed;
   h->last_stat[3] = std::min(split - 1, L); h->last_stat[4] = L - std::min(split - 1, L);   // upper tree levels in global / shared memory
   h->last_stat[5] = T; h->last_stat[6] = kern.block; h->last_stat[7] = (int64_t)smem;
+  h->last_stat[8] = rebuilds;                                                                 // leaf and level rebuilds, all analyses
   h->last_key_order_waves = 0;
   h->each_ran = true;
   return CCSIM_OK;

@@ -149,6 +149,10 @@ struct cc_handle {
   // cc_run_each: one read-only view per podspec (cc_analysis); a view's node names are its base's
   std::vector<std::unique_ptr<cc_handle>> analyses;
   const cc_handle *base = nullptr;
+  // cc_new_each: a per-analysis handle; parts[t] holds podspec t's own terms (counters, counter inits, topology columns, PreFilter
+  // message, node count; its static bits moved like the merged template's), the node columns of its encoding are dropped after the merge
+  bool each = false;
+  std::vector<Encoded> parts;
 };
 
 // the encoding a handle's node indices refer to (a view's is its base's)
@@ -170,16 +174,20 @@ static void shl256(const uint64_t in[CCSIM_MAX_STATIC_WORDS], int off, uint64_t 
 // Several templates against one snapshot (the roadmap's "list of pods", README.md:305-306; template index = k % T,
 // report.go:160): every template is encoded on its own, then the snapshots are merged — node state and the taint dictionary do
 // not depend on the template; the static predicate bits of template t move up by the bits of templates 0..t-1; extended
-// resources are the union. Per-domain counters (PodTopologySpread / InterPodAffinity terms) stay single-template.
+// resources are the union. A list handle's run is one run: per-domain counters (PodTopologySpread / InterPodAffinity terms) stay
+// single-template there. A per-analysis handle (h->each) keeps every part's counters, counter inits, topology columns and PreFilter
+// message as that analysis's own (h->parts), and its hostPort self-conflict becomes bit t.
 static void encode_list(cc_handle *h) {
   const size_t T = h->tmpls.size();
-  std::vector<Encoded> parts;
+  std::vector<Encoded> &parts = h->parts;
+  parts.clear();
   parts.reserve(T);
   for (size_t t = 0; t < T; t++) {
     Encoder enc(h->cfg, h->tmpls[t], h->nodes, h->pods, h->ns_labels, h->exclude);
     enc.set_workloads(&h->workloads);
     parts.push_back(enc.encode());
     const Encoded &e = parts.back();
+    if (h->each) continue;
     if (!e.counters.empty()) throw Unsupported("several podspecs of which one has topology spread / pod (anti-)affinity terms or scores (single podspec only)");
     if (!e.prefilter_msg.empty()) throw Unsupported("several podspecs of which one is rejected by PreFilter");
     if (e.has_placed_mask) throw Unsupported("several podspecs with hostPorts");
@@ -217,6 +225,8 @@ static void encode_list(cc_handle *h) {
     }
     if (parts[t].tmpl.prefilter_bit >= 0) hi = std::max(hi, parts[t].tmpl.prefilter_bit + 1);
     if (parts[t].tmpl.spts_ignored_bit >= 0) hi = std::max(hi, parts[t].tmpl.spts_ignored_bit + 1);
+    for (const ccsim_counter &c : parts[t].counters) if (c.elig_bit >= 0) hi = std::max(hi, c.elig_bit + 1);
+    for (int c = 0; c < parts[t].tmpl.n_spts; c++) if (parts[t].tmpl.spts[c].has_key_bit >= 0) hi = std::max(hi, parts[t].tmpl.spts[c].has_key_bit + 1);
     off[t] = total; nbits[t] = hi; total += hi;
   }
   if (total > 64 * CCSIM_MAX_STATIC_WORDS) throw Unsupported("the podspecs need more than 256 static node-predicate bits together");
@@ -239,6 +249,12 @@ static void encode_list(cc_handle *h) {
     for (int k = 0; k < CCSIM_MAX_AFF_TERMS; k++) { mv(P.aff_term_mask[k]); mv(P.pref_mask[k]); }
     if (P.prefilter_bit >= 0) P.prefilter_bit += off[t];
     if (P.spts_ignored_bit >= 0) P.spts_ignored_bit += off[t];
+    for (int c = 0; c < P.n_spts; c++) if (P.spts[c].has_key_bit >= 0) P.spts[c].has_key_bit += off[t];
+    if (h->each) {
+      for (ccsim_counter &c : parts[t].counters) if (c.elig_bit >= 0) c.elig_bit += off[t];
+      if (P.port_tmpl_conflict & 1ull) P.port_tmpl_conflict = 1ull << t;   // a clone conflicts with the analysis's own clones
+      parts[t].tmpl = P;
+    }
     // extended resources: re-index into the union
     int64_t rs[CCSIM_MAX_SCALARS] = {0, 0, 0, 0};
     for (size_t k = 0; k < e.scalar_names.size(); k++) rs[std::find(names.begin(), names.end(), e.scalar_names[k]) - names.begin()] = e.tmpl.req_scalar[k];
@@ -248,11 +264,21 @@ static void encode_list(cc_handle *h) {
     h->enc_tmpls[t] = P;
   }
   m.tmpl = h->enc_tmpls[0];
+  if (h->each) {   // the terms are the parts'; each part keeps only them
+    for (auto &e : parts) m.has_placed_mask |= e.has_placed_mask;
+    m.counters.clear(); m.counter_init.clear(); m.topo.clear(); m.prefilter_msg.clear();
+    for (auto &e : parts) {
+      Encoded k;
+      k.n = e.n; k.counters = std::move(e.counters); k.counter_init = std::move(e.counter_init); k.topo = std::move(e.topo);
+      k.prefilter_msg = std::move(e.prefilter_msg); k.tmpl = e.tmpl;
+      e = std::move(k);
+    }
+  } else parts.clear();
 }
 
 static void ensure_encoded(cc_handle *h) {
   if (h->have_enc) return;
-  if (h->tmpls.size() > 1) { encode_list(h); h->have_enc = true; return; }
+  if (h->tmpls.size() > 1 || h->each) { encode_list(h); h->have_enc = true; return; }
   auto t0 = std::chrono::steady_clock::now();
   Encoder enc(h->cfg, h->tmpl, h->nodes, h->pods, h->ns_labels, h->exclude);
   enc.set_workloads(&h->workloads);
@@ -302,6 +328,13 @@ extern "C" int cc_new_list(const char *sched_config_json, const char *pods_json,
   if (!pods_json || !out) return fail(nullptr, CC_EINVAL, "null argument");
   try { return new_handle(sched_config_json, items_of(pods_json), max_pods, exclude_nodes, device, out); }
   catch (const std::exception &e) { return fail(nullptr, CC_EINVAL, e.what()); }
+}
+
+extern "C" int cc_new_each(const char *sched_config_json, const char *pods_json, int64_t max_pods, const char *exclude_nodes,
+                           int32_t device, cc_handle **out) {
+  const int rc = cc_new_list(sched_config_json, pods_json, max_pods, exclude_nodes, device, out);
+  if (rc == CC_OK) (*out)->each = true;
+  return rc;
 }
 
 static std::vector<Json> items_of(const char *text) {
@@ -710,7 +743,22 @@ static ccsim_handle *loaded_engine(cc_handle *h, const ccsim_config &cfg, int &r
   if (!(rc = ccsim_load_nodes(eng, &nd))) {
     tick("ccsim_load_nodes");
     what = "ccsim_set_templates";
-    if (!(rc = ccsim_set_templates(eng, (int32_t)h->enc_tmpls.size(), h->enc_tmpls.data(), (int32_t)E.counters.size(), E.counters.data()))) {
+    if (h->each) {   // every analysis with its own counters and columns
+      what = "ccsim_set_analyses";
+      std::vector<std::vector<ccsim_counter>> ctr(h->parts.size());
+      std::vector<ccsim_analysis_terms> terms(h->parts.size());
+      for (size_t t = 0; t < h->parts.size(); t++) {
+        const Encoded &e = h->parts[t];
+        ctr[t] = e.counters;
+        for (size_t j = 0; j < ctr[t].size(); j++) ctr[t][j].init = e.counter_init[j].data();
+        ccsim_analysis_terms &a = terms[t];
+        memset(&a, 0, sizeof(a));
+        a.n_counters = (int32_t)ctr[t].size(); a.counters = ctr[t].data();
+        a.n_topo_cols = (int32_t)e.topo.size();
+        for (size_t k = 0; k < e.topo.size() && k < CCSIM_MAX_TOPO_COLS; k++) a.topo[k] = e.topo[k].data();
+      }
+      if (!(rc = ccsim_set_analyses(eng, (int32_t)h->enc_tmpls.size(), h->enc_tmpls.data(), terms.data()))) { tick(what); return eng; }
+    } else if (!(rc = ccsim_set_templates(eng, (int32_t)h->enc_tmpls.size(), h->enc_tmpls.data(), (int32_t)E.counters.size(), E.counters.data()))) {
       tick("ccsim_set_templates");
       return eng;
     }
@@ -739,6 +787,7 @@ static ccsim_config engine_config(const cc_handle *h) {
 
 extern "C" int cc_run(cc_handle *h) {
   if (!h) return CC_EINVAL;
+  if (h->each) return fail(h, CC_ESTATE, "a per-analysis handle (cc_new_each) runs with cc_run_each");
   int rc = encode_for_run(h);
   if (rc) return rc;
   const Encoded &E = h->enc;
@@ -786,9 +835,10 @@ extern "C" int cc_run_each(cc_handle *h) {
   if ((rc = ccsim_run_each(eng, h->max_pods, res.data()))) return engine_failed(h, eng, "ccsim_run_each", rc);
   for (size_t t = 0; t < T; t++) {
     cc_handle &v = *views[t];
+    v.ran = true;
+    if (h->each && stop_before_engine(h->parts[t], v.stop_reason)) continue;   // PreFilter rejected podspec t: no placements
     v.pod_node.assign(res[t].pod_node, res[t].pod_node + res[t].placed);
     v.stop_reason = stop_reason_of(E, res[t], h->max_pods, h->tmpls[t]);   // every pod of analysis t is a clone of podspec t
-    v.ran = true;
   }
   engine_release(cfg, eng);
   h->analyses = std::move(views);
@@ -1009,6 +1059,22 @@ extern "C" const char *cc_debug_encoded_snapshot(cc_handle *h) {
   j.set("counters", ctr);
   { Json is = Json::array(); for (auto x : E.image_score) is.push(Json::number(x)); j.set("image_score", is); }   // template_hex holds a process-local pointer
   j.set("prefilter_msg", Json::string(E.prefilter_msg));
+  if (h->each) {   // a per-analysis handle: every analysis's own terms
+    Json an = Json::array();
+    for (const Encoded &e : h->parts) {
+      Json a = Json::object(), ac = Json::array(), at = Json::array();
+      for (size_t k = 0; k < e.counters.size(); k++) {
+        Json c = Json::object();
+        c.set("topo_col", Json::number(e.counters[k].topo_col)); c.set("n_present", Json::number(e.counters[k].n_present));
+        c.set("inc", Json::number(e.counters[k].inc)); c.set("elig_bit", Json::number(e.counters[k].elig_bit)); c.set("init", arr32(e.counter_init[k]));
+        ac.push(c);
+      }
+      for (auto &c : e.topo) at.push(arr32(c));
+      a.set("counters", ac); a.set("topo", at); a.set("prefilter_msg", Json::string(e.prefilter_msg));
+      an.push(a);
+    }
+    j.set("analyses", an);
+  }
   h->out = json_dump(j);
   return h->out.c_str();
 }

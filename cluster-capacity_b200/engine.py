@@ -17,7 +17,7 @@ _lib = None
 EXPORTS = ["ccsim_create", "ccsim_destroy", "ccsim_last_error", "ccsim_abi_version", "ccsim_load_nodes",
            "ccsim_set_templates", "ccsim_run", "ccsim_prepare", "ccsim_node_counts", "ccsim_peer_export", "ccsim_peer_import",
            "ccsim_device_info", "ccsim_kernel_launches", "ccsim_kernel_name", "ccsim_flush_l2", "ccsim_run_stats", "ccsim_peer_local",
-           "ccsim_peer_import_local", "ccsim_key_order_waves", "ccsim_run_each"]
+           "ccsim_peer_import_local", "ccsim_key_order_waves", "ccsim_run_each", "ccsim_set_analyses"]
 
 
 class EngineError(RuntimeError):
@@ -41,6 +41,8 @@ def lib():
         L.ccsim_load_nodes.argtypes = [C.c_void_p, C.POINTER(abi.Nodes)]
         L.ccsim_set_templates.restype = C.c_int
         L.ccsim_set_templates.argtypes = [C.c_void_p, C.c_int32, C.POINTER(abi.Template), C.c_int32, C.POINTER(abi.Counter)]
+        L.ccsim_set_analyses.restype = C.c_int
+        L.ccsim_set_analyses.argtypes = [C.c_void_p, C.c_int32, C.POINTER(abi.Template), C.POINTER(abi.AnalysisTerms)]
         L.ccsim_prepare.restype = C.c_int
         L.ccsim_prepare.argtypes = [C.c_void_p, C.c_int64]
         L.ccsim_run.restype = C.c_int
@@ -120,6 +122,22 @@ class Engine:
         self._check(lib().ccsim_set_templates(self._h, len(templates), T, len(counters), Cn), "ccsim_set_templates")
         self._n_templates = len(templates)
 
+    def set_analyses(self, templates, terms):
+        """Templates for run_each() with every analysis's own terms (ccsim_set_analyses). terms[t] = (counters, topo columns):
+        abi.Counter structs whose topo_col index the analysis's int32 numpy columns of n_nodes domain ids."""
+        T = (abi.Template * len(templates))(*templates)
+        A = (abi.AnalysisTerms * len(templates))()
+        keep = []
+        for t, (counters, cols) in enumerate(terms):
+            Cn = (abi.Counter * max(1, len(counters)))(*counters)
+            cols = [np.ascontiguousarray(c, dtype=np.int32) for c in cols]
+            keep += [Cn, cols]
+            A[t].n_counters, A[t].n_topo_cols, A[t].counters = len(counters), len(cols), Cn
+            for k, c in enumerate(cols):
+                A[t].topo[k] = c.ctypes.data_as(abi.P32)
+        self._check(lib().ccsim_set_analyses(self._h, len(templates), T, A), "ccsim_set_analyses")
+        self._n_templates = len(templates)
+
     def prepare(self, max_pods=0):
         """The allocation / restore half of run(max_pods); see ccsim_prepare."""
         self._check(lib().ccsim_prepare(self._h, max_pods), "ccsim_prepare")
@@ -184,8 +202,8 @@ class Engine:
         st = {"engine": self.ENGINE_NAMES[int(v[0])] if int(v[0]) < len(self.ENGINE_NAMES) else self.EACH_ENGINE, "kernel": self.kernel_name(), "waves": int(v[1]), "placed": int(v[2]),
               "candidates": int(v[3]), "bar_raised_waves": int(v[4]), "grid": int(v[5]), "block": int(v[6]), "smem_bytes": int(v[7]),
               "phase_cycles": [int(x) for x in v[8:16]]}
-        if int(v[0]) == 5:      # per-analysis runs: where the upper levels of the max-trees live
-            st["global_levels"], st["shared_levels"] = int(v[3]), int(v[4])
+        if int(v[0]) == 5:      # per-analysis runs: where the upper levels of the max-trees live, rebuilds of all analyses
+            st["global_levels"], st["shared_levels"], st["rebuilds"] = int(v[3]), int(v[4]), int(v[8])
         return st
 
     def key_order_waves(self):

@@ -54,6 +54,12 @@ int cc_new(const char *sched_config_json, const char *pod_json, int64_t max_pods
  * one of them does not fit or at max_pods. Podspecs with topology-spread / pod-(anti-)affinity terms are single-podspec only. */
 int cc_new_list(const char *sched_config_json, const char *pods_json, int64_t max_pods, const char *exclude_nodes,
                 int32_t device, cc_handle **out);
+/* A per-analysis handle: the arguments of cc_new_list, run with cc_run_each only (cc_run fails with CC_ESTATE). Every podspec keeps
+ * its own topology-spread and pod-(anti-)affinity counters, topology columns and hostPorts, so podspecs with hard (DoNotSchedule)
+ * spread, required pod (anti-)affinity and hostPorts are analysed like cc_new(podspec t) + cc_run; a podspec PreFilter rejects ends
+ * its own analysis with cc_run's message and no placements. */
+int cc_new_each(const char *sched_config_json, const char *pods_json, int64_t max_pods, const char *exclude_nodes,
+                int32_t device, cc_handle **out);
 int cc_sync_with_objects(cc_handle *h, const char *nodes_json, const char *pods_json, const char *namespaces_json);
 /* Optional, between cc_sync_with_objects and cc_run: the Services / ReplicationControllers / ReplicaSets / StatefulSets
  * SyncWithClient copies (simulator.go:217-281). The scheduler reads them in one place only: helper.DefaultSelector
@@ -64,8 +70,11 @@ int cc_sync_workloads(cc_handle *h, const char *services_json, const char *rcs_j
                       const char *statefulsets_json);
 int cc_run(cc_handle *h);
 /* Every podspec of the handle analysed on its own against the synced snapshot, all in one GPU launch: analysis t is what
- * cc_new(podspec t) + cc_sync_with_objects + cc_run gives under the same configuration, max_pods and exclude_nodes. Node-local
- * podspecs only: topology spread, pod (anti-)affinity, normalised soft scorers, hostPorts and reference sampling are refused by name. */
+ * cc_new(podspec t) + cc_sync_with_objects + cc_run gives under the same configuration, max_pods and exclude_nodes. On a cc_new_list
+ * handle node-local podspecs only: topology spread, pod (anti-)affinity and hostPorts are refused by name; a cc_new_each handle takes
+ * them. Always refused by name: normalised soft scorers (preferred node affinity, ScheduleAnyway / system-default spreading,
+ * InterPodAffinity scoring, which a required affinity matching the pod's own labels brings under hardPodAffinityWeight > 0),
+ * node shards and reference sampling. */
 int cc_run_each(cc_handle *h);
 /* After cc_run_each: a read-only view of analysis t (podspec t alone and its Status), owned by h and valid until the next
  * cc_run_each or cc_close(h). cc_report_json / cc_report_print / cc_stop_reason / cc_scheduled_* read it like a handle of its own;

@@ -300,10 +300,29 @@ int  ccsim_run(ccsim_handle *h, int64_t max_pods, ccsim_result *out);
  * template t alone (pod_node, placed, stop_code, reason_hist, preempt_*); waves = placed (+1 when Unschedulable), evals = the nodes
  * pushed through the Filter (every node once, then each placement's winner), examined = waves * n_nodes, run_ms = the whole launch.
  * pod_node arrays are owned by the handle until the next run. Afterwards ccsim_node_counts(h, t, ...) gives analysis t's counts.
- * Refuses (CCSIM_EUNSUPPORTED, before any launch): per-domain counters, normalised soft scorers, hostPorts (placed mask), world > 1,
+ * After ccsim_set_templates it refuses (CCSIM_EUNSUPPORTED, before any launch) per-domain counters and hostPorts (placed mask): one
+ * counter table is one run's; ccsim_set_analyses gives each analysis its own. Always refused: normalised soft scorers, world > 1,
  * reference sampling, a template without NodeResourcesFit when max_pods <= 0, and sequence buffers (n_templates x min(max_pods,
  * free pod slots + 1) x 4 B) larger than the free device memory. */
 int  ccsim_run_each(ccsim_handle *h, int64_t max_pods, ccsim_result *out /* [n_templates] */);
+
+/* The per-analysis terms of one template (ccsim_set_analyses): its own counters and topology columns, what ccsim_set_templates and
+ * ccsim_load_nodes give a run of that template alone. counters[].topo_col indexes topo[]; topo[k] holds n_nodes domain ids. */
+typedef struct ccsim_analysis_terms {
+  int32_t n_counters;                    /* <= CCSIM_MAX_COUNTERS */
+  int32_t n_topo_cols;                   /* <= CCSIM_MAX_TOPO_COLS */
+  const ccsim_counter *counters;
+  const int32_t *topo[CCSIM_MAX_TOPO_COLS];
+} ccsim_analysis_terms;
+
+/* Templates for per-analysis runs whose coupled terms (hard topology spread, required pod (anti-)affinity, hostPorts) are each
+ * analysis's own: template t's pts[].counter, aff_counter[] and anti_counter[] index terms[t].counters, and a hostPort self-conflict
+ * is bit t of its port_tmpl_conflict. Validates every analysis as ccsim_set_templates validates one template (CCSIM_EINVAL for
+ * indexes, CCSIM_EUNSUPPORTED for weights), and refuses (CCSIM_EUNSUPPORTED) an analysis with more than CCSIM_EACH_MAX_GROUPS
+ * domain groups (DESIGN.md §4.1g). Afterwards ccsim_run_each runs them, each bounded like ccsim_run of its template alone
+ * (int32 counters included); ccsim_run and ccsim_prepare fail with CCSIM_ESTATE until the next ccsim_set_templates. */
+#define CCSIM_EACH_MAX_GROUPS 4096
+int  ccsim_set_analyses(ccsim_handle *h, int32_t n_templates, const ccsim_template *templates, const ccsim_analysis_terms *terms);
 /* Optional: everything ccsim_run(h, max_pods) does BEFORE the wave kernel starts (buffers, restoring the snapshot, engine choice),
  * synchronously. A host that drives several ranks from one process calls it on every handle, then starts the ccsim_run calls
  * concurrently: no rank's persistent kernel then waits for a peer that is still inside a (device-synchronising) allocation. */
