@@ -7,16 +7,16 @@
 // placement reads the root, commits the winner, re-evaluates that one node and re-reduces O(log N) entries.
 //
 // One tree segment per normalisation class (untolerated PreferNoSchedule taints, static per template and node): the segments cover a
-// stable partition of the nodes by class, and their roots go through select_host_over_classes like the class winners of the wave
-// kernels. Level 0 (the leaves) and the upper levels that do not fit in shared memory live in global memory; the host chooses the
-// split (EachParams::split).
+// stable partition of the nodes by class, made on the host (EachTerms: segment offsets, each node's leaf position), and their roots go
+// through select_host_over_classes like the class winners of the wave kernels. Level 0 (the leaves) and the upper levels that do not
+// fit in shared memory live in global memory; the host chooses the split (EachParams::split).
 //
 // Templates with coupled terms (ccsim_set_analyses: hard spread, required pod (anti-)affinity, hostPorts) keep their counters per
 // analysis (EachTerms). A term whose domains hold one node each (node-local counters, hostname columns) and the hostPort self-conflict
 // (k > 0) depend on the node's own clones only: they fold into the leaf. The other terms split the nodes into domain groups (class,
-// domain in each of their columns), partitioned on the host; each group is a segment, and a placement takes a group's root only when
-// the group's domains pass those terms (coupled_ok on one of its nodes, the code filter_node runs). When a leaf-folded term changes
-// on every node at once (a folded spread minimum moves, the affinity bypass ends) the leaves and levels are rebuilt.
+// domain in each of their columns), also partitioned on the host; each group is a segment, and a placement takes a group's root only
+// when the group's domains pass those terms (coupled_ok on one of its nodes, the code filter_node runs). When a leaf-folded term
+// changes on every node at once (a folded spread minimum moves, the affinity bypass ends) the leaves and levels are rebuilt.
 #pragma once
 
 #define EACH_THREADS 512
@@ -33,13 +33,14 @@ struct EachTerms {      // one analysis's coupled terms (ccsim_set_analyses), de
   DevCounter counters[CCSIM_MAX_COUNTERS];   // work: the analysis's working counts (initialised from init at kernel start)
   const int32_t *topo[CCSIM_MAX_TOPO_COLS];  // the analysis's topology columns
   int32_t n_counters;
-  int32_t n_seg;        // domain groups = tree segments
+  int32_t n_seg;        // tree segments: classes, or domain groups
+  int32_t port_self;    // a clone's hostPorts conflict with the next clone's (template bit t, with a placed mask as in ccsim_run)
   uint32_t leaf_sel;    // coupled_ok selection of the terms folded into the leaf
   uint32_t group_sel;   // the terms tested per group
   const long long *cof; // [(L + 1) * (n_seg + 1)]: group s's entries of level l are [cof[l * (n_seg + 1) + s], cof[... + s + 1])
   const int32_t *seg_rep;   // [n_seg] a node of group s (its domains in the group columns are the group's)
   const int32_t *seg_cls;   // [n_seg] the group's normalisation class
-  int32_t *pos;             // [n] leaf position of each node
+  const int32_t *pos;       // [n] leaf position of each node; nullptr when the partition is the identity
 };
 
 struct EachParams {
@@ -51,11 +52,10 @@ struct EachParams {
   long long max_pods;
   int32_t *k;                   // [T][N] clones placed on each node
   unsigned long long *leaf;     // [T][N] leaf keys in partition order
-  int32_t *pos;                 // [T][N] leaf position of each node; nullptr with one class (position = node index)
   unsigned long long *glev;     // [T][glev_stride]
   int32_t *seq;                 // [T][seq_cap] node of clone k
   EachOut *out;                 // [T]
-  const EachTerms *terms;       // [T] (ccsim_set_analyses), nullptr: node-local templates, partitioned by class here
+  const EachTerms *terms;       // [T]
   DevOut *diag;                 // [T] the diagnosis's outputs: final spread minima and affinity total
   // the snapshot rows a node's state is computed from
   const int64_t *s_req_cpu, *s_req_mem, *s_req_eph, *s_nz_cpu, *s_nz_mem;
@@ -68,10 +68,8 @@ struct __align__(16) EachShared {
   FilterConsts fc;
   ScoreWeights sw;
   int32_t w_image;
-  int32_t wcnt[EACH_THREADS / 32][CCSIM_MAX_CLASSES];   // partition: nodes of each class per warp in the current chunk
-  int32_t crun[CCSIM_MAX_CLASSES];                       // partition: next position of each class
-  long long coff[EACH_MAX_LEVELS + 1][CCSIM_MAX_CLASSES + 1];   // class c's entries of level l: [coff[l][c], coff[l][c+1])
-  const long long *cof;   // segment offsets: es.coff (classes) or the analysis's group table
+  long long coff[EACH_MAX_LEVELS + 1][CCSIM_MAX_CLASSES + 1];   // node-local analyses: class c's entries of level l, the host's cof
+  const long long *cof;   // the analysis's segment offsets (EachTerms::cof)
   int32_t cstride, nseg;  // entries per level of cof, segments
   int32_t grouped;        // segments are domain groups: a placement tests each group's terms and takes the maximum per class
   int32_t coupled;        // the analysis has counters or hostPorts
@@ -84,8 +82,8 @@ struct __align__(16) EachShared {
   unsigned long long aff_total;
 };
 __shared__ EachShared es;
-// G: the analyses have ccsim_set_analyses terms (segments from the host's table); else class segments in es.coff, read directly
-// (the node-local path's per-placement loads stay plain shared-memory loads)
+// G: some analysis has counters or a hostPort self-conflict (segments from the host's table); else the analyses are node-local, their
+// segments are classes and the host's offsets are read from es.coff (the per-placement loads stay plain shared-memory loads)
 template <bool G> __device__ __forceinline__ long long cof(int l, int s) {
   return G ? es.cof[(long long)l * es.cstride + s] : es.coff[l][s];
 }
@@ -119,11 +117,6 @@ __device__ void each_pts_recount(int c, int lane) {
 // x + k * r with the wrap of k repeated int64 additions (the wave kernels' commit)
 __device__ __forceinline__ long long each_add(int64_t x, uint32_t k, int64_t r) {
   return (long long)((unsigned long long)x + (unsigned long long)k * (unsigned long long)r);
-}
-
-// normalisation class of node i (filter_node's raw TaintToleration count): static per template and node
-__device__ __forceinline__ int each_class(const DevParams &p, int32_t ti, int32_t i) {
-  return __popcll(p.taint_mask[i] & es.fc.prefer0) + (p.taint_words > 1 ? prefer_count_hi(p.self, ti, i) : 0);
 }
 
 // leaf key of node i after kk clones of the analysis's template: filter_node's Filter and the wave kernel's score on the computed
@@ -166,11 +159,12 @@ __device__ __forceinline__ unsigned long long *each_level(const EachParams &ep, 
 }
 
 // every leaf at its node's position, evaluated after its current clones (at kernel start: none), by threads t0, t0 + nt, ...
+template <bool G>
 __device__ void each_leaves(const DevParams &p, const EachParams &ep, int32_t ti, int32_t *kcol, unsigned long long *leaf,
                             const int32_t *pos, bool start, int t0, int nt) {
   for (int32_t i = t0; i < p.n; i += nt) {
     if (start) kcol[i] = 0;
-    leaf[pos[i]] = each_leaf<true>(p, ep, ti, i, start ? 0u : (uint32_t)kcol[i]);
+    leaf[pos ? pos[i] : i] = each_leaf<G>(p, ep, ti, i, start ? 0u : (uint32_t)kcol[i]);
   }
 }
 
@@ -192,8 +186,7 @@ __device__ void each_levels(const EachParams &ep, unsigned long long *leaf, unsi
   }
 }
 
-// G: the analyses of ccsim_set_analyses (coupled terms, host-made groups); else node-local templates, partitioned by class here. Two
-// instantiations, so that the node-local one is compiled and register-allocated on its own
+// Two instantiations (G above), so that the node-local one is compiled and register-allocated on its own
 template <bool G>
 __global__ void __launch_bounds__(EACH_THREADS, 1) ccsim_each_kernel(const DevParams p, const EachParams ep) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -201,18 +194,17 @@ __global__ void __launch_bounds__(EACH_THREADS, 1) ccsim_each_kernel(const DevPa
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nw = blockDim.x >> 5;
   const int32_t ti = blockIdx.x, n = p.n;
   const int ncls = p.n_classes, L = ep.n_levels;
-  const EachTerms *et = G ? ep.terms + ti : nullptr;
+  const EachTerms *et = ep.terms + ti;
   int32_t *kcol = ep.k + (size_t)ti * n;
   unsigned long long *leaf = ep.leaf + (size_t)ti * n;
-  int32_t *pos = et ? et->pos : (ep.pos ? ep.pos + (size_t)ti * n : nullptr);
+  const int32_t *pos = et->pos;
   unsigned long long *glev = ep.glev + (size_t)ti * ep.glev_stride;
   int32_t *seq = ep.seq + (size_t)ti * ep.seq_cap;
 
   // ---- template, the analysis's working counters, folded Filter constants, score configuration ----
   for (int q = tid; q < (int)(sizeof(ccsim_template) / 8); q += blockDim.x)
     reinterpret_cast<unsigned long long *>(&es.tmpl)[q] = reinterpret_cast<const unsigned long long *>(&p.templates[ti])[q];
-  if (tid < CCSIM_MAX_CLASSES) es.crun[tid] = 0;
-  const int ncnt = et ? et->n_counters : 0;
+  const int ncnt = et->n_counters;
   for (int j = 0; j < ncnt; j++) {
     const DevCounter &dc = et->counters[j];
     for (int d = tid; d < dc.n_domains; d += blockDim.x) dc.work[d] = dc.init[d];
@@ -221,13 +213,12 @@ __global__ void __launch_bounds__(EACH_THREADS, 1) ccsim_each_kernel(const DevPa
   if (tid == 0) {
     const ccsim_template &t = es.tmpl;
     es.aff_total = (unsigned long long)t.aff_total_init;
-    es.leaf_sel = et ? et->leaf_sel : 0u; es.group_sel = et ? et->group_sel : 0u;
-    es.grouped = et && et->group_sel ? 1 : 0;
-    es.port_self = et && (t.filter_enable & CCSIM_PL_NODE_PORTS) && (t.flags & CCSIM_TF_HAS_HOST_PORTS) && ((t.port_tmpl_conflict >> ti) & 1ull);
+    es.leaf_sel = et->leaf_sel; es.group_sel = et->group_sel;
+    es.grouped = et->group_sel ? 1 : 0;
+    es.port_self = et->port_self;
     es.coupled = ncnt > 0 || es.port_self;
-    if (et) { es.cof = et->cof; es.cstride = et->n_seg + 1; es.nseg = et->n_seg; }
-    else { es.cof = &es.coff[0][0]; es.cstride = CCSIM_MAX_CLASSES + 1; es.nseg = ncls; }
-    for (int k = 0; k < CCSIM_MAX_TOPO_COLS; k++) es.topo_ptr[k] = et ? et->topo[k] : nullptr;
+    es.cof = et->cof; es.cstride = et->n_seg + 1; es.nseg = et->n_seg;
+    for (int k = 0; k < CCSIM_MAX_TOPO_COLS; k++) es.topo_ptr[k] = et->topo[k];
     for (int j = 0; j < CCSIM_MAX_COUNTERS; j++) es.cnt_ptr[j] = j < ncnt ? et->counters[j].work : nullptr;
     for (int j = 0; j < ncnt; j++) {   // what a commit does to each counter (the generic wave kernel's CommitInfo)
       const DevCounter &dc = et->counters[j];
@@ -244,7 +235,7 @@ __global__ void __launch_bounds__(EACH_THREADS, 1) ccsim_each_kernel(const DevPa
   __syncthreads();
   if (tid == 0) {
     const ccsim_template &t = es.tmpl;
-    build_filter_consts(p, et ? et->counters : p.counters, t, ti, es.topo_ptr, es.cnt_ptr, es.ptsmin, (long long)es.aff_total, es.fc);
+    build_filter_consts(p, et->counters, t, ti, es.topo_ptr, es.cnt_ptr, es.ptsmin, (long long)es.aff_total, es.fc);
     es.fc.extras &= ~CCSIM_X_PLACED;   // hostPorts against the analysis's own clones: k > 0 in the leaf
     es.sw.w_fit = (t.score_enable & CCSIM_PL_FIT) ? t.w_fit : 0;
     es.sw.w_balanced = ((t.score_enable & CCSIM_PL_BALANCED) && !(t.flags & CCSIM_TF_BALANCED_SKIP)) ? t.w_balanced : 0;
@@ -255,70 +246,13 @@ __global__ void __launch_bounds__(EACH_THREADS, 1) ccsim_each_kernel(const DevPa
   if (warp == 0) for (int c = 0; c < es.fc.n_pts; c++) each_pts_recount(c, lane);   // the spread minima and their limits
   __syncthreads();
 
-  if (G) {
-    // ---- leaves at the host's positions (partition by domain group) ----
-    each_leaves(p, ep, ti, kcol, leaf, pos, true, tid, blockDim.x);
-  } else {
-    // ---- class sizes (several classes only): class c's leaves are positions [coff[0][c], coff[0][c+1]) ----
-    if (ncls > 1) {
-      int cnt[CCSIM_MAX_CLASSES] = {};
-      for (int32_t i = tid; i < n; i += blockDim.x) {
-        const int c = each_class(p, ti, i);
-        #pragma unroll
-        for (int q = 0; q < CCSIM_MAX_CLASSES; q++) cnt[q] += (q == c);
-      }
-      #pragma unroll
-      for (int q = 0; q < CCSIM_MAX_CLASSES; q++) {
-        const int v = __reduce_add_sync(0xffffffffu, cnt[q]);
-        if (lane == 0 && v) atomicAdd(&es.crun[q], v);
-      }
-    } else if (tid == 0) es.crun[0] = n;
-    __syncthreads();
-    if (tid == 0) {   // entries per class and level: ceil(size / 32^l); crun becomes the partition's running position
-      long long run = 0;
-      for (int c = 0; c < ncls; c++) { const long long sz = es.crun[c]; es.crun[c] = (int32_t)run; es.coff[0][c] = run; run += sz; }
-      es.coff[0][ncls] = run;
-      for (int l = 1; l <= L; l++) {
-        long long acc = 0;
-        for (int c = 0; c < ncls; c++) {
-          const long long sz = es.coff[l - 1][c + 1] - es.coff[l - 1][c];
-          es.coff[l][c] = acc; acc += (sz + 31) >> 5;
-        }
-        es.coff[l][ncls] = acc;
-      }
-    }
-    __syncthreads();
+  if (!G)   // the host's class offsets into shared memory (classes <= CCSIM_MAX_CLASSES, levels <= EACH_MAX_LEVELS)
+    for (int q = tid; q < (L + 1) * (es.nseg + 1); q += blockDim.x) es.coff[q / (es.nseg + 1)][q % (es.nseg + 1)] = et->cof[q];
 
-    // ---- leaves: stable partition by class (node order inside a class), every node evaluated with no clone placed ----
-    for (int32_t base = 0; base < n; base += blockDim.x) {
-      const int32_t i = base + tid;
-      int32_t at = i;
-      if (ncls > 1) {
-        const int c = i < n ? each_class(p, ti, i) : -1;
-        int rank = 0;
-        for (int q = 0; q < ncls; q++) {
-          const unsigned b = __ballot_sync(0xffffffffu, c == q);
-          if (c == q) rank = __popc(b & ((1u << lane) - 1u));
-          if (lane == 0) es.wcnt[warp][q] = __popc(b);
-        }
-        __syncthreads();
-        if (c >= 0) {
-          at = es.crun[c] + rank;
-          for (int w = 0; w < warp; w++) at += es.wcnt[w][c];
-        }
-        __syncthreads();
-        if (tid < ncls) { int s = 0; for (int w = 0; w < nw; w++) s += es.wcnt[w][tid]; es.crun[tid] += s; }
-        __syncthreads();
-      }
-      if (i < n) {
-        kcol[i] = 0;
-        if (pos) pos[i] = at;
-        leaf[at] = each_leaf<false>(p, ep, ti, i, 0u);
-      }
-    }
-  }
+  // ---- leaves at the host's positions, every node evaluated with no clone placed; then the upper levels ----
+  each_leaves<G>(p, ep, ti, kcol, leaf, pos, true, tid, blockDim.x);
   __syncthreads();
-  each_levels<G, true>(ep, leaf, glev, slev, G ? es.nseg : ncls, warp, nw, lane);
+  each_levels<G, true>(ep, leaf, glev, slev, es.nseg, warp, nw, lane);
 
   // ---- placements: warp 0 alone ----
   if (warp != 0) return;
@@ -402,7 +336,7 @@ __global__ void __launch_bounds__(EACH_THREADS, 1) ccsim_each_kernel(const DevPa
       __syncwarp();
     }
     if (G && rebuild) {   // every leaf and level again, with the code of the kernel start
-      each_leaves(p, ep, ti, kcol, leaf, pos, false, lane, 32);
+      each_leaves<G>(p, ep, ti, kcol, leaf, pos, false, lane, 32);
       __syncwarp();
       each_levels<G, false>(ep, leaf, glev, slev, es.nseg, 0, 1, lane);
       rebuilds++;

@@ -193,8 +193,8 @@ static const WaveKernel WAVE_KERNELS[] = {
   {(const void *)ccsim_wave_stream_kernel<0>, "stream<0>", ENG_STREAM, STREAM_BLOCK, sizeof(StreamShared), stream_smem_bytes(0, 0)},
   {(const void *)ccsim_wave_stream_kernel<1>, "stream<1>", ENG_STREAM, STREAM_BLOCK, sizeof(StreamShared), stream_smem_bytes(1, 0)},
   {(const void *)ccsim_wave_stream_kernel<2>, "stream<2>", ENG_STREAM, STREAM_BLOCK, sizeof(StreamShared), 0},
-  {(const void *)ccsim_each_kernel<false>, "each", ENG_EACH, EACH_THREADS, sizeof(EachShared), 0},   // ccsim_run_each only
-  {(const void *)ccsim_each_kernel<true>, "each", ENG_EACH, EACH_THREADS, sizeof(EachShared), 0},    // ... after ccsim_set_analyses
+  {(const void *)ccsim_each_kernel<false>, "each", ENG_EACH, EACH_THREADS, sizeof(EachShared), 0},   // ccsim_run_each: node-local analyses
+  {(const void *)ccsim_each_kernel<true>, "each", ENG_EACH, EACH_THREADS, sizeof(EachShared), 0},    // ... some with counters or hostPorts
 };
 enum { WK_WAVE, WK_WAVE_STREAMED, WK_LEAN, WK_LEAN_SAMPLING, WK_BATCHED, WK_MULTI, WK_MULTI_SHARDED, WK_STREAM /* + mode */,
        WK_EACH = WK_STREAM + 3, WK_EACH_TERMS };
@@ -215,7 +215,7 @@ struct TemplateFacts { bool fit_off, has_soft, lean_filter; };
 // pod slots (lim_fit) or not (lim_any), and the domain that sets each bound
 struct CounterRange { int64_t lim_fit, lim_any; int32_t dom_fit, dom_any, init_fit, init_any; };
 
-// ccsim_set_analyses: one analysis's terms as the host keeps them
+// ccsim_run_each: one analysis's terms and tree segments as the host keeps them
 struct AnalysisState {
   EachTerms terms;                            // its device copy is d_terms[t]
   int32_t n_topo = 0;
@@ -303,11 +303,11 @@ struct ccsim_handle {
   int32_t *d_each_seq = nullptr; int64_t each_seq_cap = 0;
   std::vector<int64_t> each_placed;
   std::vector<std::vector<int32_t>> each_seq;
-  // ccsim_set_analyses: every analysis's own counters, columns and domain groups (until the next ccsim_set_templates)
-  bool analyses = false;
+  // ccsim_run_each: every analysis's own counters, columns and tree segments, made by ccsim_set_analyses or, for the node-local
+  // templates of ccsim_set_templates, by the first ccsim_run_each (until the next ccsim_set_templates / set_analyses / load_nodes)
+  bool analyses = false;                      // the templates came from ccsim_set_analyses
   std::vector<AnalysisState> an;
   EachTerms *d_terms = nullptr;
-  int32_t max_seg = 0;                        // most tree segments of an analysis
   std::vector<uint64_t> h_taint;              // the loaded taint masks (word-major): the normalisation class of each node
 };
 
@@ -431,7 +431,7 @@ extern "C" int ccsim_load_nodes(ccsim_handle *h, const ccsim_nodes *nd) {
     return fail(h, CCSIM_EINVAL, "ccsim_nodes dimensions out of range");
   CK(cudaSetDevice(h->cfg.device));
   free_pool(h, h->allocs);
-  h->have_nodes = false; h->have_templates = false; h->plan.valid = false;
+  h->have_nodes = false; h->have_templates = false; h->plan.valid = false; h->an.clear();
   const int32_t N = nd->n_nodes;
   // node-axis shard of this rank (SURVEY.md §8e): contiguous block of the nodeTree order
   const int32_t per = (N + h->cfg.world - 1) / h->cfg.world;
@@ -538,8 +538,9 @@ static bool needs_extras(const ccsim_handle *h, const ccsim_template &T) {
   return false;
 }
 
-// One template's index ranges against its counter table (CCSIM_EINVAL) and its score weights (CCSIM_EUNSUPPORTED)
-static int check_template(ccsim_handle *h, int t, const ccsim_template &T, int32_t n_counters, const ccsim_counter *counters) {
+// One template's index ranges against its counter table, and the counters' eligibility bits (CCSIM_EINVAL; `who` prefixes the
+// counter messages)
+static int check_template(ccsim_handle *h, int t, const ccsim_template &T, int32_t n_counters, const ccsim_counter *counters, const char *who) {
   const ccsim_nodes &nd = h->meta;
   if (T.n_pref_terms < 0 || T.n_pref_terms > CCSIM_MAX_AFF_TERMS) return fail(h, CCSIM_EINVAL, "template %d: n_pref_terms", t);
   if (T.n_pts < 0 || T.n_pts > CCSIM_MAX_PTS || T.n_aff < 0 || T.n_aff > CCSIM_MAX_IPA || T.n_anti < 0 || T.n_anti > CCSIM_MAX_IPA ||
@@ -564,6 +565,7 @@ static int check_template(ccsim_handle *h, int t, const ccsim_template &T, int32
     if (sc.has_key_bit >= 64 * nd.static_words) return fail(h, CCSIM_EINVAL, "template %d: spts has_key_bit", t);
   }
   for (int a = 0; a < T.n_ipa_score; a++) if (T.ipa_score_counter[a] < 0 || T.ipa_score_counter[a] >= n_counters) return fail(h, CCSIM_EINVAL, "ipa score counter index");
+  for (int j = 0; j < n_counters; j++) if (counters[j].elig_bit >= 64 * nd.static_words) return fail(h, CCSIM_EINVAL, "%scounter %d: elig_bit", who, j);
   return CCSIM_OK;
 }
 
@@ -600,10 +602,24 @@ static CounterRange counter_range(const ccsim_handle *h, const ccsim_counter &c,
   return r;
 }
 
-// The facts and the device copy of the templates (ImageLocality columns: this shard's slice goes to the device, the device copy of
-// the template points at it)
+// What both setters do first: the state and count checks, then the handle's templates, counters and analyses dropped
+static int begin_templates(ccsim_handle *h, int32_t n_templates) {
+  if (!h->have_nodes) return fail(h, CCSIM_ESTATE, "ccsim_load_nodes must come first");
+  if (n_templates < 1 || n_templates > CCSIM_MAX_TEMPLATES) return fail(h, CCSIM_EINVAL, "n_templates out of range");
+  CK(cudaSetDevice(h->cfg.device));
+  free_pool(h, h->tmpl_allocs);
+  h->have_templates = false; h->plan.valid = false; h->each_ran = false; h->analyses = false; h->an.clear();
+  return CCSIM_OK;
+}
+
+// The score weights and the class limit checked, then the facts and the device copy of the templates (ImageLocality columns: this
+// shard's slice goes to the device, the device copy of the template points at it)
 static int upload_templates(ccsim_handle *h, int32_t n_templates, const ccsim_template *templates, int32_t n_counters, const ccsim_counter *counters) {
   const ccsim_nodes &nd = h->meta;
+  int rc;
+  for (int t = 0; t < n_templates; t++) if ((rc = check_weights(h, t, templates[t]))) return rc;
+  if (h->max_prefer_pop + 1 > CCSIM_MAX_CLASSES)
+    return fail(h, CCSIM_EUNSUPPORTED, "a node carries %d PreferNoSchedule taints (max %d)", h->max_prefer_pop, CCSIM_MAX_CLASSES - 1);
   h->h_templates.assign(templates, templates + n_templates);
   TemplateFacts &tf = h->tf;
   tf = TemplateFacts{false, false, nd.taint_words == 1 && nd.static_words <= 1};
@@ -616,7 +632,6 @@ static int upload_templates(ccsim_handle *h, int32_t n_templates, const ccsim_te
   }
   for (int j = 0; j < n_counters; j++) if (counters[j].elig_bit >= 0) tf.has_soft = true;
   if (tf.has_soft) tf.lean_filter = false;
-  int rc;
   std::vector<ccsim_template> dev_t(templates, templates + n_templates);
   for (int t = 0; t < n_templates; t++)
     if (templates[t].image_score) {
@@ -629,24 +644,25 @@ static int upload_templates(ccsim_handle *h, int32_t n_templates, const ccsim_te
   return CCSIM_OK;
 }
 
+// Counter j of template T on the device, without its columns (init, work) and its place (smem_off)
+static DevCounter dev_counter(const ccsim_counter &c, const ccsim_template &T, int j) {
+  DevCounter d;
+  memset(&d, 0, sizeof(d));
+  d.topo_col = c.topo_col; d.n_domains = c.n_domains; d.n_present = c.n_present; d.inc = c.inc; d.smem_off = -1; d.elig_bit = c.elig_bit;
+  for (int a = 0; a < T.n_aff; a++) if (T.aff_counter[a] == j) d.is_aff = 1;
+  return d;
+}
+
 extern "C" int ccsim_set_templates(ccsim_handle *h, int32_t n_templates, const ccsim_template *templates,
                                    int32_t n_counters, const ccsim_counter *counters) {
   if (!h || !templates) return fail(h, CCSIM_EINVAL, "null argument");
-  if (!h->have_nodes) return fail(h, CCSIM_ESTATE, "ccsim_load_nodes must come first");
-  if (n_templates < 1 || n_templates > CCSIM_MAX_TEMPLATES) return fail(h, CCSIM_EINVAL, "n_templates out of range");
+  int rc;
+  if ((rc = begin_templates(h, n_templates))) return rc;
   if (n_counters < 0 || n_counters > CCSIM_MAX_COUNTERS || (n_counters && !counters)) return fail(h, CCSIM_EINVAL, "n_counters out of range");
   if (n_templates > 1 && n_counters > 0)
     return fail(h, CCSIM_EUNSUPPORTED, "PodTopologySpread/InterPodAffinity templates are single-template only");
-  CK(cudaSetDevice(h->cfg.device));
-  free_pool(h, h->tmpl_allocs);
-  h->have_templates = false; h->plan.valid = false; h->each_ran = false; h->analyses = false;
   const ccsim_nodes &nd = h->meta;
-  int rc;
-  for (int t = 0; t < n_templates; t++) if ((rc = check_template(h, t, templates[t], n_counters, counters))) return rc;
-  for (int j = 0; j < n_counters; j++) if (counters[j].elig_bit >= 64 * nd.static_words) return fail(h, CCSIM_EINVAL, "counter %d: elig_bit", j);
-  for (int t = 0; t < n_templates; t++) if ((rc = check_weights(h, t, templates[t]))) return rc;
-  if (h->max_prefer_pop + 1 > CCSIM_MAX_CLASSES)
-    return fail(h, CCSIM_EUNSUPPORTED, "a node carries %d PreferNoSchedule taints (max %d)", h->max_prefer_pop, CCSIM_MAX_CLASSES - 1);
+  for (int t = 0; t < n_templates; t++) if ((rc = check_template(h, t, templates[t], n_counters, counters, ""))) return rc;
   if ((rc = upload_templates(h, n_templates, templates, n_counters, counters))) return rc;
   for (int c = 0; c < CCSIM_MAX_PTS; c++) { h->d_stamp[c] = nullptr; h->stamp_len[c] = 0; }
   for (int c = 0; c < templates[0].n_spts; c++)
@@ -660,8 +676,7 @@ extern "C" int ccsim_set_templates(ccsim_handle *h, int32_t n_templates, const c
   for (int j = 0; j < n_counters; j++) {
     const ccsim_counter &c = counters[j];
     DevCounter &d = h->counters[j];
-    d.topo_col = c.topo_col; d.inc = c.inc; d.n_present = c.n_present; d.is_aff = 0; d.smem_off = -1; d.work = nullptr; d.elig_bit = c.elig_bit; d.pad = 0;
-    for (int a = 0; a < templates[0].n_aff; a++) if (templates[0].aff_counter[a] == j) d.is_aff = 1;
+    d = dev_counter(c, templates[0], j);
     if (c.topo_col >= nd.n_topo_cols) return fail(h, CCSIM_EINVAL, "counter %d: topo_col", j);
     h->cnt_range[j] = counter_range(h, c, c.topo_col < 0 ? nullptr : &h->dom_slots[c.topo_col]);
     if (c.topo_col < 0) {
@@ -672,7 +687,6 @@ extern "C" int ccsim_set_templates(ccsim_handle *h, int32_t n_templates, const c
       if ((rc = dev_alloc<int32_t>(h, h->tmpl_allocs, &d.work, (size_t)h->n))) return rc;
     } else {
       if (c.n_domains < 0 || c.n_present < 0 || c.n_present > c.n_domains) return fail(h, CCSIM_EINVAL, "counter %d: domains", j);
-      d.n_domains = c.n_domains;
       if ((rc = dev_upload<int32_t>(h, h->tmpl_allocs, &d.init, c.init, (size_t)c.n_domains))) return rc;
       if (h->smem_cnt_ints + c.n_domains <= SMEM_CNT_MAX_INTS) { d.smem_off = h->smem_cnt_ints; h->smem_cnt_ints += c.n_domains; }
       else if ((rc = dev_alloc<int32_t>(h, h->tmpl_allocs, &d.work, (size_t)grid_max * c.n_domains))) return rc;
@@ -693,27 +707,154 @@ static int each_tree_levels(int32_t n) {
   return L;
 }
 
-extern "C" int ccsim_set_analyses(ccsim_handle *h, int32_t n_templates, const ccsim_template *templates, const ccsim_analysis_terms *terms) {
-  if (!h || !templates || !terms) return fail(h, CCSIM_EINVAL, "null argument");
-  if (!h->have_nodes) return fail(h, CCSIM_ESTATE, "ccsim_load_nodes must come first");
-  if (n_templates < 1 || n_templates > CCSIM_MAX_TEMPLATES) return fail(h, CCSIM_EINVAL, "n_templates out of range");
-  CK(cudaSetDevice(h->cfg.device));
-  free_pool(h, h->tmpl_allocs);
-  h->have_templates = false; h->plan.valid = false; h->each_ran = false; h->analyses = false;
+// Analysis t's device state: its counters and columns, and its tree segments. The segments cover a stable partition of the nodes by
+// normalisation class (TaintToleration's raw count of untolerated PreferNoSchedule taints), then by domain in each column of a term
+// tested per group. Without such terms segment c is class c (possibly empty), and the partition is a counting one.
+static int build_analysis(ccsim_handle *h, int t, const ccsim_template &T, const ccsim_analysis_terms &A, AnalysisState &S) {
   const ccsim_nodes &nd = h->meta;
   const int32_t n = h->n;
-  if (h->cfg.world > 1) return fail(h, CCSIM_EUNSUPPORTED, "per-analysis runs: node-sharded runs (world %d) are not supported", h->cfg.world);
+  const int ncls = h->max_prefer_pop + 1, L = each_tree_levels(n);
   int rc;
+  EachTerms &E = S.terms;
+  memset(&E, 0, sizeof(E));
+  S.n_topo = A.n_topo_cols;
+  // the columns, and whether a column's domains hold one node each
+  bool single[CCSIM_MAX_TOPO_COLS] = {};
+  for (int k = 0; k < A.n_topo_cols; k++) {
+    int32_t *d = nullptr;
+    if ((rc = dev_upload<int32_t>(h, h->tmpl_allocs, &d, A.topo[k], (size_t)n))) return rc;
+    E.topo[k] = d;
+    std::vector<int64_t> &slots = S.dom_slots[k];
+    std::vector<int32_t> members;
+    for (int32_t i = 0; i < n; i++) {
+      const int32_t dd = A.topo[k][i];
+      if (dd < 0) continue;
+      if ((size_t)dd >= slots.size()) { slots.resize((size_t)dd + 1, 0); members.resize((size_t)dd + 1, 0); }
+      slots[dd] += h->node_slots[i];
+      members[dd]++;
+    }
+    single[k] = std::all_of(members.begin(), members.end(), [](int32_t m) { return m <= 1; });
+  }
+  // the counters: their initial counts, one block of working counts, the int32 range of each
+  int32_t total = 0;
+  for (int j = 0; j < A.n_counters; j++) { S.final_off[j] = total; total += A.counters[j].n_domains; }
+  if ((rc = dev_alloc<int32_t>(h, h->tmpl_allocs, &S.work, (size_t)std::max(total, 1)))) return rc;
+  E.n_counters = A.n_counters;
+  for (int j = 0; j < A.n_counters; j++) {
+    const ccsim_counter &c = A.counters[j];
+    DevCounter &d = E.counters[j];
+    d = dev_counter(c, T, j);
+    int32_t *init = nullptr;
+    if ((rc = dev_upload<int32_t>(h, h->tmpl_allocs, &init, c.init, (size_t)c.n_domains))) return rc;
+    d.init = init; d.work = S.work + S.final_off[j];
+    S.range[j] = counter_range(h, c, c.topo_col < 0 ? nullptr : &S.dom_slots[c.topo_col]);
+  }
+  // the terms: folded into the leaf when their domains hold one node each, else tested per domain group
+  const uint32_t fe = T.filter_enable;
+  bool group_col[CCSIM_MAX_TOPO_COLS] = {};
+  auto place = [&](int counter, uint32_t bit) {
+    const int32_t col = A.counters[counter].topo_col;
+    if (col < 0 || single[col]) E.leaf_sel |= bit;
+    else { E.group_sel |= bit; group_col[col] = true; }
+  };
+  if (fe & CCSIM_PL_POD_TOPOLOGY_SPREAD) for (int c = 0; c < T.n_pts; c++) place(T.pts[c].counter, 1u << c);
+  if (fe & CCSIM_PL_INTER_POD_AFFINITY) {
+    for (int a = 0; a < T.n_aff; a++) place(T.aff_counter[a], COUPLED_AFF_SEL(a));
+    for (int a = 0; a < T.n_anti; a++) place(T.anti_counter[a], COUPLED_ANTI_SEL(a));
+  }
+  std::vector<int32_t> cls((size_t)n, 0);
+  if (T.score_enable & CCSIM_PL_TAINT_TOLERATION)
+    for (int32_t i = 0; i < n; i++)
+      for (int w = 0; w < nd.taint_words; w++) cls[i] += __builtin_popcountll(h->h_taint[(size_t)w * n + i] & nd.taint_prefer[w] & ~T.tol_prefer[w]);
+  std::vector<int32_t> pos((size_t)n), rep, seg_cls;
+  std::vector<long long> start;
+  if (!E.group_sel) {   // segment c = class c (possibly empty), as many as the cluster has classes
+    std::vector<long long> at((size_t)ncls + 1, 0);
+    for (int32_t i = 0; i < n; i++) at[cls[i] + 1]++;
+    for (int c = 0; c < ncls; c++) { at[c + 1] += at[c]; start.push_back(at[c]); rep.push_back(0); seg_cls.push_back(c); }
+    for (int32_t i = 0; i < n; i++) pos[i] = (int32_t)at[cls[i]]++;
+  } else {              // one group per (class, domain in each group column)
+    std::vector<int32_t> gcols;
+    for (int k = 0; k < A.n_topo_cols; k++) if (group_col[k]) gcols.push_back(k);
+    const size_t kw = 1 + gcols.size();
+    std::vector<int32_t> key((size_t)n * kw);
+    for (int32_t i = 0; i < n; i++) {
+      key[(size_t)i * kw] = cls[i];
+      for (size_t q = 0; q < gcols.size(); q++) key[(size_t)i * kw + 1 + q] = A.topo[gcols[q]][i];
+    }
+    std::vector<int32_t> order((size_t)n);
+    for (int32_t i = 0; i < n; i++) order[i] = i;
+    auto less = [&](int32_t x, int32_t y) {
+      return std::lexicographical_compare(&key[(size_t)x * kw], &key[(size_t)x * kw + kw], &key[(size_t)y * kw], &key[(size_t)y * kw + kw]);
+    };
+    std::stable_sort(order.begin(), order.end(), less);
+    for (int32_t r = 0; r < n; r++) {
+      const int32_t i = order[r];
+      pos[i] = r;
+      if (r == 0 || less(order[r - 1], i)) { start.push_back(r); rep.push_back(i); seg_cls.push_back(cls[i]); }
+    }
+  }
+  const int32_t G = (int32_t)start.size();
+  if (G > CCSIM_EACH_MAX_GROUPS)
+    return fail(h, CCSIM_EUNSUPPORTED, "per-analysis runs: analysis %d has %d domain groups (max %d)", t, G, CCSIM_EACH_MAX_GROUPS);
+  std::vector<long long> cof((size_t)(L + 1) * (G + 1));
+  for (int g = 0; g < G; g++) cof[g] = start[g];
+  cof[G] = n;
+  for (int l = 1; l <= L; l++) {
+    long long acc = 0;
+    for (int g = 0; g < G; g++) {
+      const long long sz = cof[(size_t)(l - 1) * (G + 1) + g + 1] - cof[(size_t)(l - 1) * (G + 1) + g];
+      cof[(size_t)l * (G + 1) + g] = acc; acc += (sz + 31) >> 5;
+    }
+    cof[(size_t)l * (G + 1) + G] = acc;
+  }
+  E.n_seg = G;
+  E.port_self = h->w_placed && (T.filter_enable & CCSIM_PL_NODE_PORTS) && (T.flags & CCSIM_TF_HAS_HOST_PORTS) && ((T.port_tmpl_conflict >> t) & 1ull);
+  bool identity = true;   // then the kernel reads a node's position as its index
+  for (int32_t i = 0; i < n && identity; i++) identity = pos[i] == i;
+  long long *d_cof = nullptr; int32_t *d_rep = nullptr, *d_cls = nullptr, *d_pos = nullptr;
+  if ((rc = dev_upload<long long>(h, h->tmpl_allocs, &d_cof, cof.data(), cof.size())) ||
+      (rc = dev_upload<int32_t>(h, h->tmpl_allocs, &d_rep, rep.data(), rep.size())) ||
+      (rc = dev_upload<int32_t>(h, h->tmpl_allocs, &d_cls, seg_cls.data(), seg_cls.size())) ||
+      (!identity && (rc = dev_upload<int32_t>(h, h->tmpl_allocs, &d_pos, pos.data(), pos.size()))))
+    return rc;
+  E.cof = d_cof; E.seg_rep = d_rep; E.seg_cls = d_cls; E.pos = d_pos;
+  CK(cudaStreamSynchronize(h->stream));   // the host vectors go out of scope
+  return CCSIM_OK;
+}
+
+// Every analysis's state (terms: nullptr, the node-local templates of ccsim_set_templates), and its device copy d_terms
+static int build_analyses(ccsim_handle *h, const ccsim_analysis_terms *terms) {
+  const ccsim_analysis_terms none = {};
+  std::vector<AnalysisState> an((size_t)h->n_templates);
+  std::vector<EachTerms> dev_terms;
+  int rc;
+  for (int t = 0; t < h->n_templates; t++) {
+    if ((rc = build_analysis(h, t, h->h_templates[t], terms ? terms[t] : none, an[t]))) return rc;
+    dev_terms.push_back(an[t].terms);
+  }
+  if ((rc = dev_upload<EachTerms>(h, h->tmpl_allocs, &h->d_terms, dev_terms.data(), dev_terms.size()))) return rc;
+  CK(cudaStreamSynchronize(h->stream));   // dev_terms goes out of scope
+  h->an.swap(an);
+  return CCSIM_OK;
+}
+
+extern "C" int ccsim_set_analyses(ccsim_handle *h, int32_t n_templates, const ccsim_template *templates, const ccsim_analysis_terms *terms) {
+  if (!h || !templates || !terms) return fail(h, CCSIM_EINVAL, "null argument");
+  int rc;
+  if ((rc = begin_templates(h, n_templates))) return rc;
+  const int32_t n = h->n;
+  if (h->cfg.world > 1) return fail(h, CCSIM_EUNSUPPORTED, "per-analysis runs: node-sharded runs (world %d) are not supported", h->cfg.world);
   for (int t = 0; t < n_templates; t++) {   // every analysis validated as ccsim_set_templates validates its template alone
     const ccsim_analysis_terms &A = terms[t];
     if (A.n_counters < 0 || A.n_counters > CCSIM_MAX_COUNTERS || (A.n_counters && !A.counters))
       return fail(h, CCSIM_EINVAL, "analysis %d: n_counters out of range", t);
     if (A.n_topo_cols < 0 || A.n_topo_cols > CCSIM_MAX_TOPO_COLS) return fail(h, CCSIM_EINVAL, "analysis %d: n_topo_cols out of range", t);
     for (int k = 0; k < A.n_topo_cols; k++) if (!A.topo[k] && n > 0) return fail(h, CCSIM_EINVAL, "analysis %d: null topo column %d", t, k);
-    if ((rc = check_template(h, t, templates[t], A.n_counters, A.counters))) return rc;
+    char who[32]; snprintf(who, sizeof(who), "analysis %d: ", t);
+    if ((rc = check_template(h, t, templates[t], A.n_counters, A.counters, who))) return rc;
     for (int j = 0; j < A.n_counters; j++) {
       const ccsim_counter &c = A.counters[j];
-      if (c.elig_bit >= 64 * nd.static_words) return fail(h, CCSIM_EINVAL, "analysis %d: counter %d: elig_bit", t, j);
       if (c.topo_col >= A.n_topo_cols) return fail(h, CCSIM_EINVAL, "analysis %d: counter %d: topo_col", t, j);
       if (c.topo_col < 0 ? c.n_domains != n : (c.n_domains < 0 || c.n_present < 0 || c.n_present > c.n_domains))
         return fail(h, CCSIM_EINVAL, "analysis %d: counter %d: domains", t, j);
@@ -723,125 +864,9 @@ extern "C" int ccsim_set_analyses(ccsim_handle *h, int32_t n_templates, const cc
           if (A.topo[c.topo_col][i] >= c.n_domains) return fail(h, CCSIM_EINVAL, "analysis %d: counter %d: node %d's domain out of range", t, j, i);
     }
   }
-  for (int t = 0; t < n_templates; t++) if ((rc = check_weights(h, t, templates[t]))) return rc;
-  if (h->max_prefer_pop + 1 > CCSIM_MAX_CLASSES)
-    return fail(h, CCSIM_EUNSUPPORTED, "a node carries %d PreferNoSchedule taints (max %d)", h->max_prefer_pop, CCSIM_MAX_CLASSES - 1);
   if ((rc = upload_templates(h, n_templates, templates, 0, nullptr))) return rc;
-  const int ncls = h->max_prefer_pop + 1, L = each_tree_levels(n);
-  h->an.assign((size_t)n_templates, AnalysisState());
-  std::vector<EachTerms> dev_terms((size_t)n_templates);
-  h->max_seg = ncls;
-  for (int t = 0; t < n_templates; t++) {
-    const ccsim_template &T = templates[t];
-    const ccsim_analysis_terms &A = terms[t];
-    AnalysisState &S = h->an[t];
-    EachTerms &E = S.terms;
-    memset(&E, 0, sizeof(E));
-    S.n_topo = A.n_topo_cols;
-    // the columns, and whether a column's domains hold one node each
-    bool single[CCSIM_MAX_TOPO_COLS] = {};
-    for (int k = 0; k < A.n_topo_cols; k++) {
-      int32_t *d = nullptr;
-      if ((rc = dev_upload<int32_t>(h, h->tmpl_allocs, &d, A.topo[k], (size_t)n))) return rc;
-      E.topo[k] = d;
-      std::vector<int64_t> &slots = S.dom_slots[k];
-      std::vector<int32_t> members;
-      for (int32_t i = 0; i < n; i++) {
-        const int32_t dd = A.topo[k][i];
-        if (dd < 0) continue;
-        if ((size_t)dd >= slots.size()) { slots.resize((size_t)dd + 1, 0); members.resize((size_t)dd + 1, 0); }
-        slots[dd] += h->node_slots[i];
-        members[dd]++;
-      }
-      single[k] = std::all_of(members.begin(), members.end(), [](int32_t m) { return m <= 1; });
-    }
-    // the counters: their initial counts, one block of working counts, the int32 range of each
-    int32_t total = 0;
-    for (int j = 0; j < A.n_counters; j++) { S.final_off[j] = total; total += A.counters[j].n_domains; }
-    if ((rc = dev_alloc<int32_t>(h, h->tmpl_allocs, &S.work, (size_t)std::max(total, 1)))) return rc;
-    E.n_counters = A.n_counters;
-    for (int j = 0; j < A.n_counters; j++) {
-      const ccsim_counter &c = A.counters[j];
-      DevCounter &d = E.counters[j];
-      d.topo_col = c.topo_col; d.n_domains = c.n_domains; d.n_present = c.n_present; d.inc = c.inc; d.smem_off = -1; d.elig_bit = c.elig_bit;
-      for (int a = 0; a < T.n_aff; a++) if (T.aff_counter[a] == j) d.is_aff = 1;
-      int32_t *init = nullptr;
-      if ((rc = dev_upload<int32_t>(h, h->tmpl_allocs, &init, c.init, (size_t)c.n_domains))) return rc;
-      d.init = init; d.work = S.work + S.final_off[j];
-      S.range[j] = counter_range(h, c, c.topo_col < 0 ? nullptr : &S.dom_slots[c.topo_col]);
-    }
-    // the terms: folded into the leaf when their domains hold one node each, else tested per domain group
-    const uint32_t fe = T.filter_enable;
-    bool group_col[CCSIM_MAX_TOPO_COLS] = {};
-    auto place = [&](int counter, uint32_t bit) {
-      const int32_t col = A.counters[counter].topo_col;
-      if (col < 0 || single[col]) E.leaf_sel |= bit;
-      else { E.group_sel |= bit; group_col[col] = true; }
-    };
-    if (fe & CCSIM_PL_POD_TOPOLOGY_SPREAD) for (int c = 0; c < T.n_pts; c++) place(T.pts[c].counter, 1u << c);
-    if (fe & CCSIM_PL_INTER_POD_AFFINITY) {
-      for (int a = 0; a < T.n_aff; a++) place(T.aff_counter[a], COUPLED_AFF_SEL(a));
-      for (int a = 0; a < T.n_anti; a++) place(T.anti_counter[a], COUPLED_ANTI_SEL(a));
-    }
-    // domain groups: (class, domain in each group column), a stable partition of the nodes; without group terms one group per class
-    std::vector<int32_t> gcols;
-    for (int k = 0; k < A.n_topo_cols; k++) if (group_col[k]) gcols.push_back(k);
-    const size_t kw = 1 + gcols.size();
-    std::vector<int32_t> key((size_t)n * kw);
-    for (int32_t i = 0; i < n; i++) {
-      int cls = 0;
-      if (T.score_enable & CCSIM_PL_TAINT_TOLERATION)
-        for (int w = 0; w < nd.taint_words; w++) cls += __builtin_popcountll(h->h_taint[(size_t)w * n + i] & nd.taint_prefer[w] & ~T.tol_prefer[w]);
-      key[(size_t)i * kw] = cls;
-      for (size_t q = 0; q < gcols.size(); q++) key[(size_t)i * kw + 1 + q] = A.topo[gcols[q]][i];
-    }
-    std::vector<int32_t> order((size_t)n);
-    for (int32_t i = 0; i < n; i++) order[i] = i;
-    auto less = [&](int32_t x, int32_t y) {
-      return std::lexicographical_compare(&key[(size_t)x * kw], &key[(size_t)x * kw + kw], &key[(size_t)y * kw], &key[(size_t)y * kw + kw]);
-    };
-    std::stable_sort(order.begin(), order.end(), less);
-    std::vector<int32_t> pos((size_t)n), rep, cls;
-    std::vector<long long> start;
-    for (int32_t r = 0; r < n; r++) {
-      const int32_t i = order[r];
-      pos[i] = r;
-      if (E.group_sel && (r == 0 || less(order[r - 1], i))) { start.push_back(r); rep.push_back(i); cls.push_back(key[(size_t)i * kw]); }
-    }
-    if (!E.group_sel)   // segment c = class c (possibly empty), as the class trees of node-local templates
-      for (int c = 0; c < ncls; c++) {
-        start.push_back(std::lower_bound(order.begin(), order.end(), c, [&](int32_t x, int v) { return key[(size_t)x * kw] < v; }) - order.begin());
-        rep.push_back(0); cls.push_back(c);
-      }
-    const int32_t G = (int32_t)start.size();
-    if (G > CCSIM_EACH_MAX_GROUPS)
-      return fail(h, CCSIM_EUNSUPPORTED, "per-analysis runs: analysis %d has %d domain groups (max %d)", t, G, CCSIM_EACH_MAX_GROUPS);
-    std::vector<long long> cof((size_t)(L + 1) * (G + 1));
-    for (int g = 0; g < G; g++) cof[g] = start[g];
-    cof[G] = n;
-    for (int l = 1; l <= L; l++) {
-      long long acc = 0;
-      for (int g = 0; g < G; g++) {
-        const long long sz = cof[(size_t)(l - 1) * (G + 1) + g + 1] - cof[(size_t)(l - 1) * (G + 1) + g];
-        cof[(size_t)l * (G + 1) + g] = acc; acc += (sz + 31) >> 5;
-      }
-      cof[(size_t)l * (G + 1) + G] = acc;
-    }
-    E.n_seg = G;
-    h->max_seg = std::max(h->max_seg, G);
-    long long *d_cof = nullptr; int32_t *d_rep = nullptr, *d_cls = nullptr, *d_pos = nullptr;
-    if ((rc = dev_upload<long long>(h, h->tmpl_allocs, &d_cof, cof.data(), cof.size())) ||
-        (rc = dev_upload<int32_t>(h, h->tmpl_allocs, &d_rep, rep.data(), rep.size())) ||
-        (rc = dev_upload<int32_t>(h, h->tmpl_allocs, &d_cls, cls.data(), cls.size())) ||
-        (rc = dev_upload<int32_t>(h, h->tmpl_allocs, &d_pos, pos.data(), pos.size())))
-      return rc;
-    E.cof = d_cof; E.seg_rep = d_rep; E.seg_cls = d_cls; E.pos = d_pos;
-    CK(cudaStreamSynchronize(h->stream));   // the host vectors go out of scope
-    dev_terms[t] = E;
-  }
-  if ((rc = dev_upload<EachTerms>(h, h->tmpl_allocs, &h->d_terms, dev_terms.data(), (size_t)n_templates))) return rc;
-  CK(cudaStreamSynchronize(h->stream));
   h->n_templates = n_templates; h->n_counters = 0; h->final_total = 0;
+  if ((rc = build_analyses(h, terms))) return rc;
   h->analyses = true;
   h->have_templates = true;
   return CCSIM_OK;
@@ -869,16 +894,22 @@ static int check_counter_bounds(ccsim_handle *h, int64_t max_pods, bool fit_off,
   return CCSIM_OK;
 }
 
-// The refusals a run meets before it touches anything: a run that nothing bounds, and counters that could leave int32. `cap`: the
-// output capacity, since no run can place more than sum(max(0, alloc_pods - npods)) pods (fit.go:567-576), or max_pods.
-static int check_run_bounds(ccsim_handle *h, int64_t max_pods, int64_t &cap) {
-  const bool fit_off = h->tf.fit_off;
-  // ("Too many pods" bounds a run only while NodeResourcesFit filters: with the plugin disabled through --default-config an
-  //  unlimited run never ends in the reference either)
-  if (max_pods <= 0 && fit_off)
-    return fail(h, CCSIM_EUNSUPPORTED, "NodeResourcesFit is disabled for a template: the run is unbounded, --max-limit is required");
+// The output capacity of a run, since no run can place more than sum(max(0, alloc_pods - npods)) pods (fit.go:567-576), or
+// max_pods. False: nothing bounds the run ("Too many pods" bounds a run only while NodeResourcesFit filters: with the plugin disabled
+// through --default-config an unlimited run never ends in the reference either)
+static bool run_cap(const ccsim_handle *h, int64_t max_pods, bool fit_off, int64_t &cap) {
+  if (max_pods <= 0 && fit_off) return false;
   cap = h->pod_bound + 1;
   if (max_pods > 0 && (max_pods < cap || fit_off)) cap = max_pods;
+  return true;
+}
+
+// The refusals a run meets before it touches anything: a run that nothing bounds, and counters that could leave int32. `cap`: the
+// output capacity (run_cap)
+static int check_run_bounds(ccsim_handle *h, int64_t max_pods, int64_t &cap) {
+  const bool fit_off = h->tf.fit_off;
+  if (!run_cap(h, max_pods, fit_off, cap))
+    return fail(h, CCSIM_EUNSUPPORTED, "NodeResourcesFit is disabled for a template: the run is unbounded, --max-limit is required");
   return check_counter_bounds(h, max_pods, fit_off, h->n_counters, h->counters, h->cnt_range, h->dom_slots, "");
 }
 
@@ -1247,26 +1278,26 @@ extern "C" int ccsim_run_each(ccsim_handle *h, int64_t max_pods, ccsim_result *o
         (P.n_ipa_score > 0 && (P.score_enable & CCSIM_PL_INTER_POD_AFFINITY)))
       return fail(h, CCSIM_EUNSUPPORTED, "per-analysis runs: template %d has a normalised soft scorer (preferred nodeAffinity, ScheduleAnyway spreading, pod-affinity scoring)", t);
   }
+  CK(cudaSetDevice(h->cfg.device));
+  int rc;
+  if (h->an.empty() && (rc = build_analyses(h, nullptr))) return rc;   // ccsim_set_templates: node-local analyses, no terms
   // every analysis is bounded like a run of its template alone (check_run_bounds); the sequences hold the largest bound
   int64_t cap = 1;
+  int nseg = 1;          // most tree segments of an analysis
+  bool terms = false;    // some analysis has counters or a hostPort self-conflict
   for (int t = 0; t < T; t++) {
+    const AnalysisState &S = h->an[t];
     const bool fit_off = !(h->h_templates[t].filter_enable & CCSIM_PL_FIT);
-    if (max_pods <= 0 && fit_off)
+    int64_t c = 0;
+    if (!run_cap(h, max_pods, fit_off, c))
       return fail(h, CCSIM_EUNSUPPORTED, "template %d: NodeResourcesFit is disabled: the run is unbounded, --max-limit is required", t);
-    int64_t c = h->pod_bound + 1;
-    if (max_pods > 0 && (max_pods < c || fit_off)) c = max_pods;
     cap = std::max(cap, c);
-    if (h->analyses) {
-      const AnalysisState &S = h->an[t];
-      char who[32]; snprintf(who, sizeof(who), "analysis %d: ", t);
-      int rc = check_counter_bounds(h, max_pods, fit_off, S.terms.n_counters, S.terms.counters, S.range, S.dom_slots, who);
-      if (rc) return rc;
-    }
+    char who[32]; snprintf(who, sizeof(who), "analysis %d: ", t);
+    if ((rc = check_counter_bounds(h, max_pods, fit_off, S.terms.n_counters, S.terms.counters, S.range, S.dom_slots, who))) return rc;
+    nseg = std::max(nseg, S.terms.n_seg);
+    terms |= S.terms.n_counters > 0 || S.terms.port_self;
   }
-  CK(cudaSetDevice(h->cfg.device));
   const int32_t n = h->n;
-  const int ncls = h->max_prefer_pop + 1;
-  const int nseg = h->analyses ? h->max_seg : ncls;   // tree segments per analysis: classes, or domain groups
   {
     size_t free_b = 0, total_b = 0;
     CK(cudaMemGetInfo(&free_b, &total_b));
@@ -1281,7 +1312,7 @@ extern "C" int ccsim_run_each(ccsim_handle *h, int64_t max_pods, ccsim_result *o
   // tree shape: roots on level L (32^L >= N); levels [1, split) in global memory, [split, L] in shared memory, the lowest split whose
   // shared levels fit next to the kernel's static structs
   const int L = each_tree_levels(n);
-  const WaveKernel &kern = WAVE_KERNELS[h->analyses ? WK_EACH_TERMS : WK_EACH];
+  const WaveKernel &kern = WAVE_KERNELS[terms ? WK_EACH_TERMS : WK_EACH];
   int split = 1;
   size_t smem = 0;
   for (; split <= L + 1; split++) {
@@ -1300,16 +1331,14 @@ extern "C" int ccsim_run_each(ccsim_handle *h, int64_t max_pods, ccsim_result *o
     ep.glev_stride = g;
   }
   free_pool(h, h->each_allocs);
-  int rc;
   const size_t tn = (size_t)T * (size_t)n;
   if ((rc = dev_alloc<int32_t>(h, h->each_allocs, &ep.k, tn)) || (rc = dev_alloc<unsigned long long>(h, h->each_allocs, &ep.leaf, tn)) ||
       (rc = dev_alloc<unsigned long long>(h, h->each_allocs, &ep.glev, (size_t)T * ep.glev_stride)) ||
       (rc = dev_alloc<int32_t>(h, h->each_allocs, &ep.seq, (size_t)T * cap)) || (rc = dev_alloc<EachOut>(h, h->each_allocs, &ep.out, (size_t)T)))
     return rc;
-  if (!h->analyses && ncls > 1 && (rc = dev_alloc<int32_t>(h, h->each_allocs, &ep.pos, tn))) return rc;
   DevOut *d_diag = nullptr;
   if ((rc = dev_alloc<DevOut>(h, h->each_allocs, &d_diag, (size_t)T))) return rc;
-  ep.terms = h->analyses ? h->d_terms : nullptr;
+  ep.terms = h->d_terms;
   ep.diag = d_diag;
   ep.s_req_cpu = h->s_req_cpu; ep.s_req_mem = h->s_req_mem; ep.s_req_eph = h->s_req_eph; ep.s_nz_cpu = h->s_nz_cpu; ep.s_nz_mem = h->s_nz_mem;
   ep.s_npods = h->s_npods;
@@ -1338,14 +1367,12 @@ extern "C" int ccsim_run_each(ccsim_handle *h, int64_t max_pods, ccsim_result *o
       if (eo[t].stop_code != CCSIM_STOP_UNSCHEDULABLE) continue;
       const int blocks = std::min(4 * h->sm_count, (n + 255) / 256);
       ccsim_each_scatter_kernel<<<blocks, 256, 0, s>>>(p, ep, t);
-      DevParams pd = p;
-      if (h->analyses) {   // the analysis's own counters (where the run left them) and columns
-        const AnalysisState &S = h->an[t];
-        pd.n_counters = S.terms.n_counters; pd.n_topo = S.n_topo;
-        for (int j = 0; j < S.terms.n_counters; j++) { pd.counters[j] = S.terms.counters[j]; pd.final_off[j] = S.final_off[j]; }
-        pd.final_cnt = S.work;
-        for (int k = 0; k < CCSIM_MAX_TOPO_COLS; k++) pd.topo[k] = S.terms.topo[k];
-      }
+      DevParams pd = p;   // the analysis's own counters (where the run left them) and columns
+      const AnalysisState &S = h->an[t];
+      pd.n_counters = S.terms.n_counters; pd.n_topo = S.n_topo;
+      for (int j = 0; j < S.terms.n_counters; j++) { pd.counters[j] = S.terms.counters[j]; pd.final_off[j] = S.final_off[j]; }
+      pd.final_cnt = S.work;
+      for (int k = 0; k < CCSIM_MAX_TOPO_COLS; k++) pd.topo[k] = S.terms.topo[k];
       pd.out = d_diag + t;
       ccsim_diag_kernel<<<blocks, 256, 0, s>>>(pd, t);
       h->launches += 2;

@@ -67,6 +67,20 @@ def check(snap, tmpl, limit, with_oracle=True):
     return got, st
 
 
+def check_analyses_path(snap, tmpl, limit, got, st):
+    """the same templates loaded through ccsim_set_analyses with empty terms: every result, the node counts and the tree's shape
+    and shared memory equal the ccsim_set_templates run's"""
+    _, _, counts = run_each(snap, tmpl, limit)
+    with engine.Engine(device=0) as eng:
+        eng.load_nodes(snap)
+        eng.set_analyses(tmpl, [([], [])] * len(tmpl))
+        again, ast, acounts = run_each(snap, tmpl, limit, eng)
+    for t in range(len(tmpl)):
+        same(again[t], got[t], "analysis %d through ccsim_set_analyses" % t)
+        assert np.array_equal(acounts[t][0], counts[t][0]) and np.array_equal(acounts[t][1], counts[t][1]), t
+    assert [ast[k] for k in ("global_levels", "shared_levels", "smem_bytes")] == [st[k] for k in ("global_levels", "shared_levels", "smem_bytes")]
+
+
 def nodes_c2(n, seed=1, **over):
     rng = np.random.Generator(np.random.PCG64(seed))
     cores = rng.choice([4, 8, 16, 32], size=n)
@@ -176,8 +190,9 @@ def test_each_prefer_no_schedule_classes(built, taint_words):
     tol.tol_prefer[taint_words - 1] = 0b110                      # tolerates two of the seven
     noscore = abi.default_template(700, 256 * MiB)
     noscore.score_enable &= ~abi.PL_TAINT_TOLERATION
-    got, _ = check(snap, [plain, tol, noscore], 0)
+    got, st = check(snap, [plain, tol, noscore], 0)
     assert all(g.stop_code == abi.STOP_UNSCHEDULABLE for g in got)
+    check_analyses_path(snap, [plain, tol, noscore], 0, got, st)
 
 
 @pytest.mark.parametrize("n", [1, 31, 32, 33, 1023, 1024, 1025, 32769])
@@ -193,6 +208,7 @@ def test_each_tree_edges(built, n):
     limit = 0 if n <= 1025 else 1500
     got, st = check(snap, tm, limit)
     assert st["global_levels"] + st["shared_levels"] == (0 if n == 1 else int(np.ceil(np.log(n) / np.log(32) - 1e-12)))
+    check_analyses_path(snap, tm, limit, got, st)
     if n > 2:
         assert max(np.bincount(g.pod_node, minlength=n)[n // 2] for g in got) >= 100
 
