@@ -42,7 +42,8 @@ struct DevOut {
   unsigned long long n_diag;
   long long phase_cycles[8];       // CTA 0's cycles per phase (multi-commit kernel: always; other kernels: CCSIM_PHASE_TIMERS builds)
   long long stat[4];               // multi-commit kernel: [0] candidates replayed (sum over waves), [1] waves that had to raise the bar T,
-                                   // [2] replay rounds, [3] waves replayed in key order
+                                   // [2] replay rounds, [3] waves replayed in key order (low 32 bits) and waves that selected each
+                                   // tile's candidates from the sorted tile (high 32 bits)
 };
 
 // DevParams::debug_flags, set from CCSIM_DEBUG_FLAGS (kernel experiments; INTEGRATION.md lists the same values)
@@ -53,6 +54,7 @@ constexpr uint32_t DBG_CYCLES = 8u;               // replay / per-CTA cycle summ
 constexpr uint32_t DBG_STRICT_ONLY = 16u;         // strict multi-commit waves only (no look-ahead)
 constexpr uint32_t DBG_LOOKAHEAD_ALWAYS = 32u;    // look-ahead on every spread term in every wave
 constexpr uint32_t DBG_ARGMAX_ROUND = 64u;        // single-use multi-commit waves keep the arg-max replay round instead of key order
+constexpr uint32_t DBG_REDUX_SELECT = 128u;       // single-use multi-commit waves select each tile's candidates by REDUX rounds and a merge
 
 struct DevParams {
   int32_t n;            // nodes of this shard

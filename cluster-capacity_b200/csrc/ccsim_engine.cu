@@ -188,15 +188,19 @@ static const WaveKernel WAVE_KERNELS[] = {
   {(const void *)ccsim_wave_lean_kernel<false>, "lean<false>", ENG_LEAN, LEAN_THREADS, sizeof(LeanShared), 0},
   {(const void *)ccsim_wave_lean_kernel<true>, "lean<true>", ENG_LEAN, LEAN_THREADS, sizeof(LeanShared), 0},
   {(const void *)ccsim_wave_batched_kernel, "batched", ENG_TIE_RUN, LEAN_THREADS, sizeof(LeanShared) + sizeof(BatchShared), 0},
-  {(const void *)ccsim_wave_multi_kernel<false>, "multi<false>", ENG_MULTI, LEAN_THREADS, sizeof(LeanShared) + sizeof(MultiShared), 0},
-  {(const void *)ccsim_wave_multi_kernel<true>, "multi<true>", ENG_MULTI, LEAN_THREADS, sizeof(LeanShared) + sizeof(MultiShared), 0},
+  {(const void *)ccsim_wave_multi_kernel<false, false>, "multi<false>", ENG_MULTI, LEAN_THREADS, sizeof(LeanShared) + sizeof(MultiShared), 0},
+  {(const void *)ccsim_wave_multi_kernel<true, false>, "multi<true>", ENG_MULTI, LEAN_THREADS, sizeof(LeanShared) + sizeof(MultiShared), 0},
+  // (the same kernels with the selection from the sorted tile: named alike, ccsim_sorted_tile_waves tells them apart)
+  {(const void *)ccsim_wave_multi_kernel<false, true>, "multi<false>", ENG_MULTI, LEAN_THREADS, sizeof(LeanShared) + sizeof(MultiShared) + MULTI_SORTED_SMEM, 0},
+  {(const void *)ccsim_wave_multi_kernel<true, true>, "multi<true>", ENG_MULTI, LEAN_THREADS, sizeof(LeanShared) + sizeof(MultiShared) + MULTI_SORTED_SMEM, 0},
   {(const void *)ccsim_wave_stream_kernel<0>, "stream<0>", ENG_STREAM, STREAM_BLOCK, sizeof(StreamShared), stream_smem_bytes(0, 0)},
   {(const void *)ccsim_wave_stream_kernel<1>, "stream<1>", ENG_STREAM, STREAM_BLOCK, sizeof(StreamShared), stream_smem_bytes(1, 0)},
   {(const void *)ccsim_wave_stream_kernel<2>, "stream<2>", ENG_STREAM, STREAM_BLOCK, sizeof(StreamShared), 0},
   {(const void *)ccsim_each_kernel<false>, "each", ENG_EACH, EACH_THREADS, sizeof(EachShared), 0},   // ccsim_run_each: node-local analyses
   {(const void *)ccsim_each_kernel<true>, "each", ENG_EACH, EACH_THREADS, sizeof(EachShared), 0},    // ... some with counters or hostPorts
 };
-enum { WK_WAVE, WK_WAVE_STREAMED, WK_LEAN, WK_LEAN_SAMPLING, WK_BATCHED, WK_MULTI, WK_MULTI_SHARDED, WK_STREAM /* + mode */,
+enum { WK_WAVE, WK_WAVE_STREAMED, WK_LEAN, WK_LEAN_SAMPLING, WK_BATCHED, WK_MULTI, WK_MULTI_SHARDED, WK_MULTI_SORTED, WK_MULTI_SHARDED_SORTED,
+       WK_STREAM /* + mode */,
        WK_EACH = WK_STREAM + 3, WK_EACH_TERMS };
 static_assert(sizeof(WAVE_KERNELS) / sizeof(WAVE_KERNELS[0]) == WK_EACH_TERMS + 1, "one WAVE_KERNELS entry per WK_* index");
 
@@ -289,6 +293,7 @@ struct ccsim_handle {
   uint32_t xwave0 = 0;                                    // exchanges of earlier sharded runs (buffer parity continues across runs)
   int64_t last_stat[16] = {};                             // ccsim_run_stats
   int64_t last_key_order_waves = 0;                       // ccsim_key_order_waves
+  int64_t last_sorted_tile_waves = 0;                     // ccsim_sorted_tile_waves
   RunPlan plan;
   int32_t *d_topo_full[CCSIM_MAX_TOPO_COLS] = {};
   int32_t *d_pod_node = nullptr; int64_t pod_cap = 0;
@@ -1060,7 +1065,22 @@ static void plan_multi(const ccsim_handle *h, RunPlan &pl, const WaveKernel *&k)
   }
   // + the per-node payload column, and 16 bytes that nothing reads: kept so that the kernel's shared-memory size, which
   //   run_stats() reports, stays what it has been
-  take_if_fits(h, pl, k, WAVE_KERNELS[h->cfg.world > 1 ? WK_MULTI_SHARDED : WK_MULTI], lean_smem_bytes(lp, p.chunk_pad, 8) + 16);
+  const size_t dyn = lean_smem_bytes(lp, p.chunk_pad, 8) + 16;
+  // Single-use template (a self-matching required anti-affinity on a node-local counter: a node takes one clone, so no winner comes
+  // back in its wave): each tile's candidates come from the tile sorted by key, in the instantiation that has that selection and
+  // its rank array — unless CCSIM_DEBUG_FLAGS bit 7 asks for the REDUX selection, or the rank array does not fit next to the tile.
+  // The kernel checks the same condition itself (ccsim_multi.cuh: ms.single_use) and runs the REDUX selection when it fails.
+  bool single_use = false;
+  if (T.filter_enable & CCSIM_PL_INTER_POD_AFFINITY)
+    for (int a = 0; a < T.n_anti; a++) {
+      const DevCounter &dc = h->counters[T.anti_counter[a]];
+      single_use |= dc.topo_col < 0 && dc.inc > 0 && !(dc.is_aff && !(T.flags & CCSIM_TF_AFF_SELF_MATCH_ALL));
+    }
+  const bool sharded = h->cfg.world > 1;
+  if (single_use && !(p.debug_flags & DBG_REDUX_SELECT) &&
+      take_if_fits(h, pl, k, WAVE_KERNELS[sharded ? WK_MULTI_SHARDED_SORTED : WK_MULTI_SORTED], dyn))
+    return;
+  take_if_fits(h, pl, k, WAVE_KERNELS[sharded ? WK_MULTI_SHARDED : WK_MULTI], dyn);
 }
 
 // Streaming waves (ccsim_stream.cuh: TMA-staged tiles, per-template score memo) when the lean tile is not taken; fills its padded columns
@@ -1233,7 +1253,8 @@ extern "C" int ccsim_run(ccsim_handle *h, int64_t max_pods, ccsim_result *out) {
   h->last_stat[0] = k.engine; h->last_stat[1] = ho.waves; h->last_stat[2] = ho.placed;
   h->last_stat[3] = ho.stat[0]; h->last_stat[4] = ho.stat[1]; h->last_stat[5] = grid; h->last_stat[6] = k.block; h->last_stat[7] = (int64_t)smem;
   for (int q = 0; q < 8; q++) h->last_stat[8 + q] = ho.phase_cycles[q];
-  h->last_key_order_waves = k.engine == ENG_MULTI ? ho.stat[3] : 0;
+  h->last_key_order_waves = k.engine == ENG_MULTI ? (ho.stat[3] & 0xffffffffll) : 0;
+  h->last_sorted_tile_waves = k.engine == ENG_MULTI ? (int64_t)((unsigned long long)ho.stat[3] >> 32) : 0;
   out->placed = ho.placed; out->stop_code = ho.stop_code; out->waves = ho.waves; out->evals = ho.evals; out->run_ms = ms;
   out->examined = ho.examined ? ho.examined : ho.evals;
   h->last_placed = ho.placed;
@@ -1415,6 +1436,7 @@ extern "C" int ccsim_run_each(ccsim_handle *h, int64_t max_pods, ccsim_result *o
   h->last_stat[5] = T; h->last_stat[6] = kern.block; h->last_stat[7] = (int64_t)smem;
   h->last_stat[8] = rebuilds;                                                                 // leaf and level rebuilds, all analyses
   h->last_key_order_waves = 0;
+  h->last_sorted_tile_waves = 0;
   h->each_ran = true;
   return CCSIM_OK;
 }
@@ -1465,6 +1487,7 @@ extern "C" int ccsim_run_stats(const ccsim_handle *h, int64_t out[16]) {
 }
 
 extern "C" int64_t ccsim_key_order_waves(const ccsim_handle *h) { return h ? h->last_key_order_waves : 0; }
+extern "C" int64_t ccsim_sorted_tile_waves(const ccsim_handle *h) { return h ? h->last_sorted_tile_waves : 0; }
 
 extern "C" int ccsim_flush_l2(ccsim_handle *h) {
   if (!h) return CCSIM_EINVAL;

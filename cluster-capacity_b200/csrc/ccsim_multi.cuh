@@ -47,6 +47,14 @@
 //   commit -> the kill test on each lane's one slot. A row is judged by a full cell test when the replay reaches it; a wake-up goes
 //   back to row 0 (see "the round in key order" below). C4: 778 -> 515 profiled cycles per round, kernel time 21.67-21.72 ->
 //   20.87-21.01 ms (one H100 80GB HBM3, 700 W power limit). CCSIM_DEBUG_FLAGS bit 6 keeps the arg-max round.
+// Sorted tile (single-use templates): a live node's key does not change during a launch (its row changes only when it wins, and
+//   then it is infeasible for the rest of the run; the replicated counters change feasibility, not scores). So the tile is ranked
+//   by key once per launch, the scan stores every node's key at its node's rank, and the tile's top 16 are its first 16 non-zero
+//   keys: one ballot per warp, a barrier and a prefix count instead of up to 16 REDUX rounds per warp and warp 0's 24-way merge.
+//   The lines are word for word the same. C4: CTA 0's scan + barrier + merge/publish 4 480 -> 2 880 cycles per wave, kernel time
+//   18.75-18.78 -> 17.54-17.56 ms (one H100 80GB HBM3, 700 W power limit). The host picks the instantiation (template parameter
+//   SORTED): the ones without it are the REDUX selection alone, compiled as before this selection existed (every sorted-tile
+//   statement sits behind `if constexpr`), for templates with second lives and CCSIM_DEBUG_FLAGS bit 7.
 // Look-ahead waves: a PodTopologySpread minimum move that REOPENS closed domains would end the wave (the reopened nodes were
 //   rejected by the scan and are in nobody's list). When a term's limit is about to move, the scan publishes the nodes of its
 //   closed cells too; they sit in the replay as dormant candidates (key 0: set-up reads the look-ahead terms' cells) and are
@@ -140,8 +148,14 @@ struct __align__(16) MultiShared {
   uint32_t wtop[LEAN_WARPS][MULTI_M];               // per-warp top-M (compact) keys of this wave
   int32_t gt_c1[MULTI_GT][4];                       // per replicated-counter term: {limit, payload shift, payload mask, domains of the counter}
   int32_t gt_commit[MULTI_GT][4];                   // ... {counter base, inc, PTS constraint tracked or -1, n_present}
-  uint32_t ckey[MULTI_CAP], cdom[MULTI_CAP], cnext[MULTI_CAP];   // the wave's candidates keyed >= T, in key order (node shards:
-                                                                 // unordered, and in a key-order wave cnext[r] = the candidate of rank r)
+  union {
+    struct {
+      uint32_t ckey[MULTI_CAP], cdom[MULTI_CAP], cnext[MULTI_CAP];   // the wave's candidates keyed >= T, in key order (node shards:
+                                                                     // unordered, and in a key-order wave cnext[r] = the candidate of rank r)
+    };
+    uint32_t skey[LEAN_THREADS];   // sorted tile: this wave's key of the tile node of rank r (0: infeasible), from the scan to the
+                                   // publish; the candidate arrays are written after the gather and read up to barrier R only
+  };
   unsigned long long gcnt[MULTI_GROUPS];            // compaction: per group of 32 gathered entries, its candidates per level (16 bits each)
   uint8_t kpart[MULTI_RANK_PARTS][MULTI_CAP];       // node shards, key order: partial ranks (keys greater than candidate i in one span)
   uint32_t red[LEAN_WARPS], red2[LEAN_WARPS];       // block reductions (T, best key)
@@ -154,9 +168,9 @@ struct __align__(16) MultiShared {
   int32_t single_use, ncand;
   int32_t xcount[CCSIM_MAX_WORLD];                  // node shards: candidates in each rank's summary
   uint32_t xglob[4];                                // node shards: best key, T_list, bar over all ranks
-  uint32_t delta, pad_ms;
+  uint32_t delta, st_tile_sel;                      // ..., CTA 0 / thread 0: waves that selected from the sorted tile
   int32_t relax[LEAN_MAX_TERMS];                    // per Filter term: this wave's look-ahead over the limit (0: strict), see "dormant candidates"
-  int32_t force_strict, st_relaxed, st_empty, pad_r;
+  int32_t force_strict, st_relaxed, st_empty, tile_sorted;
   long long ph[8], tc0, st_cand, st_overflow, st_rounds, st_key_order;   // CTA 0 / thread 0: clock cycles per phase, replay statistics
 #ifdef MULTI_ROUND_PROFILE
   long long rp_cyc[RP_N], rp_cnt[RP_N], rp_t;                  // CTA 0's replay warp: cycles and events per part of the replay
@@ -169,6 +183,15 @@ struct __align__(16) MultiShared {
 
 __shared__ MultiShared ms;
 static_assert(offsetof(MultiShared, ckey) % 16 == 0 && (MULTI_RANK_SPAN * 4) % 16 == 0, "key order: 16-byte loads of ckey");
+static_assert(3 * MULTI_CAP >= LEAN_THREADS && LEAN_THREADS % 4 == 0 && LEAN_THREADS <= 65536,
+              "sorted tile: the keys fit the candidate arrays, 16-byte loads of them, 16-bit ranks");
+// sorted tile: tile node j's rank in key order (once per launch). Only the sorted instantiation references it, so only its static
+// shared memory holds it (WAVE_KERNELS in ccsim_engine.cu adds it there)
+__shared__ uint16_t multi_tile_rank[LEAN_THREADS];
+#define MULTI_SORTED_SMEM (sizeof(uint16_t) * LEAN_THREADS)
+
+// the position of entry r (0 = best) of a CTA's list in its key line: the best key and the last key share the line's first 16 bytes
+__device__ __forceinline__ int multi_kpos(int r) { return r == 0 ? 0 : (r == MULTI_M - 1 ? 1 : r + 1); }
 
 struct MultiParams {
   uint32_t pay_shift[LEAN_MAX_SLOTS];   // record slot s (a topology column) -> bit position of its dom+1 field in the payload
@@ -296,7 +319,9 @@ __device__ __forceinline__ void multi_report(long long waves) {
 #endif
 }
 
-template <bool XGPU>
+// SORTED: the host chose the selection from the sorted tile (a single-use template: see plan_multi); the instantiations without it
+// are the REDUX selection alone, for templates with second lives and CCSIM_DEBUG_FLAGS bit 7
+template <bool XGPU, bool SORTED>
 __global__ void __launch_bounds__(LEAN_THREADS, 1) ccsim_wave_multi_kernel(const DevParams p, const LeanParams lp, const MultiParams mp) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   const size_t cp = (size_t)p.chunk_pad;
@@ -314,6 +339,7 @@ __global__ void __launch_bounds__(LEAN_THREADS, 1) ccsim_wave_multi_kernel(const
   const int tot = nlists * MULTI_M;
 
   if (tid == 0) { ms.accepted = 0; ms.dead = 0; ms.stopb = 0; ms.n_gt = 0; ms.ncand = 0; ms.delta = 1u << MULTI_IDX_BITS; ms.force_strict = 0; ms.st_relaxed = 0; ms.st_empty = 0;
+                  if (SORTED) { ms.tile_sorted = 0; ms.st_tile_sel = 0; }
                   for (int q = 0; q < LEAN_MAX_TERMS; q++) ms.relax[q] = 0;
                   for (int q = 0; q < 8; q++) ms.ph[q] = 0; ms.tc0 = 0; ms.st_cand = 0; ms.st_overflow = 0; ms.st_rounds = 0; ms.st_key_order = 0;
                   RPROF(for (int q = 0; q < RP_N; q++) ms.rp_cyc[q] = ms.rp_cnt[q] = 0; ms.rp_t = 0;)
@@ -364,9 +390,38 @@ __global__ void __launch_bounds__(LEAN_THREADS, 1) ccsim_wave_multi_kernel(const
         ms.single_use = su1;
       }
       __syncthreads();
+      // ---- single-use templates: the tile in key order, once per launch. A live node's key does not change during the launch: its
+      //      row changes only when it wins, and then it never passes the scan again; the replicated counters decide feasibility,
+      //      not scores. So with every node's key stored at the node's rank (ms.skey), the tile's top M are its first M non-zero
+      //      entries (see the selection below). Keyed exactly as the scan keys them; rank = the number of greater keys (keys are
+      //      unique: the index bits), counted by the node's own thread over the keys staged in ms.skey. The constants builds after
+      //      a minimum move keep the order. ----
+      if (SORTED && wv == 0 && ms.single_use) {     // (device-checked: otherwise this instantiation runs the REDUX selection)
+        uint32_t mine = 0u;
+        if (tid < cnt_nodes) {
+          int32_t sc = lean_rec4(t, lp, tid)[LR_SCORE];
+          if (sc < 0) sc = lean_rescore(t, lp, tid);
+          mine = ckey(sc, (uint32_t)(p.node_base + lo + tid));
+          ms.skey[tid] = mine;
+        }
+        __syncthreads();
+        if (tid < cnt_nodes) {
+          int r = 0, i = 0;
+          #pragma unroll 2
+          for (; i + 4 <= cnt_nodes; i += 4) {
+            const uint4 v = *reinterpret_cast<const uint4 *>(&ms.skey[i]);
+            r += (int)(v.x > mine) + (int)(v.y > mine) + (int)(v.z > mine) + (int)(v.w > mine);
+          }
+          for (; i < cnt_nodes; i++) r += (int)(ms.skey[i] > mine);
+          multi_tile_rank[tid] = (uint16_t)r;
+        }
+        if (tid == 0) ms.tile_sorted = 1;
+        __syncthreads();
+      }
       if (tid == 0) ls.dirty = 0;
     }
     // ---- fused Filter pass: this thread's node ----
+    const bool tile_sel = SORTED && ms.tile_sorted != 0;     // (block-uniform)
     uint32_t key = 0u;
     if (tid < cnt_nodes) {
       const int32_t j = tid;
@@ -386,11 +441,17 @@ __global__ void __launch_bounds__(LEAN_THREADS, 1) ccsim_wave_multi_kernel(const
         if (sc < 0) sc = lean_rescore(t, lp, j);
         key = ckey(sc, (uint32_t)(p.node_base + lo + j));
       }
+      if constexpr (SORTED) { if (tile_sel) ms.skey[multi_tile_rank[j]] = key; }
     }
-    // ---- the warp's M best keys (REDUX rounds; keys are unique, 0 = none) ----
+    // ---- the warp's M best keys (REDUX rounds; keys are unique, 0 = none). Sorted tile (single-use templates): none here, its keys
+    //      are in ms.skey by rank, see below (its instantiation keeps this loop for a device that finds the template is not single
+    //      use; "sorted" goes into the ballot, not into a branch around the loop: a trip count from a ballot is warp-uniform to the
+    //      compiler, which then puts no divergence check in front of every REDUX) ----
     {
       uint32_t rem = key;
-      const int nf = __popc(__ballot_sync(0xffffffffu, key != 0u));
+      bool has = key != 0u;
+      if constexpr (SORTED) has = has && !tile_sel;
+      const int nf = __popc(__ballot_sync(0xffffffffu, has));
       if (lane == 0) ms.wfeas[warp] = nf;
       if (lane >= nf && lane < MULTI_M) ms.wtop[warp][lane] = 0u;
       // (warp-uniform trip count: no REDUX rounds for entries that do not exist; not unrolled — sixteen predicated REDUX
@@ -408,7 +469,39 @@ __global__ void __launch_bounds__(LEAN_THREADS, 1) ccsim_wave_multi_kernel(const
     MPH_MARK(1);
     const unsigned long long tagbits = (unsigned long long)tag << KEY_TAG_SHIFT;
     const int par = (int)(wv & 1);
-    if (warp == 0) {
+    // two lines of 16 tagged words: line 0 [0] key 0  [1] key 15 | more-bit  [2..15] keys 1..14, line 1 [0..15] payloads 0..15 —
+    // a poller reads words 0-1 of line 0 in one 16-byte load: the list's best key and its last key (with "this tile has more
+    // feasible nodes"). (Node shards too: the lines stay on this GPU; what crosses NVLink is one summary per rank, below.)
+    bool merge = warp == 0;
+    if constexpr (SORTED) {
+      if (tile_sel) {
+        // ---- the CTA's M best from the sorted tile: its first M non-zero keys in rank order. Thread t holds rank t; its rank among
+        //      the feasible nodes is the feasible nodes of the warps before it plus those of the lanes before it (one count per warp,
+        //      barrier S2). The threads of ranks < M write their entries, threads tid < M past the last one the empty entries: the
+        //      same words as the merge below. ----
+        const uint32_t v = tid < cnt_nodes ? ms.skey[tid] : 0u;
+        const unsigned fm = __ballot_sync(0xffffffffu, v != 0u);
+        if (lane == 0) ms.wfeas[warp] = __popc(fm);
+        __syncthreads();                                                  // S2
+        const int32_t nfw = lane < LEAN_WARPS ? ms.wfeas[lane] : 0;
+        const int32_t total = __reduce_add_sync(0xffffffffu, nfw);
+        const int r = __reduce_add_sync(0xffffffffu, lane < warp ? nfw : 0) + __popc(fm & ((1u << lane) - 1u));
+        unsigned long long *myslots = p.slots + ((size_t)par * CCSIM_MAX_GRID + cta) * MULTI_LINE_WORDS;
+        if (v != 0u && r < MULTI_M) {
+          unsigned long long kw = (unsigned long long)v;
+          if (r == MULTI_M - 1 && total > MULTI_M) kw |= 1ull << MULTI_MORE_BIT;
+          st_slot(&myslots[multi_kpos(r)], kw | tagbits);
+          st_slot(&myslots[SLOT_STRIDE + r], c_pay[ckey_index(v) - (p.node_base + lo)] | tagbits);
+        }
+        if (tid < MULTI_M && tid >= total) {
+          st_slot(&myslots[multi_kpos(tid)], tagbits);
+          st_slot(&myslots[SLOT_STRIDE + tid], tagbits);
+        }
+        if (cta == 0 && tid == 0) ms.st_tile_sel++;
+      }
+      merge = merge && !tile_sel;
+    }
+    if (merge) {
       // ---- the CTA's M best: merge of the 24 sorted warp lists (lane w walks warp w's list), then publish the pairs ----
       int32_t total = lane < LEAN_WARPS ? ms.wfeas[lane] : 0;
       total = __reduce_add_sync(0xffffffffu, total);
@@ -448,21 +541,18 @@ __global__ void __launch_bounds__(LEAN_THREADS, 1) ccsim_wave_multi_kernel(const
         }
         }
       }
-      // two lines of 16 tagged words: line 0 [0] key 0  [1] key 15 | more-bit  [2..15] keys 1..14, line 1 [0..15] payloads 0..15 —
-      // a poller reads words 0-1 of line 0 in one 16-byte load: the list's best key and its last key (with "this tile has more
-      // feasible nodes")
       unsigned long long kw = (unsigned long long)mykey;
       if (lane == MULTI_M - 1 && total > L) kw |= 1ull << MULTI_MORE_BIT;
-      const int kpos = lane == 0 ? 0 : (lane == MULTI_M - 1 ? 1 : lane + 1);
-      {   // (node shards too: the lines stay on this GPU; what crosses NVLink is one summary per rank, below)
+      const int kpos = multi_kpos(lane);
+      {
         unsigned long long *myslots = p.slots + ((size_t)par * CCSIM_MAX_GRID + cta) * MULTI_LINE_WORDS;
         if (lane < MULTI_M) {
           st_slot(&myslots[kpos], kw | tagbits);
           st_slot(&myslots[SLOT_STRIDE + lane], pay | tagbits);
         }
       }
-      GPROF(if (lane == 0) { if (cta == 0) ms.gp_pub = clock64(); if (wv < GP_MAX_WAVES) gp_pub_ns[wv * CCSIM_MAX_GRID + cta] = globaltimer_ns(); })
     }
+    GPROF(if (tid == 0) { if (cta == 0) ms.gp_pub = clock64(); if (wv < GP_MAX_WAVES) gp_pub_ns[wv * CCSIM_MAX_GRID + cta] = globaltimer_ns(); })
     MPH_MARK(2);
     // ---- gather, level 1: the lines of THIS GPU's CTAs. Every thread waits for its own (<= MULTI_EPT) entries — key word and payload
     //      word — so that the bar and the entries cost ONE L2 round trip after the slowest CTA's lines land ----
@@ -1082,7 +1172,7 @@ __global__ void __launch_bounds__(LEAN_THREADS, 1) ccsim_wave_multi_kernel(const
     o->evals = o->waves * (long long)p.n;
     o->examined = o->evals;
     for (int q = 0; q < 8; q++) o->phase_cycles[q] = ms.ph[q];
-    o->stat[0] = ms.st_cand; o->stat[1] = ms.st_overflow; o->stat[2] = ms.st_rounds; o->stat[3] = ms.st_key_order;
+    o->stat[0] = ms.st_cand; o->stat[1] = ms.st_overflow; o->stat[2] = ms.st_rounds; o->stat[3] = SORTED ? (ms.st_key_order | ((long long)ms.st_tile_sel << 32)) : ms.st_key_order;
     // (CCSIM_DEBUG_FLAGS bit 3's summary stays in the kernel body: a printf inlined from a helper puts its argument buffer ahead
     //  of the MultiParams copy in the stack frame, which then grows from 136 to 192 bytes and takes a register more)
     if (p.debug_flags & DBG_CYCLES)

@@ -17,7 +17,7 @@ _lib = None
 EXPORTS = ["ccsim_create", "ccsim_destroy", "ccsim_last_error", "ccsim_abi_version", "ccsim_load_nodes",
            "ccsim_set_templates", "ccsim_run", "ccsim_prepare", "ccsim_node_counts", "ccsim_peer_export", "ccsim_peer_import",
            "ccsim_device_info", "ccsim_kernel_launches", "ccsim_kernel_name", "ccsim_flush_l2", "ccsim_run_stats", "ccsim_peer_local",
-           "ccsim_peer_import_local", "ccsim_key_order_waves", "ccsim_run_each", "ccsim_set_analyses"]
+           "ccsim_peer_import_local", "ccsim_key_order_waves", "ccsim_sorted_tile_waves", "ccsim_run_each", "ccsim_set_analyses"]
 
 
 class EngineError(RuntimeError):
@@ -67,6 +67,8 @@ def lib():
         L.ccsim_run_stats.argtypes = [C.c_void_p, abi.P64]
         L.ccsim_key_order_waves.restype = C.c_int64
         L.ccsim_key_order_waves.argtypes = [C.c_void_p]
+        L.ccsim_sorted_tile_waves.restype = C.c_int64
+        L.ccsim_sorted_tile_waves.argtypes = [C.c_void_p]
         L.ccsim_peer_export.restype = C.c_int
         L.ccsim_peer_export.argtypes = [C.c_void_p, abi.PU8]
         L.ccsim_peer_import.restype = C.c_int
@@ -209,6 +211,11 @@ class Engine:
     def key_order_waves(self):
         """Waves of the last run the multi-commit kernel replayed in key order (see ccsim_key_order_waves in include/ccsim.h)."""
         return int(lib().ccsim_key_order_waves(self._h))
+
+    def sorted_tile_waves(self):
+        """Waves of the last run the multi-commit kernel selected each tile's candidates from the tile sorted by key (see
+        ccsim_sorted_tile_waves in include/ccsim.h)."""
+        return int(lib().ccsim_sorted_tile_waves(self._h))
 
     def kernel_launches(self):
         return int(lib().ccsim_kernel_launches(self._h))

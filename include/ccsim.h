@@ -370,6 +370,10 @@ int  ccsim_run_stats(const ccsim_handle *h, int64_t out[16]);
  * winner taken by a ballot); 0 for the other engines, for templates whose winners may come back in their wave, and under
  * CCSIM_DEBUG_FLAGS bit 6 */
 int64_t ccsim_key_order_waves(const ccsim_handle *h);
+/* waves of the last run in which the multi-commit kernel took each tile's published candidates from the tile sorted by key once
+ * per launch (single-use templates: the first 16 feasible nodes in key order, by a prefix count); 0 for the other engines, for
+ * templates whose winners may come back in their wave, and under CCSIM_DEBUG_FLAGS bit 7 */
+int64_t ccsim_sorted_tile_waves(const ccsim_handle *h);
 
 #ifdef __cplusplus
 }
