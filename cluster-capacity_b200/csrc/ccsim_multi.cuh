@@ -28,9 +28,10 @@
 //
 // Exchange: two 128-byte lines per CTA = M (key, payload) pairs (keys in line 0, payloads in line 1), each word tagged
 //   (self-validating, no fences).
-//   single GPU : lines live in the handle's slot buffer (L2), st/ld.relaxed.gpu;
-//   node shards: every CTA stores its line into EVERY rank's line buffer (CUDA IPC mappings, st.relaxed.sys.v2 over NVLink)
-//                and polls its local copy — an all-gather of world x grid lines fused into the persistent kernel.
+//   lines live in the handle's slot buffer (L2), st/ld.relaxed.gpu; every CTA compacts the candidates of all lines.
+//   node shards: the lines stay on their GPU; after that compaction ONE CTA of every rank stores a summary of the rank's candidates
+//                into every peer's line buffer (CUDA IPC mappings, st.relaxed.sys over NVLink), and every CTA compacts the
+//                summaries in rank order the same way.
 // Replay: ONE warp, no barrier inside: <= 8 candidates per lane in registers; a round is arg-max (REDUX) -> commit (lane q =
 //   counter term q: cell += inc, over-limit test, PTS-minimum tracking, all from registers) -> kill the candidates sitting in
 //   a cell that just filled (SWAR field test against the OR-reduced filled cells). Measured on C4 (one H100 80GB HBM3,
@@ -41,8 +42,7 @@
 //   those cycles (scripts/round_profile.sh). Work around the round stays on this warp: moved onto the whole block (the set-up
 //   between G1 and G2, the look-ahead decision after R) it measured slower on C4, whose terms have 8 and 64 domains.
 //   Row updates of the winners are done by each node's own thread after that barrier (a thread owns its node).
-// Key order (single-use templates: no second lives): the compaction stores the wave's candidates in key order (node shards: the
-//   block ranks them after the second gather level), and the replay
+// Key order (single-use templates: no second lives): the compaction stores the wave's candidates in key order, and the replay
 //   warp holds them in rows of 32 in key order; a round is ballot(live) -> the lowest live lane -> one SHFL of its payload -> the same
 //   commit -> the kill test on each lane's one slot. A row is judged by a full cell test when the replay reaches it; a wake-up goes
 //   back to row 0 (see "the round in key order" below). C4: 778 -> 515 profiled cycles per round, kernel time 21.67-21.72 ->
@@ -65,7 +65,8 @@
 
 #define MULTI_M 16                /* candidates per CTA and wave: 16 keys in one 128-byte slot line, their 16 payloads in a second */
 #define MULTI_LINE_WORDS (2 * SLOT_STRIDE)   /* 64-bit words per CTA in the slot buffer: its two lines (one writer per line) */
-#define MULTI_EPT 3               /* gather: published entries per thread (grid x MULTI_M <= MULTI_EPT x LEAN_THREADS, host-checked) */
+#define MULTI_EPT 3               /* gather: entries per thread (grid x MULTI_M <= MULTI_EPT x LEAN_THREADS, host-checked; node shards:
+                                     the ranks' summaries, static_assert below) */
 #define SLOTS_WORDS (2 * CCSIM_MAX_GRID * MULTI_LINE_WORDS)   /* the handle's slot buffer, sized for this kernel's [parity][CTA][2 lines];
                                                                  the other kernels use [parity][CTA][1 line], its first half */
 #define MULTI_PAY_BITS 27         /* payload bits for domain ids (dom+1 per topology slot, each field followed by a zero guard bit) */
@@ -79,13 +80,9 @@
 #define MULTI_CAP (32 * MULTI_CPT)
 #define MULTI_LEVELS 4            /* compaction: score levels below the best key it ranks (one 16-bit count per level in a 64-bit word) */
 #define MULTI_GROUPS (MULTI_EPT * LEAN_WARPS)   /* compaction: groups of 32 gathered entries (two lists), one count word each */
-#define MULTI_BINS 64             /* node shards, gather level 2: histogram bins of the bar raise */
 #define MULTI_RELAX_K 8           /* look-ahead on a PTS term when at most this many of its domains still sit at the global minimum ... */
 #define MULTI_RELAX_R 3           /* ... nodes in cells up to this far over the limit are published as dormant candidates */
-#define MULTI_XPT (((CCSIM_MAX_WORLD - 1) * MULTI_CAP + LEAN_THREADS - 1) / LEAN_THREADS)   /* node shards: remote candidates per thread */
-#define MULTI_RANK_PARTS (LEAN_THREADS / MULTI_CAP)                       /* node shards, key order: threads that count one candidate's rank ... */
-#define MULTI_RANK_SPAN (((MULTI_CAP + MULTI_RANK_PARTS - 1) / MULTI_RANK_PARTS + 3) & ~3)   /* ... each over this many keys (16-byte loads) */
-static_assert(MULTI_RANK_PARTS >= 1 && MULTI_RANK_SPAN < 256, "key order: a partial rank fits a byte");
+static_assert(CCSIM_MAX_WORLD * MULTI_CAP <= MULTI_EPT * LEAN_THREADS, "node shards: the ranks' summaries fit the gather's entries");
 static_assert(MULTI_GROUPS <= 96 && MULTI_EPT * LEAN_THREADS < 65536, "compaction: three count words per lane, a count fits 16 bits");
 static_assert(MULTI_CPT <= 32, "key order: one won bit per row");
 static_assert(MULTI_M == SLOT_STRIDE, "the keys of a CTA's list fill exactly one slot line");
@@ -105,10 +102,9 @@ static_assert(4 + 2 * MULTI_CAP <= CCSIM_MAX_GRID * SLOT_STRIDE, "node shards: a
 #define RP_HANDOFF 5              /* after the loop: winners -> ms.mult */
 #define RP_DECIDE 6               /* after the loop: the next wave's look-ahead decision */
 #define RP_MINMOVE 7              /* + term q */
-#define RP_RANK (RP_MINMOVE + MULTI_GT)   /* node shards, key order: ranking the wave's candidates (block-wide, up to the barrier after it) */
-#define RP_KROUND (RP_RANK + 1)   /* key order: the common round (ballot -> commit -> kill) */
-#define RP_ADVANCE (RP_RANK + 2)  /* key order: moving on to the next row (loads + full cell test), per row loaded */
-#define RP_N (RP_RANK + 3)
+#define RP_KROUND (RP_MINMOVE + MULTI_GT)   /* key order: the common round (ballot -> commit -> kill) */
+#define RP_ADVANCE (RP_KROUND + 1)  /* key order: moving on to the next row (loads + full cell test), per row loaded */
+#define RP_N (RP_KROUND + 2)
 #ifdef MULTI_ROUND_PROFILE
 #define RPROF(...) __VA_ARGS__
 #define RP_ADD(i, cyc, n) do { if (cta == 0 && lane == 0) { ms.rp_cyc[i] += (cyc); ms.rp_cnt[i] += (n); } } while (0)
@@ -120,7 +116,8 @@ static_assert(4 + 2 * MULTI_CAP <= CCSIM_MAX_GRID * SLOT_STRIDE, "node shards: a
 // Gather profile (profiling builds only: -DMULTI_GATHER_PROFILE; the hooks expand to nothing otherwise). CTA 0 adds up, per wave:
 // the cycles from its own publish to the poll round in which the last of its entries was valid (the latest of its threads), and
 // the number of poll rounds (the most any thread took); from there to the point where the CTA may read every entry (G1); the
-// compaction in key order up to the barrier after its stores (G3), and in how many waves the level clamp raised the bar. Every CTA
+// compaction in key order up to the barrier after its stores (G3), and how often the level clamp raised the bar (node shards: both
+// gather levels). Every CTA
 // also writes its %globaltimer at publish into gp_pub_ns[wave][CTA]; the host reports the skew of the publishes, latest minus CTA
 // 0's, per wave. scripts/gather_profile.sh prints both.
 #define GP_POLL 0
@@ -150,23 +147,21 @@ struct __align__(16) MultiShared {
   int32_t gt_commit[MULTI_GT][4];                   // ... {counter base, inc, PTS constraint tracked or -1, n_present}
   union {
     struct {
-      uint32_t ckey[MULTI_CAP], cdom[MULTI_CAP], cnext[MULTI_CAP];   // the wave's candidates keyed >= T, in key order (node shards:
-                                                                     // unordered, and in a key-order wave cnext[r] = the candidate of rank r)
+      uint32_t ckey[MULTI_CAP], cdom[MULTI_CAP], cnext[MULTI_CAP];   // the wave's candidates keyed >= T, in key order: key, domain
+                                                                     // payload, second-life key
     };
     uint32_t skey[LEAN_THREADS];   // sorted tile: this wave's key of the tile node of rank r (0: infeasible), from the scan to the
                                    // publish; the candidate arrays are written after the gather and read up to barrier R only
   };
   unsigned long long gcnt[MULTI_GROUPS];            // compaction: per group of 32 gathered entries, its candidates per level (16 bits each)
-  uint8_t kpart[MULTI_RANK_PARTS][MULTI_CAP];       // node shards, key order: partial ranks (keys greater than candidate i in one span)
   uint32_t red[LEAN_WARPS], red2[LEAN_WARPS];       // block reductions (T, best key)
-  uint32_t hist[MULTI_BINS];
   int32_t wfeas[LEAN_WARPS];
   int32_t gt_term[MULTI_GT];                        // indices of the Filter terms that read a replicated (non node-local) counter
   int32_t acc_node[MULTI_MAX_ACC];                  // replay: nodes accepted in this wave, in order
   int32_t mult[LEAN_THREADS];                       // replay -> row updates: times tile node j was accepted in this wave (its thread resets it)
   int32_t n_gt, accepted, dead, stopb;
-  int32_t single_use, ncand;
-  int32_t xcount[CCSIM_MAX_WORLD];                  // node shards: candidates in each rank's summary
+  int32_t single_use;
+  int32_t xcount[CCSIM_MAX_WORLD];                  // node shards: candidates in each rank's summary (this rank's: its own)
   uint32_t xglob[4];                                // node shards: best key, T_list, bar over all ranks
   uint32_t delta, st_tile_sel;                      // ..., CTA 0 / thread 0: waves that selected from the sorted tile
   int32_t relax[LEAN_MAX_TERMS];                    // per Filter term: this wave's look-ahead over the limit (0: strict), see "dormant candidates"
@@ -182,8 +177,7 @@ struct __align__(16) MultiShared {
 };
 
 __shared__ MultiShared ms;
-static_assert(offsetof(MultiShared, ckey) % 16 == 0 && (MULTI_RANK_SPAN * 4) % 16 == 0, "key order: 16-byte loads of ckey");
-static_assert(3 * MULTI_CAP >= LEAN_THREADS && LEAN_THREADS % 4 == 0 && LEAN_THREADS <= 65536,
+static_assert(offsetof(MultiShared, skey) % 16 == 0 && 3 * MULTI_CAP >= LEAN_THREADS && LEAN_THREADS % 4 == 0 && LEAN_THREADS <= 65536,
               "sorted tile: the keys fit the candidate arrays, 16-byte loads of them, 16-bit ranks");
 // sorted tile: tile node j's rank in key order (once per launch). Only the sorted instantiation references it, so only its static
 // shared memory holds it (WAVE_KERNELS in ccsim_engine.cu adds it there)
@@ -220,48 +214,69 @@ __device__ __forceinline__ int nth_set_lane(unsigned m, int g) {
   return m ? __ffs(m) - 1 : -1;
 }
 
-// node shards, gather level 2: warp-aggregated append of the lanes' candidates to the wave's candidate arrays (unordered: keys are unique)
-__device__ __forceinline__ void multi_append(bool keep, uint32_t ck, unsigned long long b, int lane) {
-  const unsigned m = __ballot_sync(0xffffffffu, keep);
-  if (m) {
-    int base = 0;
-    const int leader = __ffs(m) - 1;
-    if (lane == leader) base = atomicAdd(&ms.ncand, __popc(m));
-    base = __shfl_sync(0xffffffffu, base, leader);
-    const int idx = base + __popc(m & ((1u << lane) - 1u));
-    if (keep && idx < MULTI_CAP) {
-      ms.ckey[idx] = ck;
-      ms.cdom[idx] = (uint32_t)b & ((1u << MULTI_PAY_BITS) - 1u);
-      ms.cnext[idx] = (uint32_t)(b >> MULTI_NEXT_SHIFT) & 0xfffu;
+// ---- the gathered entries keyed >= T go into shared memory in key order, straight to their ranks (every thread of the block calls
+//      this, with the same T and kbest). Entry u of thread tid is entry e = tid + u * LEAN_THREADS of a concatenation that is in key
+//      order within every score level: ea[u] holds its key (0: none), eb[u] its payload. An entry's level is its score's distance below
+//      the best key's score. Entry u of warp w's threads lies in group g = w + LEAN_WARPS * u of 32 entries, in lane order. So a
+//      candidate's rank is
+//        #(candidates on higher levels) + #(candidates on its level in groups < g) + #(candidates on its level in lanes < its lane),
+//      exact because keys are unique. Per-level ballots give the last term and the group's counts, one barrier publishes the
+//      counts (one 64-bit word per group), and every warp sums what it needs of them itself.
+//      At most MULTI_LEVELS levels are ranked: when the candidates span more, the bar goes up to the lowest key of the lowest
+//      level ranked. More than MULTI_CAP candidates: the bar is the key of rank MULTI_CAP - 1. Either bar is above T, and any bar
+//      above T is valid: the best candidate is still in, and a strict wave places it. Returns the candidates stored (<= MULTI_CAP)
+//      and sets T to the bar. The candidate arrays are written after the first barrier only. ----
+__device__ __forceinline__ int multi_compact(const unsigned long long (&ea)[MULTI_EPT], const unsigned long long (&eb)[MULTI_EPT], uint32_t &T,
+                                             const uint32_t kbest, const int cta) {
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  GPROF(const long long gp_t = clock64();)
+  const uint32_t kbl = kbest >> MULTI_IDX_BITS;
+  int rk[MULTI_EPT];                       // the entry's level << 8 | its place among the group's candidates on that level; -1: none
+  bool beyond = false;                     // a candidate more than MULTI_LEVELS - 1 levels below the best key
+  #pragma unroll
+  for (int u = 0; u < MULTI_EPT; u++) {
+    const uint32_t ck = (uint32_t)ea[u];   // (0 beyond the entries)
+    const bool q = ck != 0u && ck >= T;
+    const uint32_t lv = kbl - (ck >> MULTI_IDX_BITS);
+    beyond |= q && lv >= MULTI_LEVELS;
+    unsigned long long wc = 0ull;
+    int pos = 0;
+    #pragma unroll
+    for (int v = 0; v < MULTI_LEVELS; v++) {
+      const unsigned b = __ballot_sync(0xffffffffu, q && lv == (uint32_t)v);
+      wc |= (unsigned long long)__popc(b) << (16 * v);
+      if (lv == (uint32_t)v) pos = __popc(b & ((1u << lane) - 1u));
+    }
+    rk[u] = (q && lv < MULTI_LEVELS) ? (int)(lv << 8) | pos : -1;
+    if (lane == 0) ms.gcnt[warp + LEAN_WARPS * u] = wc;
+  }
+  const bool clamp = __syncthreads_or(beyond);                      // G2
+  // lane l sums groups l, l + 32, l + 64: all of them (the candidates per level), and those before each of this warp's groups
+  const unsigned long long g0 = ms.gcnt[lane], g1 = ms.gcnt[lane + 32], g2 = lane + 64 < MULTI_GROUPS ? ms.gcnt[lane + 64] : 0ull;
+  const unsigned long long gs = g0 + g1 + g2;
+  const unsigned long long S = ((unsigned long long)__reduce_add_sync(0xffffffffu, (uint32_t)(gs >> 32)) << 32) | __reduce_add_sync(0xffffffffu, (uint32_t)gs);
+  const unsigned long long Sabove = S * 0x0001000100010000ull;    // field v: the candidates on levels < v
+  const int total = (int)((S * 0x0001000100010001ull) >> 48);
+  #pragma unroll
+  for (int u = 0; u < MULTI_EPT; u++) {
+    const int g = warp + LEAN_WARPS * u;
+    const unsigned long long ps = (lane < g ? g0 : 0ull) + (lane + 32 < g ? g1 : 0ull) + (lane + 64 < g ? g2 : 0ull);
+    const unsigned long long P = ((unsigned long long)__reduce_add_sync(0xffffffffu, (uint32_t)(ps >> 32)) << 32) | __reduce_add_sync(0xffffffffu, (uint32_t)ps);
+    if (rk[u] >= 0) {
+      const int r = (int)(((Sabove + P) >> (16 * (rk[u] >> 8))) & 0xffffu) + (rk[u] & 0xff);
+      if (r < MULTI_CAP) {
+        ms.ckey[r] = (uint32_t)ea[u];
+        ms.cdom[r] = (uint32_t)eb[u] & ((1u << MULTI_PAY_BITS) - 1u);
+        ms.cnext[r] = (uint32_t)(eb[u] >> MULTI_NEXT_SHIFT) & 0xfffu;
+      }
     }
   }
-}
-
-// Node shards, gather level 2: more candidates than the replay holds. The bar T is raised to the lowest of MULTI_BINS equal steps
-// between T and the best key that leaves <= MULTI_CAP candidates; every CTA sees the same data and decides alike. The caller zeroes ms.hist; after a barrier
-// it counts its candidates into it with multi_hist_add and empties the candidate arrays (multi_bar_reset: every thread has read
-// ms.ncand before that barrier); after one more barrier multi_raise_bar returns the new T. Every warp computes it alike from the
-// histogram, so no barrier follows: the next write of ms.hist or ms.ncand is behind the barrier that ends the second append pass.
-__device__ __forceinline__ void multi_hist_add(uint32_t ck, uint32_t T, unsigned long long range) {
-  if (ck != 0u && ck >= T) atomicAdd(&ms.hist[(unsigned)(((unsigned long long)(ck - T) * MULTI_BINS) / range)], 1u);
-}
-__device__ __forceinline__ void multi_bar_reset(int cta) {
-  if (threadIdx.x == 0) ms.ncand = 0;
-  if (cta == 0 && threadIdx.x == 0) ms.st_overflow++;
-}
-static_assert(MULTI_BINS == 64, "multi_raise_bar: two histogram bins per lane");
-__device__ __forceinline__ uint32_t multi_raise_bar(uint32_t T, uint32_t kbest, unsigned long long range) {
-  // suf(b) = the candidates in bins >= b does not grow with b, so the lowest bin with suf(b) <= MULTI_CAP is the number of bins
-  // with suf(b) > MULTI_CAP (MULTI_BINS when even the top bin holds more: the bar goes to the best key). Lane l holds bins 2l and
-  // 2l + 1; a suffix sum over the lanes gives suf(2l), and suf(2l + 1) = suf(2l) - hist[2l]. (Every thread used to walk down the
-  // 64 bins one by one, a compare and a branch per bin, and two more block barriers followed.)
-  const int lane = threadIdx.x & 31;
-  const uint32_t h0 = ms.hist[2 * lane], h1 = ms.hist[2 * lane + 1];
-  uint32_t suf = h0 + h1;
-  #pragma unroll
-  for (int o = 1; o < 32; o <<= 1) { const uint32_t v = __shfl_down_sync(0xffffffffu, suf, o); if (lane + o < 32) suf += v; }
-  const int bsel = __popc(__ballot_sync(0xffffffffu, suf > (uint32_t)MULTI_CAP)) + __popc(__ballot_sync(0xffffffffu, suf - h0 > (uint32_t)MULTI_CAP));
-  return (bsel >= MULTI_BINS) ? kbest : T + (uint32_t)(((unsigned long long)bsel * range + (MULTI_BINS - 1)) / MULTI_BINS);
+  if (clamp) T = (kbl - (MULTI_LEVELS - 1)) << MULTI_IDX_BITS;
+  if (cta == 0 && tid == 0 && total > MULTI_CAP) ms.st_overflow++;
+  __syncthreads();                                                  // G3
+  if (total > MULTI_CAP) T = ms.ckey[MULTI_CAP - 1];
+  GPROF(if (cta == 0 && tid == 0) { ms.gp_cyc[GP_COMPACT] += clock64() - gp_t; ms.gp_cnt[GP_CLAMP] += clamp; })
+  return min(total, MULTI_CAP);
 }
 
 // node shards: wait until the N (2 or 3) words at src — part of a peer's summary, written into this GPU's memory over NVLink — carry
@@ -298,9 +313,8 @@ __device__ __forceinline__ void multi_report(long long waves) {
     printf("round profile: after the loop %lld waves, %.0f cycles/wave (hand-off %.0f, look-ahead decision %.0f)\n", ms.rp_cnt[RP_AFTER],
            ms.rp_cyc[RP_AFTER] / w, ms.rp_cyc[RP_HANDOFF] / w, ms.rp_cyc[RP_DECIDE] / w);
     printf("round profile: rounds with a non-zero kill mask %lld\n", ms.rp_cnt[RP_KILL]);
-    printf("round profile: key order %lld waves | ranking %.0f cycles/wave | common round %lld events, %.0f cycles/round, %.0f cycles/wave"
+    printf("round profile: key order %lld waves | common round %lld events, %.0f cycles/round, %.0f cycles/wave"
            " | row advances %lld, %.0f cycles each, %.0f cycles/wave\n", ms.st_key_order,
-           ms.rp_cyc[RP_RANK] / (double)(ms.rp_cnt[RP_RANK] > 0 ? ms.rp_cnt[RP_RANK] : 1),
            ms.rp_cnt[RP_KROUND], ms.rp_cyc[RP_KROUND] / (double)(ms.rp_cnt[RP_KROUND] > 0 ? ms.rp_cnt[RP_KROUND] : 1), ms.rp_cyc[RP_KROUND] / w,
            ms.rp_cnt[RP_ADVANCE], ms.rp_cyc[RP_ADVANCE] / (double)(ms.rp_cnt[RP_ADVANCE] > 0 ? ms.rp_cnt[RP_ADVANCE] : 1), ms.rp_cyc[RP_ADVANCE] / w);
     for (int q = 0; q < MULTI_GT; q++)
@@ -338,7 +352,7 @@ __global__ void __launch_bounds__(LEAN_THREADS, 1) ccsim_wave_multi_kernel(const
   const int nlists = p.grid;                            // lines of this GPU (node shards: every rank launches the same grid, sized from the largest shard)
   const int tot = nlists * MULTI_M;
 
-  if (tid == 0) { ms.accepted = 0; ms.dead = 0; ms.stopb = 0; ms.n_gt = 0; ms.ncand = 0; ms.delta = 1u << MULTI_IDX_BITS; ms.force_strict = 0; ms.st_relaxed = 0; ms.st_empty = 0;
+  if (tid == 0) { ms.accepted = 0; ms.dead = 0; ms.stopb = 0; ms.n_gt = 0; ms.delta = 1u << MULTI_IDX_BITS; ms.force_strict = 0; ms.st_relaxed = 0; ms.st_empty = 0;
                   if (SORTED) { ms.tile_sorted = 0; ms.st_tile_sel = 0; }
                   for (int q = 0; q < LEAN_MAX_TERMS; q++) ms.relax[q] = 0;
                   for (int q = 0; q < 8; q++) ms.ph[q] = 0; ms.tc0 = 0; ms.st_cand = 0; ms.st_overflow = 0; ms.st_rounds = 0; ms.st_key_order = 0;
@@ -600,10 +614,8 @@ __global__ void __launch_bounds__(LEAN_THREADS, 1) ccsim_wave_multi_kernel(const
     uint32_t Tlist = __reduce_max_sync(0xffffffffu, lane < LEAN_WARPS ? ms.red[lane] : 0u);
     uint32_t kbest = __reduce_max_sync(0xffffffffu, lane < LEAN_WARPS ? ms.red2[lane] : 0u);
     bool dead = ms.dead != 0;
-    GPROF(long long gp_t = 0;
-          if (cta == 0 && tid == 0) {
-            gp_t = clock64();
-            ms.gp_cyc[GP_POLL] += (long long)ms.gp_valid - ms.gp_pub; ms.gp_cyc[GP_SYNC] += gp_t - (long long)ms.gp_valid;
+    GPROF(if (cta == 0 && tid == 0) {
+            ms.gp_cyc[GP_POLL] += (long long)ms.gp_valid - ms.gp_pub; ms.gp_cyc[GP_SYNC] += clock64() - (long long)ms.gp_valid;
             ms.gp_cnt[GP_ROUNDS] += (long long)ms.gp_spins; ms.gp_valid = ms.gp_spins = 0ull;
           })
     // The replay bar: T = the largest "last key" of a list whose tile has unseen feasible nodes is the lowest VALID bar; any
@@ -612,83 +624,28 @@ __global__ void __launch_bounds__(LEAN_THREADS, 1) ccsim_wave_multi_kernel(const
     // previous waves (doubled when the replay ran out of candidates above an artificial bar, shrunk when too many qualified).
     // Every CTA of every rank computes the same sequence from the same exchanged data.
     uint32_t T = max(Tlist, kbest > delta ? kbest - delta : 0u);
-    // ---- the entries keyed >= T go into shared memory in key order, straight to their ranks. Every list is sorted (keys descending,
-    //      then zeros), so its entries keyed >= T are a prefix of it, and list l is tile l: a lower list holds lower node indices, which
-    //      rank higher at the same score. An entry's level is its score's distance below the best key's score. Entry u of warp w's
-    //      threads lies in group g = w + LEAN_WARPS * u of 32 entries: lists 2g and 2g + 1, in lane order. So a candidate's rank is
-    //        #(candidates on higher levels) + #(candidates on its level in groups < g) + #(candidates on its level in lanes < its lane),
-    //      exact because keys are unique. Per-level ballots give the last term and the group's counts, one barrier publishes the
-    //      counts (one 64-bit word per group), and every warp sums what it needs of them itself.
-    //      At most MULTI_LEVELS levels are ranked: when the candidates span more, the bar goes up to the lowest key of the lowest
-    //      level ranked. More than MULTI_CAP candidates: the bar is the key of rank MULTI_CAP - 1. Either bar is above T, and any bar
-    //      above T is valid: the best candidate is still in, and a strict wave places it. ----
+    // ---- the entries keyed >= T into shared memory in key order. Every list is sorted (keys descending, then zeros), and list l is
+    //      tile l: a lower list holds lower node indices, which rank higher at the same score. So the concatenated lists are in key
+    //      order within every score level ----
     int C = 0;
-    if (!dead) {
-      const uint32_t kbl = kbest >> MULTI_IDX_BITS;
-      int rk[MULTI_EPT];                       // the entry's level << 8 | its place among the group's candidates on that level; -1: none
-      bool beyond = false;                     // a candidate more than MULTI_LEVELS - 1 levels below the best key
-      #pragma unroll
-      for (int u = 0; u < MULTI_EPT; u++) {
-        const uint32_t ck = (uint32_t)ea[u];   // (0 beyond the entries)
-        const bool q = ck != 0u && ck >= T;
-        const uint32_t lv = kbl - (ck >> MULTI_IDX_BITS);
-        beyond |= q && lv >= MULTI_LEVELS;
-        unsigned long long wc = 0ull;
-        int pos = 0;
-        #pragma unroll
-        for (int v = 0; v < MULTI_LEVELS; v++) {
-          const unsigned b = __ballot_sync(0xffffffffu, q && lv == (uint32_t)v);
-          wc |= (unsigned long long)__popc(b) << (16 * v);
-          if (lv == (uint32_t)v) pos = __popc(b & ((1u << lane) - 1u));
-        }
-        rk[u] = (q && lv < MULTI_LEVELS) ? (int)(lv << 8) | pos : -1;
-        if (lane == 0) ms.gcnt[warp + LEAN_WARPS * u] = wc;
-      }
-      const bool clamp = __syncthreads_or(beyond);                      // G2
-      // lane l sums groups l, l + 32, l + 64: all of them (the candidates per level), and those before each of this warp's groups
-      const unsigned long long g0 = ms.gcnt[lane], g1 = ms.gcnt[lane + 32], g2 = lane + 64 < MULTI_GROUPS ? ms.gcnt[lane + 64] : 0ull;
-      const unsigned long long gs = g0 + g1 + g2;
-      const unsigned long long S = ((unsigned long long)__reduce_add_sync(0xffffffffu, (uint32_t)(gs >> 32)) << 32) | __reduce_add_sync(0xffffffffu, (uint32_t)gs);
-      const unsigned long long Sabove = S * 0x0001000100010000ull;    // field v: the candidates on levels < v
-      const int total = (int)((S * 0x0001000100010001ull) >> 48);
-      #pragma unroll
-      for (int u = 0; u < MULTI_EPT; u++) {
-        const int g = warp + LEAN_WARPS * u;
-        const unsigned long long ps = (lane < g ? g0 : 0ull) + (lane + 32 < g ? g1 : 0ull) + (lane + 64 < g ? g2 : 0ull);
-        const unsigned long long P = ((unsigned long long)__reduce_add_sync(0xffffffffu, (uint32_t)(ps >> 32)) << 32) | __reduce_add_sync(0xffffffffu, (uint32_t)ps);
-        if (rk[u] >= 0) {
-          const int r = (int)(((Sabove + P) >> (16 * (rk[u] >> 8))) & 0xffffu) + (rk[u] & 0xff);
-          if (r < MULTI_CAP) {
-            ms.ckey[r] = (uint32_t)ea[u];
-            ms.cdom[r] = (uint32_t)eb[u] & ((1u << MULTI_PAY_BITS) - 1u);
-            ms.cnext[r] = (uint32_t)(eb[u] >> MULTI_NEXT_SHIFT) & 0xfffu;
-          }
-        }
-      }
-      if (clamp) T = (kbl - (MULTI_LEVELS - 1)) << MULTI_IDX_BITS;
-      if (cta == 0 && tid == 0 && total > MULTI_CAP) ms.st_overflow++;
-      __syncthreads();                                                  // G3
-      if (total > MULTI_CAP) T = ms.ckey[MULTI_CAP - 1];
-      C = min(total, MULTI_CAP);
-      GPROF(if (cta == 0 && tid == 0) { const long long t2 = clock64(); ms.gp_cyc[GP_COMPACT] += t2 - gp_t; ms.gp_cnt[GP_CLAMP] += clamp; gp_t = t2; })
-    }
+    if (!dead) C = multi_compact(ea, eb, T, kbest, cta);
     if (XGPU) {
       // ---- gather, level 2 (node shards): every rank now holds ITS candidates keyed >= its bar T_r (<= MULTI_CAP of them, the same in
       //      all of its CTAs). One summary per (source, destination) pair crosses NVLink — {best key, count, T_r, T_list_r, the
       //      candidates} written by ONE CTA of the source as a few 128-byte stores — instead of every CTA's line going to every
       //      rank and world x grid lines being polled by every CTA. The global bar max(max_r T_r, best - delta) is at least every
-      //      rank's own bar, so the union of the summaries holds every node keyed above it: same candidates as one GPU would see. ----
+      //      rank's own bar, so the union of the summaries holds every node keyed above it: same candidates as one GPU would see.
+      //      The summaries concatenated in rank order are in key order within every score level, as the lists are at level 1: each
+      //      summary is in key order, and rank r holds the nodes [per * r, per * (r + 1)), which rank higher than rank r + 1's at the
+      //      same score. So the same compaction ranks their union. ----
       const int xpar = (int)((wv + p.xwave0) & 1);
-      const int Cl = C < MULTI_CAP ? C : MULTI_CAP;
-      uint32_t lkey = 0u; unsigned long long lpay = 0ull;        // this rank's candidate `tid`, kept across the shared-memory rebuild
-      if (tid < Cl) { lkey = ms.ckey[tid]; lpay = (unsigned long long)ms.cdom[tid] | ((unsigned long long)ms.cnext[tid] << MULTI_NEXT_SHIFT); }
       if (!dead)
         for (int d = cta; d < p.world; d += p.grid) {            // CTA d of the source writes the copy for rank d
           if (d == p.rank) continue;
           unsigned long long *dst = p.xslots_peer[d] + XLINES_OFF + ((size_t)xpar * CCSIM_MAX_WORLD + p.rank) * CCSIM_MAX_GRID * SLOT_STRIDE;
-          if (tid < 4 + 2 * Cl) {
+          if (tid < 4 + 2 * C) {
             unsigned long long v;
-            if (tid == 0) v = (unsigned long long)kbest | ((unsigned long long)Cl << 32);
+            if (tid == 0) v = (unsigned long long)kbest | ((unsigned long long)C << 32);
             else if (tid == 1) v = T;
             else if (tid == 2) v = Tlist;
             else if (tid == 3) v = 0ull;
@@ -696,11 +653,9 @@ __global__ void __launch_bounds__(LEAN_THREADS, 1) ccsim_wave_multi_kernel(const
             st_slot_sys(dst + tid, v | tagbits);
           }
         }
-      __syncthreads();                                                  // X0: the local candidates are in registers / on their way
-      if (tid == 0) ms.ncand = 0;
       uint32_t xkb = kbest, xtl = Tlist, xbar = T;
       if (tid < p.world) {
-        int cr = 0;
+        int cr = C;
         if (tid != p.rank && !dead) {
           unsigned long long h[3];
           multi_poll_sys(p.xslots_peer[p.rank] + XLINES_OFF + ((size_t)xpar * CCSIM_MAX_WORLD + tid) * CCSIM_MAX_GRID * SLOT_STRIDE, tag, h);
@@ -717,73 +672,35 @@ __global__ void __launch_bounds__(LEAN_THREADS, 1) ccsim_wave_multi_kernel(const
       dead = ms.dead != 0;
       kbest = ms.xglob[0]; Tlist = ms.xglob[1];
       T = max(ms.xglob[2], kbest > delta ? kbest - delta : 0u);
-      // the other ranks' candidates: entry e of the concatenated summaries -> (rank, index); <= 2 per thread
-      uint32_t rkey[MULTI_XPT]; unsigned long long rpay[MULTI_XPT];
-      #pragma unroll
-      for (int u = 0; u < MULTI_XPT; u++) {
-        rkey[u] = 0u; rpay[u] = 0ull;
-        int e = tid + u * LEAN_THREADS, r = 0;
-        while (r < p.world && e >= ms.xcount[r]) { e -= ms.xcount[r]; r++; }
-        if (r < p.world && !dead) {
-          unsigned long long w[2];
-          multi_poll_sys(p.xslots_peer[p.rank] + XLINES_OFF + ((size_t)xpar * CCSIM_MAX_WORLD + r) * CCSIM_MAX_GRID * SLOT_STRIDE + 4 + 2 * e, tag, w);
-          rkey[u] = (uint32_t)w[0]; rpay[u] = w[1];
+      C = 0;
+      if (!dead) {
+        // entry e of the concatenated summaries -> (rank, index). This rank's own segment comes from the candidate arrays, which the
+        // compaction stores over after its first barrier only.
+        #pragma unroll
+        for (int u = 0; u < MULTI_EPT; u++) {
+          ea[u] = eb[u] = 0ull;
+          int e = tid + u * LEAN_THREADS, r = 0;
+          while (r < p.world && e >= ms.xcount[r]) { e -= ms.xcount[r]; r++; }
+          if (r == p.rank) {
+            ea[u] = ms.ckey[e];
+            eb[u] = (unsigned long long)ms.cdom[e] | ((unsigned long long)ms.cnext[e] << MULTI_NEXT_SHIFT);
+          } else if (r < p.world) {
+            unsigned long long w[2];
+            multi_poll_sys(p.xslots_peer[p.rank] + XLINES_OFF + ((size_t)xpar * CCSIM_MAX_WORLD + r) * CCSIM_MAX_GRID * SLOT_STRIDE + 4 + 2 * e, tag, w);
+            ea[u] = w[0]; eb[u] = w[1];
+          }
         }
-      }
-      for (int pass = 0; pass < 2; pass++) {
-        multi_append(lkey != 0u && lkey >= T, lkey, lpay, lane);
-        #pragma unroll
-        for (int u = 0; u < MULTI_XPT; u++) multi_append(rkey[u] != 0u && rkey[u] >= T, rkey[u], rpay[u], lane);
-        __syncthreads();                                                // X2
-        C = ms.ncand;
-        if (C <= MULTI_CAP || pass == 1) break;
-        if (tid < MULTI_BINS) ms.hist[tid] = 0u;
-        __syncthreads();
-        const unsigned long long range = (unsigned long long)(kbest - T) + 1ull;
-        multi_hist_add(lkey, T, range);
-        #pragma unroll
-        for (int u = 0; u < MULTI_XPT; u++) multi_hist_add(rkey[u], T, range);
-        multi_bar_reset(cta);
-        __syncthreads();
-        T = multi_raise_bar(T, kbest, range);
+        C = multi_compact(ea, eb, T, kbest, cta);
       }
       dead = dead || ms.dead != 0;
     }
-    const bool overflowed = C > MULTI_CAP || T > max(Tlist, kbest > delta ? kbest - delta : 0u);
-    if (C > MULTI_CAP) C = MULTI_CAP;     // (cannot happen after the second pass: the raised T admits <= MULTI_CAP keys)
+    const bool overflowed = T > max(Tlist, kbest > delta ? kbest - delta : 0u);
     if (cta == 0 && tid == 0) ms.st_cand += C;
     MPH_MARK(3);
     // ---- key order (single-use templates): no candidate comes back after it wins, so its key stands for the whole wave and the
-    //      winner of every round is the first live candidate in key order. One GPU: the compaction stored them in key order. Node
-    //      shards: the second gather level appends them unordered, so the block ranks them (the other warps only wait at R): rank =
-    //      the number of greater keys (keys are unique), counted by MULTI_RANK_PARTS threads per candidate over one span of the array
-    //      each, then cnext[rank] = candidate. CCSIM_DEBUG_FLAGS bit 6 keeps the arg-max round. ----
+    //      winner of every round is the first live candidate in key order, the order the compaction stored them in.
+    //      CCSIM_DEBUG_FLAGS bit 6 keeps the arg-max round. ----
     const bool key_order = ms.single_use != 0 && !(p.debug_flags & DBG_ARGMAX_ROUND) && !dead;     // (block-uniform)
-    if (XGPU && key_order) {
-      const int i = tid % MULTI_CAP, part = tid / MULTI_CAP;
-      if (i < C && part < MULTI_RANK_PARTS) {
-        const uint32_t mine = ms.ckey[i];
-        const int span = ((C + MULTI_RANK_PARTS - 1) / MULTI_RANK_PARTS + 3) & ~3;     // (<= MULTI_RANK_SPAN)
-        const int j0 = part * span, j1 = min(j0 + span, C);
-        int r = 0, j = j0;
-        #pragma unroll 2
-        for (; j + 4 <= j1; j += 4) {
-          const uint4 v = *reinterpret_cast<const uint4 *>(&ms.ckey[j]);
-          r += (int)(v.x > mine) + (int)(v.y > mine) + (int)(v.z > mine) + (int)(v.w > mine);
-        }
-        for (; j < j1; j++) r += (int)(ms.ckey[j] > mine);
-        ms.kpart[part][i] = (uint8_t)r;
-      }
-      __syncthreads();                                                  // K1
-      if (tid < C) {
-        int r = 0;
-        #pragma unroll
-        for (int q = 0; q < MULTI_RANK_PARTS; q++) r += ms.kpart[q][tid];
-        ms.cnext[r] = (uint32_t)tid;
-      }
-      __syncthreads();                                                  // K2
-      RPROF(if (warp == 0) RP_ADD(RP_RANK, clock64() - ms.tc0, 1);)
-    }
     // ---- replay: the reference cycles k, k+1, ... this wave can decide; every CTA does the same, in ONE warp and without a
     //      barrier: MULTI_CPT candidates per lane in registers, lane q < n_gt also owns counter term q (its constants, and the
     //      minimum / multiplicity of the PTS constraint it tracks, stay in registers for the whole wave) ----
@@ -945,9 +862,8 @@ __global__ void __launch_bounds__(LEAN_THREADS, 1) ccsim_wave_multi_kernel(const
             __syncwarp();                      // the counter cells / limits written by the term lanes, before every lane reads them
             const int idx = row * 32 + lane;
             const bool present = idx < C;
-            const uint32_t o = !present ? 0u : (XGPU ? (uint32_t)lds_s32(MS_SA(cnext) + 4u * (uint32_t)idx) : (uint32_t)idx);   // (node shards: ranked)
-            kk = present ? (uint32_t)lds_s32(MS_SA(ckey) + 4u * o) : 0u;
-            kd = present ? (uint32_t)lds_s32(MS_SA(cdom) + 4u * o) : 0u;   // (0: no field, every cell read is cell 0 of its counter)
+            kk = present ? (uint32_t)lds_s32(MS_SA(ckey) + 4u * (uint32_t)idx) : 0u;
+            kd = present ? (uint32_t)lds_s32(MS_SA(cdom) + 4u * (uint32_t)idx) : 0u;   // (0: no field, every cell read is cell 0 of its counter)
             // the full cell test. The term constants come from the term lanes' registers (lane q holds term q's current limit;
             // lanes >= n_gt hold zeros: no field, cell 0 of the first counter), so nothing here branches and every load is
             // issued before its first use.
@@ -1130,7 +1046,7 @@ __global__ void __launch_bounds__(LEAN_THREADS, 1) ccsim_wave_multi_kernel(const
         printf("wave %lld k=%lld acc=%d C=%d T=%08x Tlist=%08x kbest=%08x delta=%08x ran_dry=%d look_ahead=%d first=%d last=%d\n", wv, k, acc, C, T, Tlist, kbest, delta,
                (int)ran_dry, (int)any_relax, acc ? ms.acc_node[0] : -1, acc ? ms.acc_node[acc - 1] : -1);
       if (lane == 0) {
-        ms.accepted = acc; ms.ncand = 0;
+        ms.accepted = acc;
         // next wave's bar distance: the replay ran out of candidates above a bar that was higher than it had to be -> look further
         // down next time; far more candidates than a wave uses -> look less far
         uint32_t nd = delta;

@@ -36,6 +36,27 @@ if __name__ == "__main__":
         probe("C4 spread-only", snap, tmpl, ctr[:3], 20000, 92)
         probe("C4 spread-only, sequential", snap, tmpl, ctr[:3], 20000, 92, abi.ENGINE_SEQUENTIAL)
     if "c5" in which: probe("C5 1M x 64 templates", *synth.c5(), 6400, 72)
+    if "sharded" in which:       # multi<true>: C4-small over node shards, the ranks as handles of this process on device 0 connected
+        sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests"))
+        import helpers           # by pointer (tests/helpers.py); a run lasts as long as its slowest rank
+        snap, tmpl, ctr = synth.c4(n=30000, n_existing=60000, zones=32, racks=256, regions=8)
+        for world in (2, 4):
+            engs = helpers.sharded_engines(snap, tmpl, ctr, world, abi.ENGINE_AUTO)
+            try:
+                for _ in range(2):
+                    helpers.run_sharded_once(engs, 0)
+                ms = []
+                for _ in range(5):
+                    res = helpers.run_sharded_once(engs, 0)
+                    ms.append(max(r.run_ms for r in res))
+                st = engs[0].run_stats()
+            finally:
+                for e in engs:
+                    e.close()
+            w = max(1, st["waves"])
+            print("%-28s world=%d %s placed=%d waves=%d candidates/wave=%.1f bar raised in %d waves  run %.3f-%.3f ms (5 runs)  pod->node sha1 %s" % (
+                "C4-small node shards", world, st["kernel"], st["placed"], st["waves"], st["candidates"] / w, st["bar_raised_waves"], min(ms), max(ms),
+                hashlib.sha1(res[0].pod_node.tobytes()).hexdigest()[:16]), flush=True)
     if "generic" in which:       # the generic wave kernel, which bench.py never reaches: normalised soft scorers and eight
         sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests"))
         import helpers           # PreferNoSchedule classes with an extended-resource request, resident and one node past the tile

@@ -3,7 +3,7 @@ into waves the way ccsim_multi.cuh does — per-tile top-M publication, the bar 
 across non-binding PTS minimum moves — and reports placements per wave and why waves end, for alternative tile layouts / M / caps.
 
     python scripts/wave_sim.py [--layout contiguous|interleaved] [--m 16] [--cap 256] [--nodelta] [--waves N] [--relax a,b,c]
-                               [--bar exact|hist] [--levels L]
+                               [--levels L]
     KNUM=8 RMAX=3 CF=1 python scripts/wave_sim.py        # the look-ahead rule ccsim_multi.cuh ships (MULTI_RELAX_K / MULTI_RELAX_R)
 The placement sequence goes to $WAVE_SIM_OUT (.npy).
 
@@ -27,8 +27,6 @@ ap.add_argument("--racks", type=int, default=1024)
 ap.add_argument("--regions", type=int, default=8)
 ap.add_argument("--perdomain", type=int, default=-1, help="publish the best node per open domain of this constraint (0 zone, 1 rack, 2 region) instead of the top-M")
 ap.add_argument("--relax", default="0,0,0", help="look-ahead per constraint: nodes whose cell is at most this far over the limit are published as dormant candidates")
-ap.add_argument("--bar", default="exact", choices=("exact", "hist"), help="more than --cap candidates: the bar is the key of rank cap-1 (exact), or the "
-                "lowest of 64 equal steps between the bar and the best key that leaves <= cap (hist: the kernel before key-order compaction)")
 ap.add_argument("--levels", type=int, default=4, help="candidates on at most this many score levels below the best key; when they span more, the "
                 "bar goes up to the lowest key of the lowest level kept (0: no limit)")
 args = ap.parse_args()
@@ -128,13 +126,7 @@ while True:
     c_idx = idx[pub & (k >= T)]; c_key = k[pub & (k >= T)]
     if len(c_idx) > args.cap:
         raised += 1
-        if args.bar == "exact":
-            T = int(c_key[args.cap - 1])
-        else:
-            rng_ = kbest - T + 1
-            suf = np.cumsum(np.bincount((c_key - T) * 64 // rng_, minlength=64)[::-1])[::-1]
-            bsel = int((suf > args.cap).sum())
-            T = kbest if bsel >= 64 else T + (bsel * rng_ + 63) // 64
+        T = int(c_key[args.cap - 1])      # more than --cap candidates: the bar is the key of rank cap-1
         keep = c_key >= T; c_idx = c_idx[keep]; c_key = c_key[keep]
     overflowed = T > T0
     C = len(c_idx); cand_total += C
@@ -183,7 +175,7 @@ h = np.array(hist_acc)
 print("layout=%s M=%d cap=%d nodelta=%s perdomain=%d: placed %d in %d waves = %.2f placements/wave; candidates/wave %.1f; ends %s" % (
     args.layout, args.m, args.cap, args.nodelta, args.perdomain, placed, waves, placed / max(1, waves), cand_total / max(1, waves), ends))
 print("waves without a placement (relaxed scan hid the feasible nodes):", empty_waves)
-print("bar %s: more than %d candidates in %d waves; candidates over %d levels, bar raised in %d waves" % (args.bar, args.cap, raised, args.levels, clamped))
+print("more than %d candidates in %d waves; candidates over %d levels, bar raised in %d waves" % (args.cap, raised, args.levels, clamped))
 print("final R", R, "pen", pen)
 print("rescans by constraint (zone, rack, region):", resc_by)
 print("placements/wave percentiles 10/50/90/max:", np.percentile(h, [10, 50, 90]).tolist(), int(h.max()))
