@@ -224,10 +224,11 @@ __device__ __forceinline__ int nth_set_lane(unsigned m, int g) {
 //      counts (one 64-bit word per group), and every warp sums what it needs of them itself.
 //      At most MULTI_LEVELS levels are ranked: when the candidates span more, the bar goes up to the lowest key of the lowest
 //      level ranked. More than MULTI_CAP candidates: the bar is the key of rank MULTI_CAP - 1. Either bar is above T, and any bar
-//      above T is valid: the best candidate is still in, and a strict wave places it. Returns the candidates stored (<= MULTI_CAP)
-//      and sets T to the bar. The candidate arrays are written after the first barrier only. ----
+//      above T is valid: the best candidate is still in, and a strict wave places it. Returns the candidates stored (<= MULTI_CAP),
+//      sets T to the bar and `over` when there were more than MULTI_CAP (block-uniform; left as it was otherwise, so that the
+//      two gather levels of a node-shard wave raise one flag). The candidate arrays are written after the first barrier only. ----
 __device__ __forceinline__ int multi_compact(const unsigned long long (&ea)[MULTI_EPT], const unsigned long long (&eb)[MULTI_EPT], uint32_t &T,
-                                             const uint32_t kbest, const int cta) {
+                                             const uint32_t kbest, const int cta, bool &over) {
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   GPROF(const long long gp_t = clock64();)
   const uint32_t kbl = kbest >> MULTI_IDX_BITS;
@@ -272,7 +273,7 @@ __device__ __forceinline__ int multi_compact(const unsigned long long (&ea)[MULT
     }
   }
   if (clamp) T = (kbl - (MULTI_LEVELS - 1)) << MULTI_IDX_BITS;
-  if (cta == 0 && tid == 0 && total > MULTI_CAP) ms.st_overflow++;
+  if (total > MULTI_CAP) over = true;
   __syncthreads();                                                  // G3
   if (total > MULTI_CAP) T = ms.ckey[MULTI_CAP - 1];
   GPROF(if (cta == 0 && tid == 0) { ms.gp_cyc[GP_COMPACT] += clock64() - gp_t; ms.gp_cnt[GP_CLAMP] += clamp; })
@@ -628,7 +629,8 @@ __global__ void __launch_bounds__(LEAN_THREADS, 1) ccsim_wave_multi_kernel(const
     //      tile l: a lower list holds lower node indices, which rank higher at the same score. So the concatenated lists are in key
     //      order within every score level ----
     int C = 0;
-    if (!dead) C = multi_compact(ea, eb, T, kbest, cta);
+    bool over = false;        // a gather level had more than MULTI_CAP candidates: the wave counts once in bar_raised_waves
+    if (!dead) C = multi_compact(ea, eb, T, kbest, cta, over);
     if (XGPU) {
       // ---- gather, level 2 (node shards): every rank now holds ITS candidates keyed >= its bar T_r (<= MULTI_CAP of them, the same in
       //      all of its CTAs). One summary per (source, destination) pair crosses NVLink — {best key, count, T_r, T_list_r, the
@@ -690,12 +692,12 @@ __global__ void __launch_bounds__(LEAN_THREADS, 1) ccsim_wave_multi_kernel(const
             ea[u] = w[0]; eb[u] = w[1];
           }
         }
-        C = multi_compact(ea, eb, T, kbest, cta);
+        C = multi_compact(ea, eb, T, kbest, cta, over);
       }
       dead = dead || ms.dead != 0;
     }
     const bool overflowed = T > max(Tlist, kbest > delta ? kbest - delta : 0u);
-    if (cta == 0 && tid == 0) ms.st_cand += C;
+    if (cta == 0 && tid == 0) { ms.st_cand += C; if (over) ms.st_overflow++; }
     MPH_MARK(3);
     // ---- key order (single-use templates): no candidate comes back after it wins, so its key stands for the whole wave and the
     //      winner of every round is the first live candidate in key order, the order the compaction stored them in.
