@@ -49,12 +49,16 @@
 //   20.87-21.01 ms (one H100 80GB HBM3, 700 W power limit). CCSIM_DEBUG_FLAGS bit 6 keeps the arg-max round.
 // Sorted tile (single-use templates): a live node's key does not change during a launch (its row changes only when it wins, and
 //   then it is infeasible for the rest of the run; the replicated counters change feasibility, not scores). So the tile is ranked
-//   by key once per launch, the scan stores every node's key at its node's rank, and the tile's top 16 are its first 16 non-zero
-//   keys: one ballot per warp, a barrier and a prefix count instead of up to 16 REDUX rounds per warp and warp 0's 24-way merge.
-//   The lines are word for word the same. C4: CTA 0's scan + barrier + merge/publish 4 480 -> 2 880 cycles per wave, kernel time
-//   18.75-18.78 -> 17.54-17.56 ms (one H100 80GB HBM3, 700 W power limit). The host picks the instantiation (template parameter
-//   SORTED): the ones without it are the REDUX selection alone, compiled as before this selection existed (every sorted-tile
-//   statement sits behind `if constexpr`), for templates with second lives and CCSIM_DEBUG_FLAGS bit 7.
+//   by key once per launch, and the tile's top 16 are its first 16 feasible ranks: one ballot per warp, a barrier and a prefix
+//   count instead of up to 16 REDUX rounds per warp and warp 0's 24-way merge. The lines are word for word the same. C4: CTA 0's
+//   scan + barrier + merge/publish 4 480 -> 2 880 cycles per wave, kernel time 18.75-18.78 -> 17.54-17.56 ms (one H100 80GB HBM3,
+//   700 W power limit). Everything but the replicated counter cells is fixed between constants builds too (the node-local Filter
+//   verdict: a winner fails it for good; the payload: static), so each rank has a record {key or 0, payload}, rebuilt at every
+//   constants build, and the scan is thread t testing the cells of rank t's record: one barrier before the publish instead of two.
+//   C4: those three phases 2 870 -> 1 940 cycles per wave, kernel time 17.47-17.59 -> 16.80-16.91 ms (same H100, 700 W). The host
+//   picks the instantiation (template parameter SORTED): the ones without it are the REDUX selection alone, compiled as before
+//   this selection existed (every sorted-tile statement sits behind `if constexpr`), for templates with second lives and
+//   CCSIM_DEBUG_FLAGS bit 7.
 // Look-ahead waves: a PodTopologySpread minimum move that REOPENS closed domains would end the wave (the reopened nodes were
 //   rejected by the scan and are in nobody's list). When a term's limit is about to move, the scan publishes the nodes of its
 //   closed cells too; they sit in the replay as dormant candidates (key 0: set-up reads the look-ahead terms' cells) and are
@@ -145,14 +149,8 @@ struct __align__(16) MultiShared {
   uint32_t wtop[LEAN_WARPS][MULTI_M];               // per-warp top-M (compact) keys of this wave
   int32_t gt_c1[MULTI_GT][4];                       // per replicated-counter term: {limit, payload shift, payload mask, domains of the counter}
   int32_t gt_commit[MULTI_GT][4];                   // ... {counter base, inc, PTS constraint tracked or -1, n_present}
-  union {
-    struct {
-      uint32_t ckey[MULTI_CAP], cdom[MULTI_CAP], cnext[MULTI_CAP];   // the wave's candidates keyed >= T, in key order: key, domain
-                                                                     // payload, second-life key
-    };
-    uint32_t skey[LEAN_THREADS];   // sorted tile: this wave's key of the tile node of rank r (0: infeasible), from the scan to the
-                                   // publish; the candidate arrays are written after the gather and read up to barrier R only
-  };
+  uint32_t ckey[MULTI_CAP], cdom[MULTI_CAP], cnext[MULTI_CAP];   // the wave's candidates keyed >= T, in key order: key, domain
+                                                                 // payload, second-life key
   unsigned long long gcnt[MULTI_GROUPS];            // compaction: per group of 32 gathered entries, its candidates per level (16 bits each)
   uint32_t red[LEAN_WARPS], red2[LEAN_WARPS];       // block reductions (T, best key)
   int32_t wfeas[LEAN_WARPS];
@@ -177,12 +175,16 @@ struct __align__(16) MultiShared {
 };
 
 __shared__ MultiShared ms;
-static_assert(offsetof(MultiShared, skey) % 16 == 0 && 3 * MULTI_CAP >= LEAN_THREADS && LEAN_THREADS % 4 == 0 && LEAN_THREADS <= 65536,
-              "sorted tile: the keys fit the candidate arrays, 16-byte loads of them, 16-bit ranks");
-// sorted tile: tile node j's rank in key order (once per launch). Only the sorted instantiation references it, so only its static
-// shared memory holds it (WAVE_KERNELS in ccsim_engine.cu adds it there)
+static_assert(LEAN_THREADS % 2 == 0 && LEAN_THREADS <= 65536, "sorted tile: 16-byte loads of two records, 16-bit ranks");
+// sorted tile: tile node j's rank in key order (once per launch), and the node record of every rank: {the node's key, 0 when the
+// node fails a node-local part of the Filter pass; its payload} (at every constants build). Only the sorted instantiation references
+// them, so only its static shared memory holds them (WAVE_KERNELS in ccsim_engine.cu adds them there)
 __shared__ uint16_t multi_tile_rank[LEAN_THREADS];
-#define MULTI_SORTED_SMEM (sizeof(uint16_t) * LEAN_THREADS)
+__shared__ __align__(16) uint2 multi_tile_rec[LEAN_THREADS];
+// sorted tile: the scan's constants of replicated-counter term q (q < ms.n_gt): {counter base, payload shift, payload mask, limit +
+// look-ahead}, written by the constants build and by the replay warp for the next wave
+__shared__ int4 multi_scan_term[MULTI_GT];
+#define MULTI_SORTED_SMEM ((sizeof(uint16_t) + sizeof(uint2)) * LEAN_THREADS + sizeof(int4) * MULTI_GT)
 
 // the position of entry r (0 = best) of a CTA's list in its key line: the best key and the last key share the line's first 16 bytes
 __device__ __forceinline__ int multi_kpos(int r) { return r == 0 ? 0 : (r == MULTI_M - 1 ? 1 : r + 1); }
@@ -394,6 +396,7 @@ __global__ void __launch_bounds__(LEAN_THREADS, 1) ccsim_wave_multi_kernel(const
                 ms.gt_commit[g][1] = ls.cinfo[j].inc; ms.gt_commit[g][2] = ls.cinfo[j].pts_idx; ms.gt_commit[g][3] = ls.cinfo[j].n_present;
                 ms.gt_c1[g][3] = p.counters[j].n_domains;
               }
+            if constexpr (SORTED) multi_scan_term[g] = make_int4(ls.terms[q].cnt_off, ms.gt_c1[g][1], ms.gt_c1[g][2], ls.terms[q].lim + ms.relax[q]);
             ms.gt_term[g++] = q;
           }
         ms.n_gt = g;
@@ -406,39 +409,71 @@ __global__ void __launch_bounds__(LEAN_THREADS, 1) ccsim_wave_multi_kernel(const
       }
       __syncthreads();
       // ---- single-use templates: the tile in key order, once per launch. A live node's key does not change during the launch: its
-      //      row changes only when it wins, and then it never passes the scan again; the replicated counters decide feasibility,
-      //      not scores. So with every node's key stored at the node's rank (ms.skey), the tile's top M are its first M non-zero
-      //      entries (see the selection below). Keyed exactly as the scan keys them; rank = the number of greater keys (keys are
-      //      unique: the index bits), counted by the node's own thread over the keys staged in ms.skey. The constants builds after
-      //      a minimum move keep the order. ----
-      if (SORTED && wv == 0 && ms.single_use) {     // (device-checked: otherwise this instantiation runs the REDUX selection)
+      //      row changes only when it wins, and then it never passes the Filter pass again; the replicated counters decide
+      //      feasibility, not scores. Rank = the number of greater keys (keys are unique: the index bits), counted by the node's own
+      //      thread over the keys staged in the records. Then, at every constants build (the node-local limits move only here), the
+      //      node's record at its rank: its key if it passes every node-local part of the Filter pass (taints, selector, resources,
+      //      pods, node-local counter terms; a missing topology key where that rejects), else 0, and its payload. The scan below
+      //      tests only the replicated counter cells of the records; a winner's record dies in the hand-off before barrier R. ----
+      if (SORTED && ms.single_use) {     // (device-checked: otherwise this instantiation runs the REDUX selection)
         uint32_t mine = 0u;
+        bool ok = false;
         if (tid < cnt_nodes) {
-          int32_t sc = lean_rec4(t, lp, tid)[LR_SCORE];
+          const int32_t *r4 = lean_rec4(t, lp, tid);
+          const LeanRow w = lean_row(reinterpret_cast<const uint4 *>(r4));
+          ok = lean_fits(w, lean_fit());
+          for (int q = 0; q < ls.n_cmp_terms; q++) {
+            const LeanTerm lt = ls.terms[q];
+            const int32_t v = r4[lt.slot];                     // node-local count, or domain id (< 0: no topology key)
+            ok &= lt.cnt_off < 0 ? v <= lt.lim : (v >= 0 || lt.miss_rejects == 0);
+          }
+          int32_t sc = w.score;
           if (sc < 0) sc = lean_rescore(t, lp, tid);
           mine = ckey(sc, (uint32_t)(p.node_base + lo + tid));
-          ms.skey[tid] = mine;
+          if (wv == 0) multi_tile_rec[tid].x = mine;
         }
-        __syncthreads();
-        if (tid < cnt_nodes) {
-          int r = 0, i = 0;
-          #pragma unroll 2
-          for (; i + 4 <= cnt_nodes; i += 4) {
-            const uint4 v = *reinterpret_cast<const uint4 *>(&ms.skey[i]);
-            r += (int)(v.x > mine) + (int)(v.y > mine) + (int)(v.z > mine) + (int)(v.w > mine);
+        if (wv == 0) {
+          __syncthreads();
+          if (tid < cnt_nodes) {
+            int r = 0, i = 0;
+            #pragma unroll 2
+            for (; i + 2 <= cnt_nodes; i += 2) {
+              const uint4 v = *reinterpret_cast<const uint4 *>(&multi_tile_rec[i]);
+              r += (int)(v.x > mine) + (int)(v.z > mine);
+            }
+            if (i < cnt_nodes) r += (int)(multi_tile_rec[i].x > mine);
+            multi_tile_rank[tid] = (uint16_t)r;
           }
-          for (; i < cnt_nodes; i++) r += (int)(ms.skey[i] > mine);
-          multi_tile_rank[tid] = (uint16_t)r;
+          if (tid == 0) ms.tile_sorted = 1;
+          __syncthreads();
         }
-        if (tid == 0) ms.tile_sorted = 1;
+        if (tid < cnt_nodes) multi_tile_rec[multi_tile_rank[tid]] = make_uint2(ok ? mine : 0u, (uint32_t)c_pay[tid]);
         __syncthreads();
       }
       if (tid == 0) ls.dirty = 0;
     }
-    // ---- fused Filter pass: this thread's node ----
     const bool tile_sel = SORTED && ms.tile_sorted != 0;     // (block-uniform)
-    uint32_t key = 0u;
-    if (tid < cnt_nodes) {
+    uint32_t key = 0u, kpay = 0u;        // (kpay: sorted tile only, the payload of rank tid)
+    if constexpr (SORTED) {
+      if (tile_sel) {
+        // ---- sorted tile: thread t takes the record of rank t and tests the replicated counter cells of its node, the rest of the
+        //      Filter pass is in the record (see the constants build) ----
+        const uint2 rc = tid < cnt_nodes ? multi_tile_rec[tid] : make_uint2(0u, 0u);
+        const int n_gt = ms.n_gt;
+        bool bad = false;
+        #pragma unroll
+        for (int q = 0; q < MULTI_GT; q++)
+          if (q < n_gt) {
+            const int4 tc = multi_scan_term[q];
+            const uint32_t f = (rc.y >> tc.y) & (uint32_t)tc.z;                 // dom + 1 (0: no domain; cell 0 is read and ignored)
+            bad |= (f != 0u) & (smem_cnt[tc.x + max((int32_t)f - 1, 0)] > tc.w);
+          }
+        key = bad ? 0u : rc.x;
+        kpay = rc.y;
+      }
+    }
+    // ---- fused Filter pass: this thread's node ----
+    if (tid < cnt_nodes && !(SORTED && tile_sel)) {
       const int32_t j = tid;
       const int32_t *r4 = lean_rec4(t, lp, j);
       const LeanRow w = lean_row(reinterpret_cast<const uint4 *>(r4));
@@ -456,18 +491,19 @@ __global__ void __launch_bounds__(LEAN_THREADS, 1) ccsim_wave_multi_kernel(const
         if (sc < 0) sc = lean_rescore(t, lp, j);
         key = ckey(sc, (uint32_t)(p.node_base + lo + j));
       }
-      if constexpr (SORTED) { if (tile_sel) ms.skey[multi_tile_rank[j]] = key; }
     }
-    // ---- the warp's M best keys (REDUX rounds; keys are unique, 0 = none). Sorted tile (single-use templates): none here, its keys
-    //      are in ms.skey by rank, see below (its instantiation keeps this loop for a device that finds the template is not single
-    //      use; "sorted" goes into the ballot, not into a branch around the loop: a trip count from a ballot is warp-uniform to the
-    //      compiler, which then puts no divergence check in front of every REDUX) ----
+    // ---- the warp's M best keys (REDUX rounds; keys are unique, 0 = none). Sorted tile (single-use templates): none here, thread t
+    //      holds rank t, and the warp's count of feasible ranks goes to ms.wfeas for the selection below (its instantiation keeps
+    //      this loop for a device that finds the template is not single use; "sorted" goes into the ballot, not into a branch
+    //      around the loop: a trip count from a ballot is warp-uniform to the compiler, which then puts no divergence check in
+    //      front of every REDUX) ----
+    const unsigned fm = __ballot_sync(0xffffffffu, key != 0u);
     {
       uint32_t rem = key;
       bool has = key != 0u;
       if constexpr (SORTED) has = has && !tile_sel;
-      const int nf = __popc(__ballot_sync(0xffffffffu, has));
-      if (lane == 0) ms.wfeas[warp] = nf;
+      const int nf = __popc(SORTED ? __ballot_sync(0xffffffffu, has) : fm);
+      if (lane == 0) ms.wfeas[warp] = __popc(fm);
       if (lane >= nf && lane < MULTI_M) ms.wtop[warp][lane] = 0u;
       // (warp-uniform trip count: no REDUX rounds for entries that do not exist; not unrolled — sixteen predicated REDUX
       //  in a row run out of uniform registers and spill)
@@ -492,21 +528,17 @@ __global__ void __launch_bounds__(LEAN_THREADS, 1) ccsim_wave_multi_kernel(const
       if (tile_sel) {
         // ---- the CTA's M best from the sorted tile: its first M non-zero keys in rank order. Thread t holds rank t; its rank among
         //      the feasible nodes is the feasible nodes of the warps before it plus those of the lanes before it (one count per warp,
-        //      barrier S2). The threads of ranks < M write their entries, threads tid < M past the last one the empty entries: the
+        //      barrier S1). The threads of ranks < M write their entries, threads tid < M past the last one the empty entries: the
         //      same words as the merge below. ----
-        const uint32_t v = tid < cnt_nodes ? ms.skey[tid] : 0u;
-        const unsigned fm = __ballot_sync(0xffffffffu, v != 0u);
-        if (lane == 0) ms.wfeas[warp] = __popc(fm);
-        __syncthreads();                                                  // S2
         const int32_t nfw = lane < LEAN_WARPS ? ms.wfeas[lane] : 0;
         const int32_t total = __reduce_add_sync(0xffffffffu, nfw);
         const int r = __reduce_add_sync(0xffffffffu, lane < warp ? nfw : 0) + __popc(fm & ((1u << lane) - 1u));
         unsigned long long *myslots = p.slots + ((size_t)par * CCSIM_MAX_GRID + cta) * MULTI_LINE_WORDS;
-        if (v != 0u && r < MULTI_M) {
-          unsigned long long kw = (unsigned long long)v;
+        if (key != 0u && r < MULTI_M) {
+          unsigned long long kw = (unsigned long long)key;
           if (r == MULTI_M - 1 && total > MULTI_M) kw |= 1ull << MULTI_MORE_BIT;
           st_slot(&myslots[multi_kpos(r)], kw | tagbits);
-          st_slot(&myslots[SLOT_STRIDE + r], c_pay[ckey_index(v) - (p.node_base + lo)] | tagbits);
+          st_slot(&myslots[SLOT_STRIDE + r], (unsigned long long)kpay | tagbits);
         }
         if (tid < MULTI_M && tid >= total) {
           st_slot(&myslots[multi_kpos(tid)], tagbits);
@@ -1010,11 +1042,17 @@ __global__ void __launch_bounds__(LEAN_THREADS, 1) ccsim_wave_multi_kernel(const
         RPROF(if (cta == 0 && lane == 0) ms.rp_t = clock64();)
         if (cta == 0 && lane == 0) { ms.st_rounds += acc + (int)ran_dry; if (ended_by_rescan) ms.ph[7] += 1; }      // (ph[7]: waves ended by a minimum move that changes verdicts)
         // the winners of this CTA's tile, handed to their threads for the row updates after barrier R (a node may be accepted
-        // twice: second life)
+        // twice: second life). Sorted tile: a winner's record dies here, before R — no barrier separates the row updates after R
+        // from the next scan, which reads the records only
         __syncwarp();
+        // (read again here: `tile_sel` kept live across the replay loop changed its register allocation and cost C4 ~1 200 cycles a wave)
+        const bool kill_rec = SORTED && ms.tile_sorted != 0;
         for (int i = lane; i < acc; i += 32) {
           const int32_t jw = lds_s32(MS_SA(acc_node) + 4u * (uint32_t)i) - (p.node_base + lo);
-          if (jw >= 0 && jw < cnt_nodes) atomicAdd(&ms.mult[jw], 1);
+          if (jw >= 0 && jw < cnt_nodes) {
+            atomicAdd(&ms.mult[jw], 1);
+            if constexpr (SORTED) { if (kill_rec) multi_tile_rec[multi_tile_rank[jw]].x = 0u; }
+          }
         }
         RPROF(__syncwarp(); const long long rp_h1 = clock64(); RP_ADD(RP_HANDOFF, rp_h1 - ms.rp_t, 1);)
         // ---- the next wave's look-ahead, per PTS term on a replicated counter: its limit is about to move (<= MULTI_RELAX_K present
@@ -1037,6 +1075,8 @@ __global__ void __launch_bounds__(LEAN_THREADS, 1) ccsim_wave_multi_kernel(const
           }
           if (p.debug_flags & DBG_LOOKAHEAD_ALWAYS) nrl = (lane < n_gt && gc.z >= 0 && gc.y > 0 && c1.x < INT32_MAX - 2 * MULTI_RELAX_R && !strict_next) ? MULTI_RELAX_R : 0;   // tests: look-ahead on every PTS term, every wave
           if (lane < n_gt) sts_s32(MS_SA(relax) + 4u * (uint32_t)lds_s32(MS_SA(gt_term) + 4u * (uint32_t)lane), nrl);
+          // (sorted tile: the next scan's constants of this lane's term — its limit as the replay left it, and the look-ahead)
+          if constexpr (SORTED) { if (lane < n_gt) multi_scan_term[lane] = make_int4(gc.x, c1.y, c1.z, c1.x + nrl); }
           if (cta == 0 && lane == 0 && acc == 0 && any_relax) ms.st_empty++;
           RPROF(__syncwarp(); RP_ADD(RP_DECIDE, clock64() - rp_h1, 1);)
         }
