@@ -16,6 +16,7 @@ MAX_IPA = 8
 MAX_TOPO_COLS = 16
 MAX_COUNTERS = 24
 MAX_TEMPLATES = 64
+EACH_MAX_ANALYSES = 4096     # CCSIM_EACH_MAX_ANALYSES: templates of ccsim_set_analyses
 MAX_CLASSES = 8
 TAINT_UNSCHEDULABLE_BIT = 63
 

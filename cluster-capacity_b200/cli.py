@@ -3,9 +3,9 @@ top of the GPU path:
 
     python -m cluster-capacity_b200.cli --podspec examples/pod.yaml --snapshot cluster.json [--max-limit N]
            [--exclude-nodes a,b] [--default-config cfg.yaml] [--verbose] [-o json|yaml] [--kubeconfig KUBECONFIG]
-    (--podspec may be repeated or name a directory: several podspecs are simulated round-robin, e.g. the genpod output of 64 namespaces;
-     with --each every podspec is analysed on its own, as if `cluster-capacity --podspec <file>` ran once per file, hard topology
-     spread, required pod (anti-)affinity and hostPorts included)
+    (--podspec may be repeated or name a directory: up to 64 podspecs are simulated round-robin; with --each up to 4096 podspecs,
+     e.g. the genpod output of every namespace, are each analysed on their own, as if `cluster-capacity --podspec <file>` ran once
+     per file, hard topology spread, required pod (anti-)affinity and hostPorts included)
 
 The analysis needs the LISTed Node/Pod/Namespace objects. `--snapshot` takes a JSON/YAML file
 {"nodes": [...], "pods": [...], "namespaces": [...]} (or a directory with nodes.json / pods.json / namespaces.json);
@@ -127,9 +127,9 @@ def main(argv=None):
     ap.add_argument("-o", "--output", default="", help="Output format. One of: json|yaml")
     ap.add_argument("--snapshot", default="", help="Node/Pod/Namespace lists as a file or directory (instead of a live API server)")
     ap.add_argument("--each", action="store_true",
-                    help="Analyse every podspec of --podspec on its own against the same snapshot (one review per podspec, in order; "
-                         "-o json prints them as one JSON array, -o yaml separates them by ---). Podspecs may carry hard topology spread, "
-                         "required pod (anti-)affinity and hostPorts; normalised soft scorers are refused.")
+                    help="Analyse every podspec of --podspec (up to 4096) on its own against the same snapshot (one review per podspec, in "
+                         "order; -o json prints them as one JSON array, -o yaml separates them by ---). Podspecs may carry hard topology "
+                         "spread, required pod (anti-)affinity and hostPorts; normalised soft scorers are refused.")
     ap.add_argument("--device", type=int, default=0)
     a = ap.parse_args(argv)
     if not a.podspec:

@@ -55,6 +55,7 @@ constexpr uint32_t DBG_STRICT_ONLY = 16u;         // strict multi-commit waves o
 constexpr uint32_t DBG_LOOKAHEAD_ALWAYS = 32u;    // look-ahead on every spread term in every wave
 constexpr uint32_t DBG_ARGMAX_ROUND = 64u;        // single-use multi-commit waves keep the arg-max replay round instead of key order
 constexpr uint32_t DBG_REDUX_SELECT = 128u;       // single-use multi-commit waves select each tile's candidates by REDUX rounds and a merge
+constexpr uint32_t DBG_EACH_ONE_PER_CTA = 256u;   // per-analysis runs launch one CTA per analysis however many analyses there are
 
 struct DevParams {
   int32_t n;            // nodes of this shard

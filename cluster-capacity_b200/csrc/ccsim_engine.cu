@@ -198,11 +198,12 @@ static const WaveKernel WAVE_KERNELS[] = {
   {(const void *)ccsim_wave_stream_kernel<2>, "stream<2>", ENG_STREAM, STREAM_BLOCK, sizeof(StreamShared), 0},
   {(const void *)ccsim_each_kernel<false>, "each", ENG_EACH, EACH_THREADS, sizeof(EachShared), 0},   // ccsim_run_each: node-local analyses
   {(const void *)ccsim_each_kernel<true>, "each", ENG_EACH, EACH_THREADS, sizeof(EachShared), 0},    // ... some with counters or hostPorts
+  {(const void *)ccsim_each_packed_kernel, "each<packed>", ENG_EACH, EACH_THREADS, 0, 0},            // ... node-local, more than the CTAs that fit
 };
 enum { WK_WAVE, WK_WAVE_STREAMED, WK_LEAN, WK_LEAN_SAMPLING, WK_BATCHED, WK_MULTI, WK_MULTI_SHARDED, WK_MULTI_SORTED, WK_MULTI_SHARDED_SORTED,
        WK_STREAM /* + mode */,
-       WK_EACH = WK_STREAM + 3, WK_EACH_TERMS };
-static_assert(sizeof(WAVE_KERNELS) / sizeof(WAVE_KERNELS[0]) == WK_EACH_TERMS + 1, "one WAVE_KERNELS entry per WK_* index");
+       WK_EACH = WK_STREAM + 3, WK_EACH_TERMS, WK_EACH_PACKED };
+static_assert(sizeof(WAVE_KERNELS) / sizeof(WAVE_KERNELS[0]) == WK_EACH_PACKED + 1, "one WAVE_KERNELS entry per WK_* index");
 
 struct RunPlan {      // what run_prepare decided, consumed by the launch
   bool valid = false, empty = false;
@@ -607,10 +608,11 @@ static CounterRange counter_range(const ccsim_handle *h, const ccsim_counter &c,
   return r;
 }
 
-// What both setters do first: the state and count checks, then the handle's templates, counters and analyses dropped
-static int begin_templates(ccsim_handle *h, int32_t n_templates) {
+// What both setters do first: the state and count checks (at most max_templates), then the handle's templates, counters and analyses
+// dropped
+static int begin_templates(ccsim_handle *h, int32_t n_templates, int32_t max_templates) {
   if (!h->have_nodes) return fail(h, CCSIM_ESTATE, "ccsim_load_nodes must come first");
-  if (n_templates < 1 || n_templates > CCSIM_MAX_TEMPLATES) return fail(h, CCSIM_EINVAL, "n_templates out of range");
+  if (n_templates < 1 || n_templates > max_templates) return fail(h, CCSIM_EINVAL, "n_templates out of range");
   CK(cudaSetDevice(h->cfg.device));
   free_pool(h, h->tmpl_allocs);
   h->have_templates = false; h->plan.valid = false; h->each_ran = false; h->analyses = false; h->an.clear();
@@ -662,7 +664,7 @@ extern "C" int ccsim_set_templates(ccsim_handle *h, int32_t n_templates, const c
                                    int32_t n_counters, const ccsim_counter *counters) {
   if (!h || !templates) return fail(h, CCSIM_EINVAL, "null argument");
   int rc;
-  if ((rc = begin_templates(h, n_templates))) return rc;
+  if ((rc = begin_templates(h, n_templates, CCSIM_MAX_TEMPLATES))) return rc;
   if (n_counters < 0 || n_counters > CCSIM_MAX_COUNTERS || (n_counters && !counters)) return fail(h, CCSIM_EINVAL, "n_counters out of range");
   if (n_templates > 1 && n_counters > 0)
     return fail(h, CCSIM_EUNSUPPORTED, "PodTopologySpread/InterPodAffinity templates are single-template only");
@@ -767,13 +769,18 @@ static int build_analysis(ccsim_handle *h, int t, const ccsim_template &T, const
     for (int a = 0; a < T.n_aff; a++) place(T.aff_counter[a], COUPLED_AFF_SEL(a));
     for (int a = 0; a < T.n_anti; a++) place(T.anti_counter[a], COUPLED_ANTI_SEL(a));
   }
-  std::vector<int32_t> cls((size_t)n, 0);
-  if (T.score_enable & CCSIM_PL_TAINT_TOLERATION)
+  // every node in class 0 when no node carries a PreferNoSchedule taint or TaintToleration does not score: no per-node pass then
+  const bool one_class = ncls == 1 || !(T.score_enable & CCSIM_PL_TAINT_TOLERATION);
+  std::vector<int32_t> cls(one_class ? 0 : (size_t)n, 0);
+  if (!one_class)
     for (int32_t i = 0; i < n; i++)
       for (int w = 0; w < nd.taint_words; w++) cls[i] += __builtin_popcountll(h->h_taint[(size_t)w * n + i] & nd.taint_prefer[w] & ~T.tol_prefer[w]);
-  std::vector<int32_t> pos((size_t)n), rep, seg_cls;
+  std::vector<int32_t> pos, rep, seg_cls;   // pos empty: every node at its own index
   std::vector<long long> start;
-  if (!E.group_sel) {   // segment c = class c (possibly empty), as many as the cluster has classes
+  if (!E.group_sel && one_class) {
+    for (int c = 0; c < ncls; c++) { start.push_back(c ? n : 0); rep.push_back(0); seg_cls.push_back(c); }
+  } else if (!E.group_sel) {   // segment c = class c (possibly empty), as many as the cluster has classes
+    pos.resize((size_t)n);
     std::vector<long long> at((size_t)ncls + 1, 0);
     for (int32_t i = 0; i < n; i++) at[cls[i] + 1]++;
     for (int c = 0; c < ncls; c++) { at[c + 1] += at[c]; start.push_back(at[c]); rep.push_back(0); seg_cls.push_back(c); }
@@ -783,8 +790,9 @@ static int build_analysis(ccsim_handle *h, int t, const ccsim_template &T, const
     for (int k = 0; k < A.n_topo_cols; k++) if (group_col[k]) gcols.push_back(k);
     const size_t kw = 1 + gcols.size();
     std::vector<int32_t> key((size_t)n * kw);
+    pos.resize((size_t)n);
     for (int32_t i = 0; i < n; i++) {
-      key[(size_t)i * kw] = cls[i];
+      key[(size_t)i * kw] = one_class ? 0 : cls[i];
       for (size_t q = 0; q < gcols.size(); q++) key[(size_t)i * kw + 1 + q] = A.topo[gcols[q]][i];
     }
     std::vector<int32_t> order((size_t)n);
@@ -796,7 +804,7 @@ static int build_analysis(ccsim_handle *h, int t, const ccsim_template &T, const
     for (int32_t r = 0; r < n; r++) {
       const int32_t i = order[r];
       pos[i] = r;
-      if (r == 0 || less(order[r - 1], i)) { start.push_back(r); rep.push_back(i); seg_cls.push_back(cls[i]); }
+      if (r == 0 || less(order[r - 1], i)) { start.push_back(r); rep.push_back(i); seg_cls.push_back(one_class ? 0 : cls[i]); }
     }
   }
   const int32_t G = (int32_t)start.size();
@@ -814,9 +822,10 @@ static int build_analysis(ccsim_handle *h, int t, const ccsim_template &T, const
     cof[(size_t)l * (G + 1) + G] = acc;
   }
   E.n_seg = G;
-  E.port_self = h->w_placed && (T.filter_enable & CCSIM_PL_NODE_PORTS) && (T.flags & CCSIM_TF_HAS_HOST_PORTS) && ((T.port_tmpl_conflict >> t) & 1ull);
+  // the analysis's own bit of port_tmpl_conflict: t mod 64 (one analysis at a time is diagnosed, so the bits of analyses 64 apart never meet)
+  E.port_self = h->w_placed && (T.filter_enable & CCSIM_PL_NODE_PORTS) && (T.flags & CCSIM_TF_HAS_HOST_PORTS) && ((T.port_tmpl_conflict >> (t & 63)) & 1ull);
   bool identity = true;   // then the kernel reads a node's position as its index
-  for (int32_t i = 0; i < n && identity; i++) identity = pos[i] == i;
+  for (int32_t i = 0; i < (int32_t)pos.size() && identity; i++) identity = pos[i] == i;
   long long *d_cof = nullptr; int32_t *d_rep = nullptr, *d_cls = nullptr, *d_pos = nullptr;
   if ((rc = dev_upload<long long>(h, h->tmpl_allocs, &d_cof, cof.data(), cof.size())) ||
       (rc = dev_upload<int32_t>(h, h->tmpl_allocs, &d_rep, rep.data(), rep.size())) ||
@@ -847,7 +856,7 @@ static int build_analyses(ccsim_handle *h, const ccsim_analysis_terms *terms) {
 extern "C" int ccsim_set_analyses(ccsim_handle *h, int32_t n_templates, const ccsim_template *templates, const ccsim_analysis_terms *terms) {
   if (!h || !templates || !terms) return fail(h, CCSIM_EINVAL, "null argument");
   int rc;
-  if ((rc = begin_templates(h, n_templates))) return rc;
+  if ((rc = begin_templates(h, n_templates, CCSIM_EACH_MAX_ANALYSES))) return rc;
   const int32_t n = h->n;
   if (h->cfg.world > 1) return fail(h, CCSIM_EUNSUPPORTED, "per-analysis runs: node-sharded runs (world %d) are not supported", h->cfg.world);
   for (int t = 0; t < n_templates; t++) {   // every analysis validated as ccsim_set_templates validates its template alone
@@ -1319,38 +1328,63 @@ extern "C" int ccsim_run_each(ccsim_handle *h, int64_t max_pods, ccsim_result *o
     terms |= S.terms.n_counters > 0 || S.terms.port_self;
   }
   const int32_t n = h->n;
-  {
-    size_t free_b = 0, total_b = 0;
-    CK(cudaMemGetInfo(&free_b, &total_b));
-    const double seq_bytes = (double)T * (double)cap * 4.0;
-    if (seq_bytes > (double)free_b)
-      return fail(h, CCSIM_EUNSUPPORTED, "per-analysis runs: the sequence buffers (%d x %lld x 4 B = %.2f GiB) exceed free device memory (%.2f GiB)",
-                  T, (long long)cap, seq_bytes / (1 << 30), (double)free_b / (1 << 30));
-  }
-  h->plan = RunPlan();
-  h->each_ran = false;
-  memset(out, 0, sizeof(ccsim_result) * (size_t)T);
+  size_t free_b = 0, total_b = 0;
+  CK(cudaMemGetInfo(&free_b, &total_b));
+  const double seq_bytes = (double)T * (double)cap * 4.0;
+  if (seq_bytes > (double)free_b)
+    return fail(h, CCSIM_EUNSUPPORTED, "per-analysis runs: the sequence buffers (%d x %lld x 4 B = %.2f GiB) exceed free device memory (%.2f GiB)",
+                T, (long long)cap, seq_bytes / (1 << 30), (double)free_b / (1 << 30));
   // tree shape: roots on level L (32^L >= N); levels [1, split) in global memory, [split, L] in shared memory, the lowest split whose
-  // shared levels fit next to the kernel's static structs
+  // shared levels fit in `budget` bytes
   const int L = each_tree_levels(n);
-  const WaveKernel &kern = WAVE_KERNELS[terms ? WK_EACH_TERMS : WK_EACH];
-  int split = 1;
-  size_t smem = 0;
-  for (; split <= L + 1; split++) {
-    smem = 0;
-    for (int l = split; l <= L; l++) smem += 8 * (size_t)each_level_bound(n, l, nseg);
-    if (smem + kern.static_smem + 1024 <= h->smem_optin) break;
-  }
   EachParams ep; memset(&ep, 0, sizeof(ep));
-  ep.n_levels = L; ep.split = split; ep.max_pods = max_pods; ep.seq_cap = cap;
-  {
+  auto shape = [&](size_t budget) {
+    int split = 1;
+    for (; split <= L + 1; split++) {
+      size_t b = 0;
+      for (int l = split; l <= L; l++) b += 8 * (size_t)each_level_bound(n, l, nseg);
+      if (b <= budget) break;
+    }
     long long g = 0, s = 0;
     for (int l = 1; l <= L; l++) {
       if (l < split) { ep.lev_off[l] = g; g += each_level_bound(n, l, nseg); }
       else { ep.lev_off[l] = s; s += each_level_bound(n, l, nseg); }
     }
-    ep.glev_stride = g;
+    ep.split = split; ep.glev_stride = g; ep.slev_stride = s;
+  };
+  // one CTA per analysis, the shared levels next to the kernel's static structs, while the device holds every CTA at once (and always
+  // for analyses with coupled terms); else node-local analyses share CTAs: A = ceil(T / SMs) of them (<= EACH_MAX_PACK), one warp's
+  // placement loop and one share of the opt-in shared memory each
+  const WaveKernel *kern = &WAVE_KERNELS[terms ? WK_EACH_TERMS : WK_EACH];
+  shape(h->smem_optin - kern->static_smem - 1024);
+  size_t smem = 8 * (size_t)ep.slev_stride;
+  int per_cta = 1;
+  if (!terms) {
+    int resident = 0;   // CTAs of the one-per-analysis launch an SM holds
+    CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&resident, kern->fn, kern->block, smem));
+    const uint32_t dbg = getenv("CCSIM_DEBUG_FLAGS") ? (uint32_t)atoi(getenv("CCSIM_DEBUG_FLAGS")) : 0u;
+    if (T > std::max(1, resident) * h->sm_count && !(dbg & DBG_EACH_ONE_PER_CTA)) {
+      per_cta = std::min<int>(EACH_MAX_PACK, (T + h->sm_count - 1) / h->sm_count);
+      kern = &WAVE_KERNELS[WK_EACH_PACKED];
+      shape((h->smem_optin - 1024 - (size_t)per_cta * sizeof(EachShared)) / (size_t)per_cta);
+      smem = (size_t)per_cta * (sizeof(EachShared) + 8 * (size_t)ep.slev_stride);
+    }
   }
+  const int grid = (T + per_cta - 1) / per_cta;
+  ep.n_levels = L; ep.max_pods = max_pods; ep.seq_cap = cap; ep.pack = per_cta; ep.n_analyses = T;
+  {   // everything the run allocates per analysis, and the topology columns ccsim_set_analyses holds, against free device memory
+    double topo = 0;
+    for (int t = 0; t < T; t++) topo += (double)h->an[t].n_topo * n * 4.0;
+    const double need = (double)T * ((double)n * 12.0 + (double)ep.glev_stride * 8.0 + (double)cap * 4.0 + sizeof(EachOut) + sizeof(DevOut)) + topo;
+    if (need > (double)free_b)
+      return fail(h, CCSIM_EUNSUPPORTED, "per-analysis runs: the per-analysis device state (%d analyses x %d nodes: clone counts and leaves, tree levels, "
+                  "sequences, diagnosis outputs, topology columns = %.2f GiB) exceeds free device memory (%.2f GiB)",
+                  T, n, need / (1 << 30), (double)free_b / (1 << 30));
+  }
+  h->plan = RunPlan();
+  h->each_ran = false;
+  memset(out, 0, sizeof(ccsim_result) * (size_t)T);
+  const int split = ep.split;
   free_pool(h, h->each_allocs);
   const size_t tn = (size_t)T * (size_t)n;
   if ((rc = dev_alloc<int32_t>(h, h->each_allocs, &ep.k, tn)) || (rc = dev_alloc<unsigned long long>(h, h->each_allocs, &ep.leaf, tn)) ||
@@ -1376,7 +1410,7 @@ extern "C" int ccsim_run_each(ccsim_handle *h, int64_t max_pods, ccsim_result *o
     CK(cudaMemsetAsync(d_diag, 0, sizeof(DevOut) * (size_t)T, s));
     void *args[] = { (void *)&p, (void *)&ep };
     CK(cudaEventRecord(h->ev0, s));
-    CK(cudaLaunchKernel(kern.fn, dim3(T), dim3(kern.block), args, smem, s));
+    CK(cudaLaunchKernel(kern->fn, dim3(grid), dim3(kern->block), args, smem, s));
     h->launches++;
     CK(cudaEventRecord(h->ev1, s));
     CK(cudaMemcpyAsync(eo.data(), ep.out, sizeof(EachOut) * (size_t)T, cudaMemcpyDeviceToHost, s));
@@ -1429,12 +1463,13 @@ extern "C" int ccsim_run_each(ccsim_handle *h, int64_t max_pods, ccsim_result *o
     r.pod_node = h->each_seq[t].data();
     waves += r.waves; placed += r.placed;
   }
-  h->plan.kern = &kern;
+  h->plan.kern = kern;
   memset(h->last_stat, 0, sizeof(h->last_stat));
   h->last_stat[0] = ENG_EACH; h->last_stat[1] = waves; h->last_stat[2] = placed;
   h->last_stat[3] = std::min(split - 1, L); h->last_stat[4] = L - std::min(split - 1, L);   // upper tree levels in global / shared memory
-  h->last_stat[5] = T; h->last_stat[6] = kern.block; h->last_stat[7] = (int64_t)smem;
+  h->last_stat[5] = grid; h->last_stat[6] = kern->block; h->last_stat[7] = (int64_t)smem;
   h->last_stat[8] = rebuilds;                                                                 // leaf and level rebuilds, all analyses
+  h->last_stat[9] = per_cta;                                                                  // analyses per CTA
   h->last_key_order_waves = 0;
   h->last_sorted_tile_waves = 0;
   h->each_ran = true;

@@ -172,77 +172,82 @@ static void shl256(const uint64_t in[CCSIM_MAX_STATIC_WORDS], int off, uint64_t 
 }
 
 // Several templates against one snapshot (the roadmap's "list of pods", README.md:305-306; template index = k % T,
-// report.go:160): every template is encoded on its own, then the snapshots are merged — node state and the taint dictionary do
-// not depend on the template; the static predicate bits of template t move up by the bits of templates 0..t-1; extended
-// resources are the union. A list handle's run is one run: per-domain counters (PodTopologySpread / InterPodAffinity terms) stay
-// single-template there. A per-analysis handle (h->each) keeps every part's counters, counter inits, topology columns and PreFilter
-// message as that analysis's own (h->parts), and its hostPort self-conflict becomes bit t.
+// report.go:160): the podspec-independent part of the encoding (node order, NodeInfo columns, taint dictionary: Cluster) is built
+// once, every template is encoded against it, and the encodings are merged: the static predicate bits of template t move up by the
+// bits of templates 0..t-1; extended resources are the union. A list handle's run is one run: per-domain counters (PodTopologySpread
+// / InterPodAffinity terms) stay single-template there. A per-analysis handle (h->each) keeps every part's counters, counter inits,
+// topology columns and PreFilter message as that analysis's own (h->parts), and its hostPort self-conflict becomes bit t mod 64.
+// Each template's static bits and extended-resource columns fold into the merged ones as soon as it is encoded, so the parts held
+// at once are the small ones whatever the number of templates.
 static void encode_list(cc_handle *h) {
   const size_t T = h->tmpls.size();
+  const auto t0 = std::chrono::steady_clock::now();
+  Cluster cluster(h->nodes, h->pods, h->exclude);
+  const auto t1 = std::chrono::steady_clock::now();
+  const int n = cluster.n();
   std::vector<Encoded> &parts = h->parts;
   parts.clear();
   parts.reserve(T);
+  std::vector<std::string> names;                               // extended resources: union of the names the templates request
+  std::vector<std::vector<int64_t>> alloc_scalar, req_scalar;   // ... and their columns
+  std::vector<int> off(T, 0), nbits(T, 0);                      // static bits: template t's bits start at off[t]
+  int total = 0;
+  std::vector<uint64_t> smask((size_t)CCSIM_MAX_STATIC_WORDS * n, 0);   // the merged static bits (word-major), while they fit
   for (size_t t = 0; t < T; t++) {
-    Encoder enc(h->cfg, h->tmpls[t], h->nodes, h->pods, h->ns_labels, h->exclude);
+    Encoder enc(h->cfg, h->tmpls[t], cluster, h->ns_labels);
     enc.set_workloads(&h->workloads);
     parts.push_back(enc.encode());
-    const Encoded &e = parts.back();
-    if (h->each) continue;
-    if (!e.counters.empty()) throw Unsupported("several podspecs of which one has topology spread / pod (anti-)affinity terms or scores (single podspec only)");
-    if (!e.prefilter_msg.empty()) throw Unsupported("several podspecs of which one is rejected by PreFilter");
-    if (e.has_placed_mask) throw Unsupported("several podspecs with hostPorts");
-  }
-  Encoded &m = h->enc;
-  m = parts[0];
-  const int n = m.n;
-  // extended resources: union of the names the templates request
-  std::vector<std::string> names;
-  for (auto &e : parts) for (auto &s : e.scalar_names) if (std::find(names.begin(), names.end(), s) == names.end()) names.push_back(s);
-  if (names.size() > CCSIM_MAX_SCALARS) throw Unsupported("the podspecs request more than 4 distinct extended resources");
-  m.scalar_names = names;
-  m.alloc_scalar.assign(names.size(), std::vector<int64_t>(n, 0));
-  m.req_scalar.assign(names.size(), std::vector<int64_t>(n, 0));
-  for (size_t k = 0; k < names.size(); k++)
-    for (auto &e : parts) {
-      auto it = std::find(e.scalar_names.begin(), e.scalar_names.end(), names[k]);
-      if (it == e.scalar_names.end()) continue;
-      m.alloc_scalar[k] = e.alloc_scalar[it - e.scalar_names.begin()]; m.req_scalar[k] = e.req_scalar[it - e.scalar_names.begin()];
-      break;
+    Encoded &e = parts.back();
+    if (!h->each) {
+      if (!e.counters.empty()) throw Unsupported("several podspecs of which one has topology spread / pod (anti-)affinity terms or scores (single podspec only)");
+      if (!e.prefilter_msg.empty()) throw Unsupported("several podspecs of which one is rejected by PreFilter");
+      if (e.has_placed_mask) throw Unsupported("several podspecs with hostPorts");
     }
-  // static bits: template t's bits start at off[t]
-  std::vector<int> off(T, 0), nbits(T, 0);
-  int total = 0;
-  for (size_t t = 0; t < T; t++) {
+    for (size_t k = 0; k < e.scalar_names.size(); k++)
+      if (std::find(names.begin(), names.end(), e.scalar_names[k]) == names.end()) {
+        names.push_back(e.scalar_names[k]); alloc_scalar.push_back(std::move(e.alloc_scalar[k])); req_scalar.push_back(std::move(e.req_scalar[k]));
+      }
+    e.alloc_scalar.clear(); e.req_scalar.clear();
     // the bits a template really uses: highest set bit over its columns (an encoder allocates them densely from 0)
     int hi = 0;
-    for (int w = 0; w < parts[t].static_words; w++) {
+    for (int w = 0; w < e.static_words; w++) {
       uint64_t acc = 0;
-      for (int i = 0; i < n; i++) acc |= parts[t].static_mask[(size_t)w * n + i];
-      const ccsim_template &P = parts[t].tmpl;
+      for (int i = 0; i < n; i++) acc |= e.static_mask[(size_t)w * n + i];
+      const ccsim_template &P = e.tmpl;
       acc |= P.sel_mask[w] | P.port_static_mask[w] | P.existing_anti_mask[w];
       for (int k = 0; k < CCSIM_MAX_AFF_TERMS; k++) acc |= P.aff_term_mask[k][w] | P.pref_mask[k][w];
       if (acc) hi = w * 64 + 64 - __builtin_clzll(acc);
     }
-    if (parts[t].tmpl.prefilter_bit >= 0) hi = std::max(hi, parts[t].tmpl.prefilter_bit + 1);
-    if (parts[t].tmpl.spts_ignored_bit >= 0) hi = std::max(hi, parts[t].tmpl.spts_ignored_bit + 1);
-    for (const ccsim_counter &c : parts[t].counters) if (c.elig_bit >= 0) hi = std::max(hi, c.elig_bit + 1);
-    for (int c = 0; c < parts[t].tmpl.n_spts; c++) if (parts[t].tmpl.spts[c].has_key_bit >= 0) hi = std::max(hi, parts[t].tmpl.spts[c].has_key_bit + 1);
+    if (e.tmpl.prefilter_bit >= 0) hi = std::max(hi, e.tmpl.prefilter_bit + 1);
+    if (e.tmpl.spts_ignored_bit >= 0) hi = std::max(hi, e.tmpl.spts_ignored_bit + 1);
+    for (const ccsim_counter &c : e.counters) if (c.elig_bit >= 0) hi = std::max(hi, c.elig_bit + 1);
+    for (int c = 0; c < e.tmpl.n_spts; c++) if (e.tmpl.spts[c].has_key_bit >= 0) hi = std::max(hi, e.tmpl.spts[c].has_key_bit + 1);
     off[t] = total; nbits[t] = hi; total += hi;
-  }
-  if (total > 64 * CCSIM_MAX_STATIC_WORDS) throw Unsupported("the podspecs need more than 256 static node-predicate bits together");
-  m.static_words = (total + 63) / 64;
-  m.static_mask.assign((size_t)std::max(1, m.static_words) * n, 0);
-  h->enc_tmpls.assign(T, ccsim_template());
-  h->enc_images.assign(T, std::vector<uint8_t>());
-  for (size_t t = 0; t < T; t++) {
-    const Encoded &e = parts[t];
-    if (nbits[t])
+    if (hi && total <= 64 * CCSIM_MAX_STATIC_WORDS)
       for (int i = 0; i < n; i++) {
         uint64_t in[CCSIM_MAX_STATIC_WORDS] = {0, 0, 0, 0}, out[CCSIM_MAX_STATIC_WORDS];
         for (int w = 0; w < e.static_words; w++) in[w] = e.static_mask[(size_t)w * n + i];
         shl256(in, off[t], out);
-        for (int w = 0; w < m.static_words; w++) m.static_mask[(size_t)w * n + i] |= out[w];
+        for (int w = 0; w < CCSIM_MAX_STATIC_WORDS; w++) smask[(size_t)w * n + i] |= out[w];
       }
+    std::vector<uint64_t>().swap(e.static_mask);
+  }
+  const auto t2 = std::chrono::steady_clock::now();
+  if (names.size() > CCSIM_MAX_SCALARS) throw Unsupported("the podspecs request more than 4 distinct extended resources");
+  if (total > 64 * CCSIM_MAX_STATIC_WORDS) throw Unsupported("the podspecs need more than 256 static node-predicate bits together");
+  Encoded &m = h->enc;
+  m = parts[0];
+  cluster.columns_into(m);
+  m.scalar_names = names;
+  m.alloc_scalar = std::move(alloc_scalar);
+  m.req_scalar = std::move(req_scalar);
+  m.static_words = (total + 63) / 64;
+  smask.resize((size_t)std::max(1, m.static_words) * n);
+  m.static_mask = std::move(smask);
+  h->enc_tmpls.assign(T, ccsim_template());
+  h->enc_images.assign(T, std::vector<uint8_t>());
+  for (size_t t = 0; t < T; t++) {
+    const Encoded &e = parts[t];
     ccsim_template P = e.tmpl;
     auto mv = [&](uint64_t (&msk)[CCSIM_MAX_STATIC_WORDS]) { uint64_t o[CCSIM_MAX_STATIC_WORDS]; shl256(msk, off[t], o); memcpy(msk, o, sizeof(o)); };
     mv(P.sel_mask); mv(P.port_static_mask); mv(P.existing_anti_mask);
@@ -252,7 +257,8 @@ static void encode_list(cc_handle *h) {
     for (int c = 0; c < P.n_spts; c++) if (P.spts[c].has_key_bit >= 0) P.spts[c].has_key_bit += off[t];
     if (h->each) {
       for (ccsim_counter &c : parts[t].counters) if (c.elig_bit >= 0) c.elig_bit += off[t];
-      if (P.port_tmpl_conflict & 1ull) P.port_tmpl_conflict = 1ull << t;   // a clone conflicts with the analysis's own clones
+      // a clone conflicts with the analysis's own clones: bit t mod 64 (one analysis at a time is diagnosed, so analyses 64 apart never meet)
+      if (P.port_tmpl_conflict & 1ull) P.port_tmpl_conflict = 1ull << (t & 63);
       parts[t].tmpl = P;
     }
     // extended resources: re-index into the union
@@ -274,18 +280,24 @@ static void encode_list(cc_handle *h) {
       e = std::move(k);
     }
   } else parts.clear();
+  if (getenv("CCHOST_TIMING"))
+    fprintf(stderr, "[cchost] encode: cluster (node order, pod assignment, node columns, taints) %.3f s, %zu podspecs %.3f s, merge %.3f s\n",
+            std::chrono::duration<double>(t1 - t0).count(), T, std::chrono::duration<double>(t2 - t1).count(),
+            std::chrono::duration<double>(std::chrono::steady_clock::now() - t2).count());
 }
 
 static void ensure_encoded(cc_handle *h) {
   if (h->have_enc) return;
   if (h->tmpls.size() > 1 || h->each) { encode_list(h); h->have_enc = true; return; }
   auto t0 = std::chrono::steady_clock::now();
-  Encoder enc(h->cfg, h->tmpl, h->nodes, h->pods, h->ns_labels, h->exclude);
-  enc.set_workloads(&h->workloads);
+  Cluster cluster(h->nodes, h->pods, h->exclude);
   auto t1 = std::chrono::steady_clock::now();
+  Encoder enc(h->cfg, h->tmpl, cluster, h->ns_labels);
+  enc.set_workloads(&h->workloads);
   h->enc = enc.encode();
+  cluster.columns_into(h->enc);
   if (getenv("CCHOST_TIMING"))
-    fprintf(stderr, "[cchost] encode: node order + pod assignment %.3f s, columns / dictionaries / counters %.3f s\n",
+    fprintf(stderr, "[cchost] encode: cluster (node order, pod assignment, node columns, taints) %.3f s, podspec (tolerations, static bits, counters) %.3f s\n",
             std::chrono::duration<double>(t1 - t0).count(), std::chrono::duration<double>(std::chrono::steady_clock::now() - t1).count());
   h->enc_tmpls.assign(1, h->enc.tmpl);
   h->have_enc = true;
@@ -295,10 +307,15 @@ extern "C" const char *cc_last_error(const cc_handle *h) { return h ? h->err.c_s
 
 static std::vector<Json> items_of(const char *text);
 
-static int new_handle(const char *sched_config_json, std::vector<Json> pods, int64_t max_pods, const char *exclude_nodes, int32_t device, cc_handle **out) {
+// each: a per-analysis handle (cc_new_each), up to CCSIM_EACH_MAX_ANALYSES podspecs; else up to CCSIM_MAX_TEMPLATES
+static int new_handle(const char *sched_config_json, std::vector<Json> pods, int64_t max_pods, const char *exclude_nodes, int32_t device, bool each,
+                      cc_handle **out) {
   if (pods.empty()) return fail(nullptr, CC_EINVAL, "no podspec");
-  if (pods.size() > CCSIM_MAX_TEMPLATES) return fail(nullptr, CC_EUNSUPPORTED, "more than 64 podspecs");
+  if (each && pods.size() > CCSIM_EACH_MAX_ANALYSES)
+    return fail(nullptr, CC_EUNSUPPORTED, "more than " + std::to_string(CCSIM_EACH_MAX_ANALYSES) + " podspecs (CCSIM_EACH_MAX_ANALYSES, per-analysis runs)");
+  if (!each && pods.size() > CCSIM_MAX_TEMPLATES) return fail(nullptr, CC_EUNSUPPORTED, "more than 64 podspecs");
   cc_handle *h = new cc_handle();
+  h->each = each;
   try {
     h->cfg = SchedConfig::parse(sched_config_json ? sched_config_json : "");
     for (auto &j : pods) h->tmpls.push_back(Pod::parse(j, /*keep_raw=*/true));
@@ -319,22 +336,22 @@ extern "C" int cc_new(const char *sched_config_json, const char *pod_json, int64
   if (!pod_json || !out) return fail(nullptr, CC_EINVAL, "null argument");
   try {
     std::vector<Json> one; one.push_back(parse_json(pod_json));
-    return new_handle(sched_config_json, std::move(one), max_pods, exclude_nodes, device, out);
+    return new_handle(sched_config_json, std::move(one), max_pods, exclude_nodes, device, false, out);
   } catch (const std::exception &e) { return fail(nullptr, CC_EINVAL, e.what()); }
 }
 
 extern "C" int cc_new_list(const char *sched_config_json, const char *pods_json, int64_t max_pods, const char *exclude_nodes,
                            int32_t device, cc_handle **out) {
   if (!pods_json || !out) return fail(nullptr, CC_EINVAL, "null argument");
-  try { return new_handle(sched_config_json, items_of(pods_json), max_pods, exclude_nodes, device, out); }
+  try { return new_handle(sched_config_json, items_of(pods_json), max_pods, exclude_nodes, device, false, out); }
   catch (const std::exception &e) { return fail(nullptr, CC_EINVAL, e.what()); }
 }
 
 extern "C" int cc_new_each(const char *sched_config_json, const char *pods_json, int64_t max_pods, const char *exclude_nodes,
                            int32_t device, cc_handle **out) {
-  const int rc = cc_new_list(sched_config_json, pods_json, max_pods, exclude_nodes, device, out);
-  if (rc == CC_OK) (*out)->each = true;
-  return rc;
+  if (!pods_json || !out) return fail(nullptr, CC_EINVAL, "null argument");
+  try { return new_handle(sched_config_json, items_of(pods_json), max_pods, exclude_nodes, device, true, out); }
+  catch (const std::exception &e) { return fail(nullptr, CC_EINVAL, e.what()); }
 }
 
 static std::vector<Json> items_of(const char *text) {

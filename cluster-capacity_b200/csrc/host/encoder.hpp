@@ -26,6 +26,7 @@
 #include <string_view>
 #include <cstring>
 #include <functional>
+#include <climits>
 #include "../../../include/ccsim.h"
 #include "objects.hpp"
 
@@ -335,11 +336,12 @@ struct Encoded {
   }
 };
 
-class Encoder {
+// The podspec-independent part of an encoding, built once per handle and shared by the Encoder of every podspec: the node order
+// (nodeTree), the pods of each node, the pods that carry (anti-)affinity terms, the lowest priority among the bound pods, and the
+// node columns and taint dictionary of Encoded (columns_into).
+class Cluster {
  public:
-  Encoder(const SchedConfig &cfg, const Pod &tmpl, const ObjList<Node> &nodes_in, const ObjList<Pod> &pods_in,
-          const std::map<std::string, Labels> &ns_labels, const std::set<std::string> &exclude)
-      : cfg_(cfg), t_(tmpl), ns_labels_(ns_labels) {
+  Cluster(const ObjList<Node> &nodes_in, const ObjList<Pod> &pods_in, const std::set<std::string> &exclude) {
     // ---- node order: nodeTree (zones in first-seen order, round-robin) ----
     std::vector<const Node *> kept;
     for (auto &n : nodes_in) if (exclude.empty() || !exclude.count(n.name)) kept.push_back(&n);
@@ -381,20 +383,131 @@ class Encoder {
       const int32_t *it = node_index_.find(std::string_view(p.node_name));
       if (!it) return;
       where[j] = *it;
-      pflags[j] = (uint8_t)((p.anti_required.empty() ? 0 : 1) | ((p.aff_required.empty() && p.aff_preferred.empty() && p.anti_preferred.empty()) ? 0 : 2) |
-                            (p.priority < t_.priority ? 4 : 0));
+      pflags[j] = (uint8_t)((p.anti_required.empty() ? 0 : 1) | ((p.aff_required.empty() && p.aff_preferred.empty() && p.anti_preferred.empty()) ? 0 : 2));
     });
     pods_on_.build(nodes_.size(), where, pods_in);
     for (size_t j = 0; j < pods_in.size(); j++) {
+      if (where[j] < 0) continue;
+      min_priority_ = std::min(min_priority_, pods_in[j].priority);
       if (!pflags[j]) continue;
       if (pflags[j] & 1) anti_required_pods_.push_back({where[j], &pods_in[j]});
       if (pflags[j] & 2) affinity_term_pods_.push_back({where[j], &pods_in[j]});
-      if (pflags[j] & 4) lower_priority_pod_ = true;
     }
     // node order, then source-list order within a node: the order in which a pass over pods_on_ would meet them (the topology keys of
     // the InterPodAffinity score get their counter slots in first-seen order)
     std::stable_sort(affinity_term_pods_.begin(), affinity_term_pods_.end(), [](auto &a, auto &b) { return a.first < b.first; });
+    columns();
   }
+
+  int n() const { return (int)nodes_.size(); }
+
+  // the node columns and the taint dictionary, moved into `e` (the Cluster has no columns afterwards)
+  void columns_into(Encoded &e) {
+    e.names = std::move(cols_.names);
+    e.alloc_cpu = std::move(cols_.alloc_cpu); e.alloc_mem = std::move(cols_.alloc_mem); e.alloc_eph = std::move(cols_.alloc_eph);
+    e.req_cpu = std::move(cols_.req_cpu); e.req_mem = std::move(cols_.req_mem); e.req_eph = std::move(cols_.req_eph);
+    e.nz_cpu = std::move(cols_.nz_cpu); e.nz_mem = std::move(cols_.nz_mem);
+    e.alloc_pods = std::move(cols_.alloc_pods); e.npods = std::move(cols_.npods);
+    e.taint_words = cols_.taint_words; e.taint_mask = std::move(cols_.taint_mask); e.taint_dict = std::move(cols_.taint_dict);
+    memcpy(e.taint_nosched, cols_.taint_nosched, sizeof(e.taint_nosched)); memcpy(e.taint_prefer, cols_.taint_prefer, sizeof(e.taint_prefer));
+    e.taint_off = std::move(cols_.taint_off); e.taint_list = std::move(cols_.taint_list);
+  }
+
+ private:
+  friend class Encoder;
+  std::vector<const Node *> nodes_;
+  FlatIndex node_index_;   // keys view the Node objects' names (they outlive the encoder)
+  // the pods of every node, in the order of the source list: one offsets array + one pointer array (a counting sort; a
+  // std::vector per node costs one allocation per node on one core)
+  struct PodsOn {
+    struct Range { const Pod *const *b, *const *e; const Pod *const *begin() const { return b; } const Pod *const *end() const { return e; } };
+    std::vector<uint32_t> off;
+    std::vector<const Pod *> ptr;
+    void build(size_t n_nodes, const std::vector<int32_t> &where, const ObjList<Pod> &pods) {
+      off.assign(n_nodes + 1, 0);
+      for (size_t j = 0; j < where.size(); j++) if (where[j] >= 0) off[(size_t)where[j] + 1]++;
+      for (size_t i = 0; i < n_nodes; i++) off[i + 1] += off[i];
+      ptr.resize(off[n_nodes]);
+      std::vector<uint32_t> cur(off.begin(), off.end() - 1);
+      for (size_t j = 0; j < where.size(); j++) if (where[j] >= 0) ptr[cur[(size_t)where[j]]++] = &pods[j];
+    }
+    Range operator[](size_t i) const { return Range{ptr.data() + off[i], ptr.data() + off[i + 1]}; }
+  } pods_on_;
+  std::vector<std::pair<int, const Pod *>> anti_required_pods_, affinity_term_pods_;   // (node index, pod) of the pods with such terms
+  int min_priority_ = INT_MAX;   // the lowest priority among the bound pods (the lower-priority check compares a podspec's with it)
+  Encoded cols_;                 // node columns and taint dictionary (columns_into)
+  // per node: the extended resources its pods request, summed in pod order (a podspec's columns take the names it requests)
+  std::vector<std::vector<std::pair<std::string, int64_t>>> pod_scalars_;
+  int32_t big_alloc_node_ = -1;  // the first node whose cpu or memory allocatable exceeds CCSIM_MAX_SCORED_ALLOCATABLE
+
+  // NodeInfo of every node: Allocatable (SetNode) and Requested / NonZeroRequested / len(Pods) (AddPodInfo), then the taint dictionary
+  void columns() {
+    Encoded &e = cols_;
+    const int n = (int)nodes_.size();
+    e.n = n;
+    e.names.resize(n);
+    auto z64 = [&](std::vector<int64_t> &v) { v.assign(n, 0); };
+    z64(e.alloc_cpu); z64(e.alloc_mem); z64(e.alloc_eph); z64(e.req_cpu); z64(e.req_mem); z64(e.req_eph); z64(e.nz_cpu); z64(e.nz_mem);
+    e.alloc_pods.assign(n, 0); e.npods.assign(n, 0);
+    pod_scalars_.assign(n, {});
+    parallel_for(n, [&](int i) {
+      const Node &nd = *nodes_[i];
+      e.names[i] = nd.name;
+      for (auto &kv : nd.allocatable) {   // NewResource(node.Status.Allocatable)
+        if (kv.first == "cpu") e.alloc_cpu[i] += kv.second.milli_value();
+        else if (kv.first == "memory") e.alloc_mem[i] += kv.second.value();
+        else if (kv.first == "ephemeral-storage") e.alloc_eph[i] += kv.second.value();
+        else if (kv.first == "pods") e.alloc_pods[i] += (int32_t)kv.second.value();
+      }
+      for (auto *p : pods_on_[i]) {
+        PodResource pr = calculate_resource(*p);
+        e.req_cpu[i] += pr.cpu; e.req_mem[i] += pr.mem; e.req_eph[i] += pr.eph;
+        e.nz_cpu[i] += pr.non0_cpu; e.nz_mem[i] += pr.non0_mem;
+        for (auto &kv : pr.scalar) {
+          auto &v = pod_scalars_[i];
+          auto it = std::find_if(v.begin(), v.end(), [&](auto &x) { return x.first == kv.first; });
+          if (it == v.end()) v.push_back(kv); else it->second += kv.second;
+        }
+        e.npods[i] += 1;
+      }
+    });
+    for (int i = 0; i < n && big_alloc_node_ < 0; i++)
+      if (e.alloc_cpu[i] > CCSIM_MAX_SCORED_ALLOCATABLE || e.alloc_mem[i] > CCSIM_MAX_SCORED_ALLOCATABLE) big_alloc_node_ = i;
+    // ---- taints: dictionary in first-seen order ----
+    std::map<Taint, int> tid;
+    for (int i = 0; i < n; i++)
+      for (auto &t : nodes_[i]->taints)
+        if (!tid.count(t)) {
+          int id = (int)e.taint_dict.size();
+          if (id == CCSIM_TAINT_UNSCHEDULABLE_BIT) { e.taint_dict.push_back(Taint{"", "", "__reserved__"}); id++; }   // bit 63 of word 0 is reserved
+          tid[t] = id; e.taint_dict.push_back(t);
+        }
+    taint_overflow_ = e.taint_dict.size() > 64 * CCSIM_MAX_TAINT_WORDS || e.taint_dict.size() > 255;
+    if (taint_overflow_) return;   // (refused by every podspec's encode)
+    e.taint_words = std::max<int>(1, (int)(e.taint_dict.size() + 63) / 64);
+    e.taint_mask.assign((size_t)e.taint_words * n, 0);
+    e.taint_off.assign(n + 1, 0);
+    for (int i = 0; i < n; i++) {
+      for (auto &t : nodes_[i]->taints) { int id = tid[t]; e.taint_mask[(size_t)(id >> 6) * n + i] |= 1ull << (id & 63); e.taint_list.push_back((uint8_t)id); }
+      e.taint_off[i + 1] = (int32_t)e.taint_list.size();
+      if (nodes_[i]->unschedulable) e.taint_mask[i] |= 1ull << CCSIM_TAINT_UNSCHEDULABLE_BIT;
+    }
+    if (e.taint_list.empty()) e.taint_list.push_back(0);
+    for (size_t id = 0; id < e.taint_dict.size(); id++) {
+      const Taint &t = e.taint_dict[id];
+      const int w = (int)id >> 6; const uint64_t b = 1ull << (id & 63);
+      if (t.effect == "NoSchedule" || t.effect == "NoExecute") e.taint_nosched[w] |= b;
+      if (t.effect == "PreferNoSchedule") e.taint_prefer[w] |= b;
+    }
+  }
+  bool taint_overflow_ = false;
+};
+
+class Encoder {
+ public:
+  Encoder(const SchedConfig &cfg, const Pod &tmpl, const Cluster &c, const std::map<std::string, Labels> &ns_labels)
+      : cfg_(cfg), t_(tmpl), ns_labels_(ns_labels), c_(c), nodes_(c.nodes_), pods_on_(c.pods_on_), anti_required_pods_(c.anti_required_pods_),
+        affinity_term_pods_(c.affinity_term_pods_) {}
 
   // Services / RCs / ReplicaSets / StatefulSets of the snapshot: only helper.DefaultSelector reads them (system-default spreading)
   void set_workloads(const std::vector<WorkloadSelector> *w) { workloads_ = w; }
@@ -441,66 +554,34 @@ class Encoder {
     if (fit.cpu == 0 && fit.mem == 0 && fit.eph == 0 && fit.scalar.empty()) T.flags |= CCSIM_TF_FIT_ALL_ZERO;
     if (T.bal_cpu == 0 && T.bal_mem == 0) T.flags |= CCSIM_TF_BALANCED_SKIP;
 
-    // ---- node columns (A1) ----
-    e.names.resize(n);
-    auto z64 = [&](std::vector<int64_t> &v) { v.assign(n, 0); };
-    z64(e.alloc_cpu); z64(e.alloc_mem); z64(e.alloc_eph); z64(e.req_cpu); z64(e.req_mem); z64(e.req_eph); z64(e.nz_cpu); z64(e.nz_mem);
-    e.alloc_pods.assign(n, 0); e.npods.assign(n, 0);
+    // ---- extended-resource columns (A1; the other node columns are the Cluster's) ----
+    const Encoded &C = c_.cols_;
     e.alloc_scalar.assign(e.scalar_names.size(), std::vector<int64_t>(n, 0));
     e.req_scalar.assign(e.scalar_names.size(), std::vector<int64_t>(n, 0));
-    parallel_for(n, [&](int i) {
-      const Node &nd = *nodes_[i];
-      e.names[i] = nd.name;
-      for (auto &kv : nd.allocatable) {   // NewResource(node.Status.Allocatable)
-        if (kv.first == "cpu") e.alloc_cpu[i] += kv.second.milli_value();
-        else if (kv.first == "memory") e.alloc_mem[i] += kv.second.value();
-        else if (kv.first == "ephemeral-storage") e.alloc_eph[i] += kv.second.value();
-        else if (kv.first == "pods") e.alloc_pods[i] += (int32_t)kv.second.value();
-        else for (size_t k = 0; k < e.scalar_names.size(); k++) if (kv.first == e.scalar_names[k]) e.alloc_scalar[k][i] += kv.second.value();
-      }
-      for (auto *p : pods_on_[i]) {
-        PodResource pr = calculate_resource(*p);
-        e.req_cpu[i] += pr.cpu; e.req_mem[i] += pr.mem; e.req_eph[i] += pr.eph;
-        e.nz_cpu[i] += pr.non0_cpu; e.nz_mem[i] += pr.non0_mem;
-        for (size_t k = 0; k < e.scalar_names.size(); k++) { auto it = pr.scalar.find(e.scalar_names[k]); if (it != pr.scalar.end()) e.req_scalar[k][i] += it->second; }
-        e.npods[i] += 1;
-      }
-    });
-    for (int i = 0; i < n; i++) {   // the engine refuses these too, by index; here the node is named
-      if (e.alloc_cpu[i] > CCSIM_MAX_SCORED_ALLOCATABLE)
-        throw Unsupported("node \"" + e.names[i] + "\": cpu allocatable " + std::to_string(e.alloc_cpu[i]) + "m exceeds " +
+    if (!e.scalar_names.empty())
+      parallel_for(n, [&](int i) {
+        for (auto &kv : nodes_[i]->allocatable)
+          for (size_t k = 0; k < e.scalar_names.size(); k++) if (kv.first == e.scalar_names[k]) e.alloc_scalar[k][i] += kv.second.value();
+        for (auto &kv : c_.pod_scalars_[i])
+          for (size_t k = 0; k < e.scalar_names.size(); k++) if (kv.first == e.scalar_names[k]) e.req_scalar[k][i] += kv.second;
+      });
+    if (const int i = c_.big_alloc_node_; i >= 0) {   // the engine refuses these too, by index; here the node is named
+      if (C.alloc_cpu[i] > CCSIM_MAX_SCORED_ALLOCATABLE)
+        throw Unsupported("node \"" + C.names[i] + "\": cpu allocatable " + std::to_string(C.alloc_cpu[i]) + "m exceeds " +
                           std::to_string(CCSIM_MAX_SCORED_ALLOCATABLE) + "m (LeastAllocated's int64 score arithmetic)");
-      if (e.alloc_mem[i] > CCSIM_MAX_SCORED_ALLOCATABLE)
-        throw Unsupported("node \"" + e.names[i] + "\": memory allocatable " + std::to_string(e.alloc_mem[i]) + " exceeds " +
-                          std::to_string(CCSIM_MAX_SCORED_ALLOCATABLE) + " (LeastAllocated's int64 score arithmetic)");
+      throw Unsupported("node \"" + C.names[i] + "\": memory allocatable " + std::to_string(C.alloc_mem[i]) + " exceeds " +
+                        std::to_string(CCSIM_MAX_SCORED_ALLOCATABLE) + " (LeastAllocated's int64 score arithmetic)");
     }
     tick("node columns");
-    // ---- taints: dictionary in first-seen order ----
-    std::map<Taint, int> tid;
-    for (int i = 0; i < n; i++)
-      for (auto &t : nodes_[i]->taints)
-        if (!tid.count(t)) {
-          int id = (int)e.taint_dict.size();
-          if (id == CCSIM_TAINT_UNSCHEDULABLE_BIT) { e.taint_dict.push_back(Taint{"", "", "__reserved__"}); id++; }   // bit 63 of word 0 is reserved
-          tid[t] = id; e.taint_dict.push_back(t);
-        }
-    if (e.taint_dict.size() > 64 * CCSIM_MAX_TAINT_WORDS || e.taint_dict.size() > 255) throw Unsupported("more than 255 distinct taints in the cluster");
-    e.taint_words = std::max<int>(1, (int)(e.taint_dict.size() + 63) / 64);
-    e.taint_mask.assign((size_t)e.taint_words * n, 0);
-    e.taint_off.assign(n + 1, 0);
-    for (int i = 0; i < n; i++) {
-      for (auto &t : nodes_[i]->taints) { int id = tid[t]; e.taint_mask[(size_t)(id >> 6) * n + i] |= 1ull << (id & 63); e.taint_list.push_back((uint8_t)id); }
-      e.taint_off[i + 1] = (int32_t)e.taint_list.size();
-      if (nodes_[i]->unschedulable) e.taint_mask[i] |= 1ull << CCSIM_TAINT_UNSCHEDULABLE_BIT;
-    }
-    if (e.taint_list.empty()) e.taint_list.push_back(0);
+    // ---- taints: the podspec's tolerations of the Cluster's dictionary ----
+    if (c_.taint_overflow_) throw Unsupported("more than 255 distinct taints in the cluster");
     std::vector<Toleration> prefer_tols;   // getAllTolerationPreferNoSchedule (taint_toleration.go:129-137)
     for (auto &tl : t_.tolerations) if (tl.effect.empty() || tl.effect == "PreferNoSchedule") prefer_tols.push_back(tl);
-    for (size_t id = 0; id < e.taint_dict.size(); id++) {
-      const Taint &t = e.taint_dict[id];
+    for (size_t id = 0; id < C.taint_dict.size(); id++) {
+      const Taint &t = C.taint_dict[id];
       const int w = (int)id >> 6; const uint64_t b = 1ull << (id & 63);
-      if (t.effect == "NoSchedule" || t.effect == "NoExecute") { e.taint_nosched[w] |= b; if (tolerations_tolerate(t_.tolerations, t)) T.tol_nosched[w] |= b; }
-      if (t.effect == "PreferNoSchedule") { e.taint_prefer[w] |= b; if (tolerations_tolerate(prefer_tols, t)) T.tol_prefer[w] |= b; }
+      if (t.effect == "NoSchedule" || t.effect == "NoExecute") { if (tolerations_tolerate(t_.tolerations, t)) T.tol_nosched[w] |= b; }
+      if (t.effect == "PreferNoSchedule") { if (tolerations_tolerate(prefer_tols, t)) T.tol_prefer[w] |= b; }
     }
     if (tolerations_tolerate(t_.tolerations, Taint{"node.kubernetes.io/unschedulable", "", "NoSchedule"})) T.flags |= CCSIM_TF_TOLERATES_UNSCHEDULABLE;
 
@@ -927,32 +1008,14 @@ class Encoder {
     return e;
   }
 
-  const std::vector<const Node *> &nodes() const { return nodes_; }
-
  private:
   SchedConfig cfg_;
   const Pod &t_;
   const std::map<std::string, Labels> &ns_labels_;
-  std::vector<const Node *> nodes_;
-  FlatIndex node_index_;   // keys view the Node objects' names (they outlive the encoder)
-  // the pods of every node, in the order of the source list: one offsets array + one pointer array (a counting sort; a
-  // std::vector per node costs one allocation per node on one core)
-  struct PodsOn {
-    struct Range { const Pod *const *b, *const *e; const Pod *const *begin() const { return b; } const Pod *const *end() const { return e; } };
-    std::vector<uint32_t> off;
-    std::vector<const Pod *> ptr;
-    void build(size_t n_nodes, const std::vector<int32_t> &where, const ObjList<Pod> &pods) {
-      off.assign(n_nodes + 1, 0);
-      for (size_t j = 0; j < where.size(); j++) if (where[j] >= 0) off[(size_t)where[j] + 1]++;
-      for (size_t i = 0; i < n_nodes; i++) off[i + 1] += off[i];
-      ptr.resize(off[n_nodes]);
-      std::vector<uint32_t> cur(off.begin(), off.end() - 1);
-      for (size_t j = 0; j < where.size(); j++) if (where[j] >= 0) ptr[cur[(size_t)where[j]]++] = &pods[j];
-    }
-    Range operator[](size_t i) const { return Range{ptr.data() + off[i], ptr.data() + off[i + 1]}; }
-  } pods_on_;
-  std::vector<std::pair<int, const Pod *>> anti_required_pods_, affinity_term_pods_;   // (node index, pod) of the pods with such terms
-  bool lower_priority_pod_ = false;
+  const Cluster &c_;
+  const std::vector<const Node *> &nodes_;
+  const Cluster::PodsOn &pods_on_;
+  const std::vector<std::pair<int, const Pod *>> &anti_required_pods_, &affinity_term_pods_;
   const std::vector<WorkloadSelector> *workloads_ = nullptr;
 
   // helper.DefaultSelector (plugins/helper/spread.go:40-93)
@@ -1000,7 +1063,7 @@ class Encoder {
     if (t_.has_pvc_volume) throw Unsupported("pod uses PersistentVolumeClaim/ephemeral volumes (VolumeBinding/VolumeZone/NodeVolumeLimits/VolumeRestrictions)");
     if (t_.has_resource_claims) throw Unsupported("pod uses resourceClaims (DynamicResources)");
     if (t_.has_scheduling_gates) throw Unsupported("pod has schedulingGates");
-    if (lower_priority_pod_) throw Unsupported("an existing pod has lower priority than the simulated pod (DefaultPreemption would evict it)");
+    if (c_.min_priority_ < t_.priority) throw Unsupported("an existing pod has lower priority than the simulated pod (DefaultPreemption would evict it)");
   }
 };
 

@@ -204,8 +204,8 @@ class Engine:
         st = {"engine": self.ENGINE_NAMES[int(v[0])] if int(v[0]) < len(self.ENGINE_NAMES) else self.EACH_ENGINE, "kernel": self.kernel_name(), "waves": int(v[1]), "placed": int(v[2]),
               "candidates": int(v[3]), "bar_raised_waves": int(v[4]), "grid": int(v[5]), "block": int(v[6]), "smem_bytes": int(v[7]),
               "phase_cycles": [int(x) for x in v[8:16]]}
-        if int(v[0]) == 5:      # per-analysis runs: where the upper levels of the max-trees live, rebuilds of all analyses
-            st["global_levels"], st["shared_levels"], st["rebuilds"] = int(v[3]), int(v[4]), int(v[8])
+        if int(v[0]) == 5:      # per-analysis runs: where the upper levels of the max-trees live, rebuilds of all analyses, analyses per CTA
+            st["global_levels"], st["shared_levels"], st["rebuilds"], st["per_cta"] = int(v[3]), int(v[4]), int(v[8]), int(v[9])
         return st
 
     def key_order_waves(self):

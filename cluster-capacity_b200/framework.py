@@ -201,8 +201,9 @@ def New(kube_scheduler_config, kube_config, simulated_pod, max_pods=0, exclude_n
 
 
 def NewEach(kube_scheduler_config, kube_config, podspecs, max_pods=0, exclude_nodes=(), device=0):
-    """A per-analysis ClusterCapacity over up to 64 podspecs (cc_new_each), for RunEach() only: analysis t is what New(podspec t) +
-    Run() gives, hard topology spread, required pod (anti-)affinity and hostPorts included. Normalised soft scorers (preferred node
+    """A per-analysis ClusterCapacity over up to 4096 podspecs (cc_new_each, CCSIM_EACH_MAX_ANALYSES), for RunEach() only: analysis t
+    is what New(podspec t) + Run() gives, hard topology spread, required pod (anti-)affinity and hostPorts included. The cluster is
+    encoded once for all of them. Normalised soft scorers (preferred node
     affinity, ScheduleAnyway spreading, InterPodAffinity scoring, which a required affinity matching the pod's own labels brings under
     the default hardPodAffinityWeight), node shards and reference sampling are refused by name."""
     h = C.c_void_p()

@@ -54,10 +54,11 @@ int cc_new(const char *sched_config_json, const char *pod_json, int64_t max_pods
  * one of them does not fit or at max_pods. Podspecs with topology-spread / pod-(anti-)affinity terms are single-podspec only. */
 int cc_new_list(const char *sched_config_json, const char *pods_json, int64_t max_pods, const char *exclude_nodes,
                 int32_t device, cc_handle **out);
-/* A per-analysis handle: the arguments of cc_new_list, run with cc_run_each only (cc_run fails with CC_ESTATE). Every podspec keeps
- * its own topology-spread and pod-(anti-)affinity counters, topology columns and hostPorts, so podspecs with hard (DoNotSchedule)
- * spread, required pod (anti-)affinity and hostPorts are analysed like cc_new(podspec t) + cc_run; a podspec PreFilter rejects ends
- * its own analysis with cc_run's message and no placements. */
+/* A per-analysis handle: the arguments of cc_new_list with up to CCSIM_EACH_MAX_ANALYSES (4096) podspecs, run with cc_run_each only
+ * (cc_run fails with CC_ESTATE). Every podspec keeps its own topology-spread and pod-(anti-)affinity counters, topology columns and
+ * hostPorts, so podspecs with hard (DoNotSchedule) spread, required pod (anti-)affinity and hostPorts are analysed like
+ * cc_new(podspec t) + cc_run; a podspec PreFilter rejects ends its own analysis with cc_run's message and no placements. The
+ * podspec-independent part of the encoding (node order, NodeInfo columns, taint dictionary) is built once for all podspecs. */
 int cc_new_each(const char *sched_config_json, const char *pods_json, int64_t max_pods, const char *exclude_nodes,
                 int32_t device, cc_handle **out);
 int cc_sync_with_objects(cc_handle *h, const char *nodes_json, const char *pods_json, const char *namespaces_json);

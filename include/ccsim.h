@@ -46,7 +46,8 @@ extern "C" {
 #define CCSIM_MAX_IPA           8   /* distinct topology keys of required (anti-)affinity   */
 #define CCSIM_MAX_TOPO_COLS     16  /* topology domain-id columns                           */
 #define CCSIM_MAX_COUNTERS      24  /* per-domain counters (PTS + IPA)                      */
-#define CCSIM_MAX_TEMPLATES     64
+#define CCSIM_MAX_TEMPLATES     64  /* templates of ccsim_set_templates (single runs, lists) */
+#define CCSIM_EACH_MAX_ANALYSES 4096 /* templates of ccsim_set_analyses (per-analysis runs) */
 #define CCSIM_MAX_CLASSES       8   /* distinct PreferNoSchedule intolerable-taint counts   */
 
 /* bit 63 of taint word 0 is node.Spec.Unschedulable (nodeunschedulable/node_unschedulable.go:133-150) */
@@ -302,8 +303,11 @@ int  ccsim_run(ccsim_handle *h, int64_t max_pods, ccsim_result *out);
  * pod_node arrays are owned by the handle until the next run. Afterwards ccsim_node_counts(h, t, ...) gives analysis t's counts.
  * After ccsim_set_templates it refuses (CCSIM_EUNSUPPORTED, before any launch) per-domain counters and hostPorts (placed mask): one
  * counter table is one run's; ccsim_set_analyses gives each analysis its own. Always refused: normalised soft scorers, world > 1,
- * reference sampling, a template without NodeResourcesFit when max_pods <= 0, and sequence buffers (n_templates x min(max_pods,
- * free pod slots + 1) x 4 B) larger than the free device memory. */
+ * reference sampling, a template without NodeResourcesFit when max_pods <= 0, sequence buffers (n_templates x min(max_pods,
+ * free pod slots + 1) x 4 B) larger than the free device memory, and then per-analysis device state larger than it (n_templates x
+ * (n_nodes x 12 B of clone counts and leaves + the global tree levels + the sequence + the diagnosis outputs) + every analysis's
+ * topology columns). Node-local analyses that outnumber the CTAs the device holds at once share CTAs, ceil(n_templates / SMs) of
+ * them (at most 16) per CTA, one warp each (ccsim_kernel_name "each<packed>"); ccsim_run_stats gives the CTAs and the analyses per CTA. */
 int  ccsim_run_each(ccsim_handle *h, int64_t max_pods, ccsim_result *out /* [n_templates] */);
 
 /* The per-analysis terms of one template (ccsim_set_analyses): its own counters and topology columns, what ccsim_set_templates and
@@ -316,8 +320,8 @@ typedef struct ccsim_analysis_terms {
 } ccsim_analysis_terms;
 
 /* Templates for per-analysis runs whose coupled terms (hard topology spread, required pod (anti-)affinity, hostPorts) are each
- * analysis's own: template t's pts[].counter, aff_counter[] and anti_counter[] index terms[t].counters, and a hostPort self-conflict
- * is bit t of its port_tmpl_conflict. Validates every analysis as ccsim_set_templates validates one template (CCSIM_EINVAL for
+ * analysis's own: up to CCSIM_EACH_MAX_ANALYSES of them; template t's pts[].counter, aff_counter[] and anti_counter[] index
+ * terms[t].counters, and a hostPort self-conflict is bit t mod 64 of its port_tmpl_conflict (one analysis at a time is diagnosed). Validates every analysis as ccsim_set_templates validates one template (CCSIM_EINVAL for
  * indexes, CCSIM_EUNSUPPORTED for weights), and refuses (CCSIM_EUNSUPPORTED) an analysis with more than CCSIM_EACH_MAX_GROUPS
  * domain groups (DESIGN.md §4.1g). Afterwards ccsim_run_each runs them, each bounded like ccsim_run of its template alone
  * (int32 counters included); ccsim_run and ccsim_prepare fail with CCSIM_ESTATE until the next ccsim_set_templates. */
@@ -355,7 +359,8 @@ int64_t ccsim_kernel_launches(const ccsim_handle *h);  /* kernels launched by th
 /* the wave-kernel instantiation the last ccsim_prepare (or the prepare inside ccsim_run) chose: "wave<true>" / "wave<false>"
  * (generic, tile resident / streamed from global memory), "lean<false>" / "lean<true>" (lean, reference sampling), "batched",
  * "multi<false>" / "multi<true>" (multi-commit, sharded), "stream<0>" / "stream<1>" / "stream<2>" (TMA streaming: every column
- * streamed / with mask columns / resident free columns), "each" (ccsim_run_each). "" before any prepare, after a failed one and for an
+ * streamed / with mask columns / resident free columns), "each" / "each<packed>" (ccsim_run_each: one CTA per analysis / several
+ * node-local analyses per CTA). "" before any prepare, after a failed one and for an
  * empty cluster.
  * Valid after ccsim_prepare alone: no kernel needs to run. The string is static. */
 const char *ccsim_kernel_name(const ccsim_handle *h);
@@ -363,8 +368,9 @@ int  ccsim_flush_l2(ccsim_handle *h);                  /* writes a buffer larger
 /* latency anatomy of the last run (bench.py's roofline block): [0] engine (0 generic, 1 lean sequential, 2 tie-run batching,
  * 3 multi-commit, 4 streaming, 5 per-analysis max-tree) [1] waves [2] placed [3] multi-commit: candidates replayed, summed over waves;
  * per-analysis: upper tree levels in global memory [4] multi-commit: waves that raised the candidate bar; per-analysis: upper tree
- * levels in shared memory [5] grid [6] block [7] dynamic shared memory bytes [8..15] CTA 0's clock cycles per phase, summed
- * over waves (multi-commit: scan, barrier, merge+publish, gather, replay, row updates+recount; 0 for the other engines) */
+ * levels in shared memory [5] grid (CTAs launched) [6] block [7] dynamic shared memory bytes [8..15] CTA 0's clock cycles per phase,
+ * summed over waves (multi-commit: scan, barrier, merge+publish, gather, replay, row updates+recount; 0 for the other engines);
+ * per-analysis: [8] leaf and level rebuilds of all analyses, [9] analyses per CTA */
 int  ccsim_run_stats(const ccsim_handle *h, int64_t out[16]);
 /* waves of the last run that the multi-commit kernel replayed in key order (single-use templates: the candidates ranked once, each
  * winner taken by a ballot); 0 for the other engines, for templates whose winners may come back in their wave, and under
