@@ -5,7 +5,7 @@ top of the GPU path:
            [--exclude-nodes a,b] [--default-config cfg.yaml] [--verbose] [-o json|yaml] [--kubeconfig KUBECONFIG]
     (--podspec may be repeated or name a directory: up to 64 podspecs are simulated round-robin; with --each up to 4096 podspecs,
      e.g. the genpod output of every namespace, are each analysed on their own, as if `cluster-capacity --podspec <file>` ran once
-     per file, hard topology spread, required pod (anti-)affinity and hostPorts included)
+     per file, hard topology spread, required pod (anti-)affinity and hostPorts included; --devices 0,1,... deals them over GPUs)
 
 The analysis needs the LISTed Node/Pod/Namespace objects. `--snapshot` takes a JSON/YAML file
 {"nodes": [...], "pods": [...], "namespaces": [...]} (or a directory with nodes.json / pods.json / namespaces.json);
@@ -131,12 +131,25 @@ def main(argv=None):
                          "order; -o json prints them as one JSON array, -o yaml separates them by ---). Podspecs may carry hard topology "
                          "spread, required pod (anti-)affinity and hostPorts; normalised soft scorers are refused.")
     ap.add_argument("--device", type=int, default=0)
+    ap.add_argument("--devices", default="",
+                    help="With --each: comma-separated CUDA ordinals (e.g. 0,1,2,3) over which the podspecs are dealt, each device running "
+                         "its share in a launch of its own; the reviews are the same as on one device. Replaces --device.")
     a = ap.parse_args(argv)
     if not a.podspec:
         print("Pod spec file is missing")          # Validate (server.go:83-86)
         ap.print_help()
         return 0
     print("Cluster capacity version %s" % VERSION)
+    devices = None
+    if a.devices:
+        if not a.each:
+            print("--devices is valid with --each only")
+            return 0
+        try:
+            devices = [int(d) for d in a.devices.split(",")]
+        except ValueError:
+            print("--devices: not a comma-separated list of CUDA ordinals: %r" % a.devices)
+            return 0
     fw = importlib.import_module("cluster-capacity_b200.framework")
     try:
         files = []
@@ -149,7 +162,7 @@ def main(argv=None):
         objs = load_snapshot(a.snapshot) if a.snapshot else list_from_cluster(a.kubeconfig)
         excl = [x for x in a.exclude_nodes.split(",") if x]
         if a.each:
-            cc = fw.NewEach(load_scheduler_config(a.default_config), None, pods, a.max_limit, excl, device=a.device)
+            cc = fw.NewEach(load_scheduler_config(a.default_config), None, pods, a.max_limit, excl, device=a.device, devices=devices)
         else:
             cc = fw.New(load_scheduler_config(a.default_config), None, pods[0] if len(pods) == 1 else pods, a.max_limit, excl, device=a.device)
         cc.SyncWithClient(fw.ListClient(objs["nodes"], objs["pods"], objs["namespaces"], objs["services"], objs["replicationcontrollers"],

@@ -317,7 +317,7 @@ struct ccsim_handle {
   std::vector<uint64_t> h_taint;              // the loaded taint masks (word-major): the normalisation class of each node
 };
 
-static std::string g_create_err;
+static thread_local std::string g_create_err;   // ccsim_create's error, per thread: several host threads may create engines at once
 
 static int fail(ccsim_handle *h, int code, const char *fmt, ...) {
   char buf[512];

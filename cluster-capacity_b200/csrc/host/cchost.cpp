@@ -8,6 +8,7 @@
 #include <thread>
 #include <mutex>
 #include <exception>
+#include <system_error>
 #include <cstring>
 #include "../../../include/cchost.h"
 #include "encoder.hpp"
@@ -131,7 +132,7 @@ struct cc_handle {
   std::vector<std::vector<uint8_t>> enc_images;   // their ImageLocality columns
   int64_t max_pods = 0;
   std::set<std::string> exclude;
-  int device = 0;
+  std::vector<int32_t> devices;   // CUDA ordinals: one, or the list of a cc_new_each_on handle
   ObjList<Node> nodes;
   ObjList<Pod> pods;
   std::map<std::string, Labels> ns_labels;
@@ -308,8 +309,8 @@ extern "C" const char *cc_last_error(const cc_handle *h) { return h ? h->err.c_s
 static std::vector<Json> items_of(const char *text);
 
 // each: a per-analysis handle (cc_new_each), up to CCSIM_EACH_MAX_ANALYSES podspecs; else up to CCSIM_MAX_TEMPLATES
-static int new_handle(const char *sched_config_json, std::vector<Json> pods, int64_t max_pods, const char *exclude_nodes, int32_t device, bool each,
-                      cc_handle **out) {
+static int new_handle(const char *sched_config_json, std::vector<Json> pods, int64_t max_pods, const char *exclude_nodes,
+                      std::vector<int32_t> devices, bool each, cc_handle **out) {
   if (pods.empty()) return fail(nullptr, CC_EINVAL, "no podspec");
   if (each && pods.size() > CCSIM_EACH_MAX_ANALYSES)
     return fail(nullptr, CC_EUNSUPPORTED, "more than " + std::to_string(CCSIM_EACH_MAX_ANALYSES) + " podspecs (CCSIM_EACH_MAX_ANALYSES, per-analysis runs)");
@@ -321,7 +322,7 @@ static int new_handle(const char *sched_config_json, std::vector<Json> pods, int
     for (auto &j : pods) h->tmpls.push_back(Pod::parse(j, /*keep_raw=*/true));
     h->tmpl = h->tmpls[0];
     h->max_pods = max_pods;
-    h->device = device;
+    h->devices = std::move(devices);
     if (exclude_nodes) {
       std::stringstream ss(exclude_nodes); std::string item;
       while (std::getline(ss, item, ',')) if (!item.empty()) h->exclude.insert(item);
@@ -336,21 +337,31 @@ extern "C" int cc_new(const char *sched_config_json, const char *pod_json, int64
   if (!pod_json || !out) return fail(nullptr, CC_EINVAL, "null argument");
   try {
     std::vector<Json> one; one.push_back(parse_json(pod_json));
-    return new_handle(sched_config_json, std::move(one), max_pods, exclude_nodes, device, false, out);
+    return new_handle(sched_config_json, std::move(one), max_pods, exclude_nodes, {device}, false, out);
   } catch (const std::exception &e) { return fail(nullptr, CC_EINVAL, e.what()); }
 }
 
 extern "C" int cc_new_list(const char *sched_config_json, const char *pods_json, int64_t max_pods, const char *exclude_nodes,
                            int32_t device, cc_handle **out) {
   if (!pods_json || !out) return fail(nullptr, CC_EINVAL, "null argument");
-  try { return new_handle(sched_config_json, items_of(pods_json), max_pods, exclude_nodes, device, false, out); }
+  try { return new_handle(sched_config_json, items_of(pods_json), max_pods, exclude_nodes, {device}, false, out); }
   catch (const std::exception &e) { return fail(nullptr, CC_EINVAL, e.what()); }
 }
 
 extern "C" int cc_new_each(const char *sched_config_json, const char *pods_json, int64_t max_pods, const char *exclude_nodes,
                            int32_t device, cc_handle **out) {
-  if (!pods_json || !out) return fail(nullptr, CC_EINVAL, "null argument");
-  try { return new_handle(sched_config_json, items_of(pods_json), max_pods, exclude_nodes, device, true, out); }
+  return cc_new_each_on(sched_config_json, pods_json, max_pods, exclude_nodes, &device, 1, out);
+}
+
+extern "C" int cc_new_each_on(const char *sched_config_json, const char *pods_json, int64_t max_pods, const char *exclude_nodes,
+                              const int32_t *devices, int32_t n_devices, cc_handle **out) {
+  if (!pods_json || !out || (n_devices > 0 && !devices)) return fail(nullptr, CC_EINVAL, "null argument");
+  if (n_devices < 1) return fail(nullptr, CC_EINVAL, "empty device list");
+  if (n_devices > CC_EACH_MAX_DEVICES)
+    return fail(nullptr, CC_EINVAL, "more than " + std::to_string(CC_EACH_MAX_DEVICES) + " devices (" + std::to_string(n_devices) + ", CC_EACH_MAX_DEVICES)");
+  for (int32_t g = 0; g < n_devices; g++)
+    if (devices[g] < 0) return fail(nullptr, CC_EINVAL, "device list entry " + std::to_string(g) + ": negative CUDA ordinal " + std::to_string(devices[g]));
+  try { return new_handle(sched_config_json, items_of(pods_json), max_pods, exclude_nodes, std::vector<int32_t>(devices, devices + n_devices), true, out); }
   catch (const std::exception &e) { return fail(nullptr, CC_EINVAL, e.what()); }
 }
 
@@ -686,28 +697,35 @@ static std::vector<std::pair<ccsim_config, ccsim_handle *>> g_eng_idle;
 static bool same_engine_cfg(const ccsim_config &a, const ccsim_config &b) {
   return a.device == b.device && a.sampling == b.sampling && a.pct_nodes_to_score == b.pct_nodes_to_score && a.engine == b.engine;
 }
-static ccsim_handle *engine_acquire(const ccsim_config &cfg, int &rc) {
+// The code and message of a failed engine step, before they become a handle's error (the shares of cc_run_each fail on threads of
+// their own)
+struct EngineFailure { int rc = CC_OK; std::string msg; };
+static ccsim_handle *engine_acquire(const ccsim_config &cfg, EngineFailure &f) {
   {
     std::lock_guard<std::mutex> g(g_eng_mu);
     for (size_t i = 0; i < g_eng_idle.size(); i++)
-      if (same_engine_cfg(g_eng_idle[i].first, cfg)) { ccsim_handle *e = g_eng_idle[i].second; g_eng_idle.erase(g_eng_idle.begin() + (long)i); rc = 0; return e; }
+      if (same_engine_cfg(g_eng_idle[i].first, cfg)) { ccsim_handle *e = g_eng_idle[i].second; g_eng_idle.erase(g_eng_idle.begin() + (long)i); return e; }
   }
   ccsim_handle *e = nullptr;
-  rc = ccsim_create(&cfg, &e);
-  return rc ? nullptr : e;
+  if (ccsim_create(&cfg, &e)) { f.rc = CC_EENGINE; f.msg = std::string("ccsim_create: ") + ccsim_last_error(nullptr); return nullptr; }
+  return e;
 }
-static void engine_release(const ccsim_config &cfg, ccsim_handle *e);
-// A libccsim call failed: the engine is destroyed (not reused) and its error becomes the handle's
-static int engine_failed(cc_handle *h, ccsim_handle *eng, const char *what, int rc) {
-  std::string m = std::string(what) + ": " + ccsim_last_error(eng);
+// A libccsim call failed: the engine is destroyed (not reused) and f takes its error
+static void engine_failed(ccsim_handle *eng, const char *what, int rc, EngineFailure &f) {
+  const std::string m = std::string(what) + ": " + ccsim_last_error(eng);
   ccsim_destroy(eng);
-  return rc == CCSIM_EUNSUPPORTED ? fail(h, CC_EUNSUPPORTED, "unsupported on the GPU path: " + m) : fail(h, CC_EENGINE, m);
+  if (rc == CCSIM_EUNSUPPORTED) { f.rc = CC_EUNSUPPORTED; f.msg = "unsupported on the GPU path: " + m; }
+  else { f.rc = CC_EENGINE; f.msg = m; }
 }
+// at most 4 idle engines per device
 static void engine_release(const ccsim_config &cfg, ccsim_handle *e) {
   if (getenv("CCHOST_NO_ENGINE_REUSE")) { ccsim_destroy(e); return; }
   {
     std::lock_guard<std::mutex> g(g_eng_mu);
-    if (g_eng_idle.size() < 4) { g_eng_idle.push_back({cfg, e}); return; }
+    if (std::count_if(g_eng_idle.begin(), g_eng_idle.end(), [&](const auto &x) { return x.first.device == cfg.device; }) < 4) {
+      g_eng_idle.push_back({cfg, e});
+      return;
+    }
   }
   ccsim_destroy(e);
 }
@@ -741,8 +759,9 @@ static std::string stop_reason_of(const Encoded &E, const ccsim_result &res, int
   return "Unschedulable: " + msg + " preemption: " + post;   // simulator.go:332
 }
 
-// The engine of the handle's configuration, loaded with its encoded snapshot and templates. On failure: nullptr, h->err set, rc the code.
-static ccsim_handle *loaded_engine(cc_handle *h, const ccsim_config &cfg, int &rc) {
+// The engine of the handle's configuration, loaded with its encoded snapshot and templates. A per-analysis handle's engine takes the
+// analyses `share` lists (global indexes, increasing): analysis share[l] becomes the engine's analysis l. On failure: nullptr, f set.
+static ccsim_handle *loaded_engine(const cc_handle *h, const ccsim_config &cfg, const std::vector<int32_t> &share, EngineFailure &f) {
   const Encoded &E = h->enc;
   const bool timing = getenv("CCHOST_TIMING") != nullptr;
   auto tlast = std::chrono::steady_clock::now();
@@ -752,35 +771,41 @@ static ccsim_handle *loaded_engine(cc_handle *h, const ccsim_config &cfg, int &r
     fprintf(stderr, "[cchost]   run/%s %.4f s\n", what, std::chrono::duration<double>(now - tlast).count());
     tlast = now;
   };
-  ccsim_handle *eng = engine_acquire(cfg, rc);
-  if (!eng) { rc = fail(h, CC_EENGINE, std::string("ccsim_create: ") + ccsim_last_error(nullptr)); return nullptr; }
+  ccsim_handle *eng = engine_acquire(cfg, f);
+  if (!eng) return nullptr;
   tick("engine (created or taken from the idle list)");
   ccsim_nodes nd; E.fill_nodes(nd);
   const char *what = "ccsim_load_nodes";
+  int rc;
   if (!(rc = ccsim_load_nodes(eng, &nd))) {
     tick("ccsim_load_nodes");
     what = "ccsim_set_templates";
     if (h->each) {   // every analysis with its own counters and columns
       what = "ccsim_set_analyses";
-      std::vector<std::vector<ccsim_counter>> ctr(h->parts.size());
-      std::vector<ccsim_analysis_terms> terms(h->parts.size());
-      for (size_t t = 0; t < h->parts.size(); t++) {
-        const Encoded &e = h->parts[t];
-        ctr[t] = e.counters;
-        for (size_t j = 0; j < ctr[t].size(); j++) ctr[t][j].init = e.counter_init[j].data();
-        ccsim_analysis_terms &a = terms[t];
+      const size_t A = share.size();
+      std::vector<ccsim_template> tm(A);
+      std::vector<std::vector<ccsim_counter>> ctr(A);
+      std::vector<ccsim_analysis_terms> terms(A);
+      for (size_t l = 0; l < A; l++) {
+        const Encoded &e = h->parts[(size_t)share[l]];
+        tm[l] = h->enc_tmpls[(size_t)share[l]];
+        // the hostPort self-conflict: bit (index in the launch) mod 64, as the engine reads it (encode_list set the global index's)
+        if (tm[l].port_tmpl_conflict) tm[l].port_tmpl_conflict = 1ull << (l & 63);
+        ctr[l] = e.counters;
+        for (size_t j = 0; j < ctr[l].size(); j++) ctr[l][j].init = e.counter_init[j].data();
+        ccsim_analysis_terms &a = terms[l];
         memset(&a, 0, sizeof(a));
-        a.n_counters = (int32_t)ctr[t].size(); a.counters = ctr[t].data();
+        a.n_counters = (int32_t)ctr[l].size(); a.counters = ctr[l].data();
         a.n_topo_cols = (int32_t)e.topo.size();
         for (size_t k = 0; k < e.topo.size() && k < CCSIM_MAX_TOPO_COLS; k++) a.topo[k] = e.topo[k].data();
       }
-      if (!(rc = ccsim_set_analyses(eng, (int32_t)h->enc_tmpls.size(), h->enc_tmpls.data(), terms.data()))) { tick(what); return eng; }
+      if (!(rc = ccsim_set_analyses(eng, (int32_t)A, tm.data(), terms.data()))) { tick(what); return eng; }
     } else if (!(rc = ccsim_set_templates(eng, (int32_t)h->enc_tmpls.size(), h->enc_tmpls.data(), (int32_t)E.counters.size(), E.counters.data()))) {
       tick("ccsim_set_templates");
       return eng;
     }
   }
-  rc = engine_failed(h, eng, what, rc);
+  engine_failed(eng, what, rc, f);
   return nullptr;
 }
 
@@ -795,9 +820,9 @@ static int encode_for_run(cc_handle *h) {
   return CC_OK;
 }
 
-static ccsim_config engine_config(const cc_handle *h) {
+static ccsim_config engine_config(const cc_handle *h, int32_t device) {
   ccsim_config cfg; memset(&cfg, 0, sizeof(cfg));
-  cfg.abi_version = CCSIM_ABI_VERSION; cfg.device = h->device; cfg.engine = CCSIM_ENGINE_AUTO; cfg.rank = 0; cfg.world = 1;
+  cfg.abi_version = CCSIM_ABI_VERSION; cfg.device = device; cfg.engine = CCSIM_ENGINE_AUTO; cfg.rank = 0; cfg.world = 1;
   if (h->cfg.reference_sampling && h->cfg.pct_nodes_to_score != 100) { cfg.sampling = CCSIM_SAMPLING_REFERENCE; cfg.pct_nodes_to_score = h->cfg.pct_nodes_to_score; }
   return cfg;
 }
@@ -811,18 +836,81 @@ extern "C" int cc_run(cc_handle *h) {
   h->pod_node.clear();
   h->have_report = false;
   if (stop_before_engine(E, h->stop_reason)) { h->ran = true; return CC_OK; }
-  const ccsim_config cfg = engine_config(h);
-  ccsim_handle *eng = loaded_engine(h, cfg, rc);
-  if (!eng) return rc;
+  const ccsim_config cfg = engine_config(h, h->devices[0]);
+  EngineFailure f;
+  ccsim_handle *eng = loaded_engine(h, cfg, {}, f);
+  if (!eng) return fail(h, f.rc, f.msg);
   ccsim_result res;
   const auto t0 = std::chrono::steady_clock::now();
-  if ((rc = ccsim_run(eng, h->max_pods, &res))) return engine_failed(h, eng, "ccsim_run", rc);
+  if ((rc = ccsim_run(eng, h->max_pods, &res))) { engine_failed(eng, "ccsim_run", rc, f); return fail(h, f.rc, f.msg); }
   if (getenv("CCHOST_TIMING")) fprintf(stderr, "[cchost]   run/ccsim_run %.4f s\n", std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count());
   h->pod_node.assign(res.pod_node, res.pod_node + res.placed);
   h->stop_reason = stop_reason_of(E, res, h->max_pods, h->tmpls[(size_t)res.placed % h->tmpls.size()]);   // the pod that did not fit: clone of template placed % T
   engine_release(cfg, eng);
   h->ran = true;
   return CC_OK;
+}
+
+// The deal of a per-analysis run over the handle's devices (cc_new_each_on): the coupled analyses (counters, or a hostPort
+// self-conflict) in podspec order go to entries 0, 1, ..., G-1, 0, ...; the node-local ones continue the deal where the coupled ones
+// stopped, so that every entry gets its part of the expensive analyses and the shares differ by one analysis at most. Entry g's share
+// lists its analyses' global indexes in increasing order. A list handle has one device: its share is every analysis.
+static std::vector<std::vector<int32_t>> deal_analyses(const cc_handle *h) {
+  const size_t G = h->devices.size(), T = h->tmpls.size();
+  std::vector<std::vector<int32_t>> share(G);
+  size_t next = 0;
+  for (const bool coupled : {true, false})
+    for (size_t t = 0; t < T; t++)
+      if ((h->each && (!h->parts[t].counters.empty() || h->parts[t].tmpl.port_tmpl_conflict)) == coupled) {
+        share[next].push_back((int32_t)t);
+        next = (next + 1) % G;
+      }
+  for (auto &s : share) std::sort(s.begin(), s.end());
+  return share;
+}
+
+// libccsim names an analysis by its index in the launch ("analysis 1: counter 0: ...", "template 1 has ..."): the global index instead
+static std::string global_indexes(const std::string &m, const std::vector<int32_t> &share) {
+  std::string out;
+  size_t p = 0;
+  while (p < m.size()) {
+    size_t at = std::string::npos, len = 0;
+    for (const char *word : {"analysis ", "template "}) {
+      const size_t q = m.find(word, p);
+      if (q < at) { at = q; len = strlen(word); }
+    }
+    if (at == std::string::npos) { out.append(m, p, std::string::npos); break; }
+    size_t d = at + len, e = d;
+    while (e < m.size() && isdigit((unsigned char)m[e])) e++;
+    out.append(m, p, d - p);
+    const size_t l = e > d && e - d < 10 ? std::stoul(m.substr(d, e - d)) : share.size();
+    out += l < share.size() ? std::to_string(share[l]) : m.substr(d, e - d);
+    p = e;
+  }
+  return out;
+}
+
+// One device's share of a per-analysis run, in one ccsim_run_each on an engine of its own
+struct EachShare {
+  ccsim_config cfg;
+  std::vector<int32_t> idx;              // its analyses' global indexes, increasing
+  ccsim_handle *eng = nullptr;           // after a successful run: the engine, which holds the placement sequences of res
+  std::vector<ccsim_result> res;         // res[l]: analysis idx[l]
+  EngineFailure f;                       // a failure, named by global indexes
+};
+
+static void run_share(const cc_handle *h, EachShare &s) {
+  const auto t0 = std::chrono::steady_clock::now();
+  ccsim_handle *eng = loaded_engine(h, s.cfg, s.idx, s.f);
+  if (eng) {
+    s.res.assign(s.idx.size(), ccsim_result());
+    if (const int rc = ccsim_run_each(eng, h->max_pods, s.res.data())) engine_failed(eng, "ccsim_run_each", rc, s.f);
+    else s.eng = eng;
+  }
+  if (s.f.rc) { s.f.msg = global_indexes(s.f.msg, s.idx); return; }
+  if (getenv("CCHOST_TIMING"))
+    fprintf(stderr, "[cchost]   run/ccsim_run_each on device %d: %zu analyses, kernel %s, %.4f s\n", s.cfg.device, s.idx.size(),
+            ccsim_kernel_name(eng), std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count());
 }
 
 extern "C" int cc_run_each(cc_handle *h) {
@@ -836,7 +924,7 @@ extern "C" int cc_run_each(cc_handle *h) {
   for (size_t t = 0; t < T; t++) {   // podspec t alone, as a handle of its own would hold it
     std::unique_ptr<cc_handle> v(new cc_handle());
     v->cfg = h->cfg; v->tmpl = h->tmpls[t]; v->tmpls.assign(1, h->tmpls[t]); v->max_pods = h->max_pods; v->exclude = h->exclude;
-    v->device = h->device; v->base = h;
+    v->base = h;
     views.push_back(std::move(v));
   }
   std::string early;
@@ -845,19 +933,45 @@ extern "C" int cc_run_each(cc_handle *h) {
     h->analyses = std::move(views);
     return CC_OK;
   }
-  const ccsim_config cfg = engine_config(h);
-  ccsim_handle *eng = loaded_engine(h, cfg, rc);
-  if (!eng) return rc;
-  std::vector<ccsim_result> res(T);
-  if ((rc = ccsim_run_each(eng, h->max_pods, res.data()))) return engine_failed(h, eng, "ccsim_run_each", rc);
-  for (size_t t = 0; t < T; t++) {
-    cc_handle &v = *views[t];
-    v.ran = true;
-    if (h->each && stop_before_engine(h->parts[t], v.stop_reason)) continue;   // PreFilter rejected podspec t: no placements
-    v.pod_node.assign(res[t].pod_node, res[t].pod_node + res[t].placed);
-    v.stop_reason = stop_reason_of(E, res[t], h->max_pods, h->tmpls[t]);   // every pod of analysis t is a clone of podspec t
+  std::vector<EachShare> shares;
+  for (std::vector<int32_t> &idx : deal_analyses(h)) {
+    shares.emplace_back();
+    shares.back().cfg = engine_config(h, h->devices[shares.size() - 1]);
+    shares.back().idx = std::move(idx);
   }
-  engine_release(cfg, eng);
+  // ccsim_run_each blocks: one host thread per distinct ordinal (the caller's for the first). An ordinal's shares run one after the
+  // other on its thread, so that the free-memory check of each engine sees the engines before it; after a failure its later shares
+  // do not run (the first failure in list order is the one reported). A share without analyses gets no engine.
+  std::vector<int32_t> ords;
+  for (int32_t d : h->devices) if (std::find(ords.begin(), ords.end(), d) == ords.end()) ords.push_back(d);
+  auto work = [&](int32_t d) {
+    for (EachShare &s : shares) {
+      if (s.cfg.device != d || s.idx.empty()) continue;
+      try { run_share(h, s); } catch (const std::exception &e) { s.f.rc = CC_EENGINE; s.f.msg = e.what(); }
+      if (s.f.rc) return;
+    }
+  };
+  std::vector<std::thread> threads;
+  for (size_t i = 1; i < ords.size(); i++) {
+    try { threads.emplace_back(work, ords[i]); } catch (const std::system_error &) { work(ords[i]); }
+  }
+  work(ords[0]);
+  for (std::thread &th : threads) th.join();
+  const EachShare *failed = nullptr;
+  for (const EachShare &s : shares) if (s.f.rc) { failed = &s; break; }
+  if (!failed)
+    for (const EachShare &s : shares)
+      for (size_t l = 0; l < s.idx.size(); l++) {
+        const size_t t = (size_t)s.idx[l];
+        const ccsim_result &r = s.res[l];
+        cc_handle &v = *views[t];
+        v.ran = true;
+        if (h->each && stop_before_engine(h->parts[t], v.stop_reason)) continue;   // PreFilter rejected podspec t: no placements
+        v.pod_node.assign(r.pod_node, r.pod_node + r.placed);
+        v.stop_reason = stop_reason_of(E, r, h->max_pods, h->tmpls[t]);   // every pod of analysis t is a clone of podspec t
+      }
+  for (const EachShare &s : shares) if (s.eng) engine_release(s.cfg, s.eng);
+  if (failed) return fail(h, failed->f.rc, failed->f.msg);
   h->analyses = std::move(views);
   return CC_OK;
 }
@@ -1091,6 +1205,9 @@ extern "C" const char *cc_debug_encoded_snapshot(cc_handle *h) {
       an.push(a);
     }
     j.set("analyses", an);
+    Json sh = Json::array();   // the deal of cc_run_each over the handle's devices
+    for (const std::vector<int32_t> &s : deal_analyses(h)) sh.push(arr32(s));
+    j.set("shares", sh);
   }
   h->out = json_dump(j);
   return h->out.c_str();

@@ -7,7 +7,8 @@
     framework.ClusterCapacityReviewPrint(review_or_cc, verbose, format)   # report.go:305
     cc.ScheduledPods(); cc.Close()
     for a in cc.RunEach(): a.Report()  # several podspecs, each analysed on its own (`cluster-capacity --podspec` per file);
-                                       # NewEach(...) takes podspecs with hard spread, pod (anti-)affinity and hostPorts too
+                                       # NewEach(...) takes podspecs with hard spread, pod (anti-)affinity and hostPorts too,
+                                       # NewEach(..., devices=[0, 1, ...]) deals them over several GPUs
 
 All the work happens in C++ (encoder) and CUDA (libccsim); this file only marshals JSON across the C-ABI.
 """
@@ -19,7 +20,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 SO_PATH = os.path.join(_HERE, "libcchost.so")
 _lib = None
 
-EXPORTS = ["cc_new", "cc_new_list", "cc_new_each", "cc_sync_with_objects", "cc_sync_workloads", "cc_run", "cc_report_json", "cc_report_print", "cc_stop_reason",
+EXPORTS = ["cc_new", "cc_new_list", "cc_new_each", "cc_new_each_on", "cc_sync_with_objects", "cc_sync_workloads", "cc_run", "cc_report_json", "cc_report_print", "cc_stop_reason",
            "cc_scheduled_count", "cc_scheduled_node", "cc_close", "cc_last_error", "cc_warnings", "cc_debug_encoded_snapshot", "cc_run_each",
            "cc_analysis"]
 
@@ -50,6 +51,8 @@ def lib():
         L.cc_run.argtypes = [C.c_void_p]
         L.cc_new_each.restype = C.c_int
         L.cc_new_each.argtypes = [C.c_char_p, C.c_char_p, C.c_int64, C.c_char_p, C.c_int32, C.POINTER(C.c_void_p)]
+        L.cc_new_each_on.restype = C.c_int
+        L.cc_new_each_on.argtypes = [C.c_char_p, C.c_char_p, C.c_int64, C.c_char_p, C.POINTER(C.c_int32), C.c_int32, C.POINTER(C.c_void_p)]
         L.cc_run_each.restype = C.c_int
         L.cc_run_each.argtypes = [C.c_void_p]
         L.cc_analysis.restype = C.c_int
@@ -200,16 +203,22 @@ def New(kube_scheduler_config, kube_config, simulated_pod, max_pods=0, exclude_n
     return ClusterCapacity(h, n)
 
 
-def NewEach(kube_scheduler_config, kube_config, podspecs, max_pods=0, exclude_nodes=(), device=0):
+def NewEach(kube_scheduler_config, kube_config, podspecs, max_pods=0, exclude_nodes=(), device=0, devices=None):
     """A per-analysis ClusterCapacity over up to 4096 podspecs (cc_new_each, CCSIM_EACH_MAX_ANALYSES), for RunEach() only: analysis t
     is what New(podspec t) + Run() gives, hard topology spread, required pod (anti-)affinity and hostPorts included. The cluster is
     encoded once for all of them. Normalised soft scorers (preferred node
     affinity, ScheduleAnyway spreading, InterPodAffinity scoring, which a required affinity matching the pod's own labels brings under
-    the default hardPodAffinityWeight), node shards and reference sampling are refused by name."""
+    the default hardPodAffinityWeight), node shards and reference sampling are refused by name.
+    devices: a list of CUDA ordinals (cc_new_each_on, up to 64, repeats allowed) instead of `device`: RunEach() deals the analyses over
+    them and runs each device's share in a launch of its own, with the same results as on one device."""
     h = C.c_void_p()
     cfg = json.dumps(kube_scheduler_config).encode() if kube_scheduler_config else None
     podspecs = list(podspecs)
-    rc = lib().cc_new_each(cfg, json.dumps(podspecs).encode(), int(max_pods), ",".join(exclude_nodes).encode(), device, C.byref(h))
+    devs = [int(device)] if devices is None else [int(d) for d in devices]
+    if any(not -2 ** 31 <= d < 2 ** 31 for d in devs):
+        raise FrameworkError("NewEach: a device ordinal outside int32: %r" % devs)
+    rc = lib().cc_new_each_on(cfg, json.dumps(podspecs).encode(), int(max_pods), ",".join(exclude_nodes).encode(), (C.c_int32 * len(devs))(*devs),
+                              len(devs), C.byref(h))
     if rc:
         raise FrameworkError("NewEach rc=%d: %s" % (rc, lib().cc_last_error(None).decode()))
     return ClusterCapacity(h, len(podspecs))

@@ -14,6 +14,7 @@
  *   cc_new_list          <- the roadmap's "accept a list of pods" (README.md:305-306): framework.New with several podspecs, pod k of the
  *                           run is a clone of podspec k % T (the template index parsePodsReview uses, report.go:160)
  *   cc_run_each / cc_analysis <- `cluster-capacity --podspec <file>` once per podspec of a list (the genpod workflow), in one launch
+ *                           per device (cc_new_each_on: the podspecs dealt over several GPUs)
  *   cc_stop_reason / cc_scheduled_count / cc_scheduled_node <- Status{StopReason, Pods} as the callers of Report() read them
  *                           (simulator.go:90-93; ScheduledPods in the reference's tests, simulator_test.go:226-240)
  *   cc_warnings          <- nothing in the reference: what this analysis left out that the reference would have done (pending pods)
@@ -61,6 +62,15 @@ int cc_new_list(const char *sched_config_json, const char *pods_json, int64_t ma
  * podspec-independent part of the encoding (node order, NodeInfo columns, taint dictionary) is built once for all podspecs. */
 int cc_new_each(const char *sched_config_json, const char *pods_json, int64_t max_pods, const char *exclude_nodes,
                 int32_t device, cc_handle **out);
+/* cc_new_each over a list of CUDA ordinals devices[0..n_devices-1] (cc_new_each(..., d, ...) is the list {d}): cc_run_each deals the
+ * analyses over the list and runs every non-empty share on its device, each device holding the whole snapshot; analysis t gives
+ * exactly what the one-device handle gives. The deal: the coupled analyses (counters, or a hostPort self-conflict) in podspec order go
+ * to entries 0, 1, ..., n_devices-1, 0, ...; the node-local ones continue the deal where the coupled ones stopped. An ordinal may repeat
+ * (its shares then run one after the other, each with an engine of its own). CC_EINVAL for an empty list, a negative ordinal or more
+ * than CC_EACH_MAX_DEVICES entries; an ordinal without a CUDA device fails at cc_run_each with CC_EENGINE. */
+#define CC_EACH_MAX_DEVICES 64
+int cc_new_each_on(const char *sched_config_json, const char *pods_json, int64_t max_pods, const char *exclude_nodes,
+                   const int32_t *devices, int32_t n_devices, cc_handle **out);
 int cc_sync_with_objects(cc_handle *h, const char *nodes_json, const char *pods_json, const char *namespaces_json);
 /* Optional, between cc_sync_with_objects and cc_run: the Services / ReplicationControllers / ReplicaSets / StatefulSets
  * SyncWithClient copies (simulator.go:217-281). The scheduler reads them in one place only: helper.DefaultSelector
@@ -70,7 +80,7 @@ int cc_sync_with_objects(cc_handle *h, const char *nodes_json, const char *pods_
 int cc_sync_workloads(cc_handle *h, const char *services_json, const char *rcs_json, const char *replicasets_json,
                       const char *statefulsets_json);
 int cc_run(cc_handle *h);
-/* Every podspec of the handle analysed on its own against the synced snapshot, all in one GPU launch: analysis t is what
+/* Every podspec of the handle analysed on its own against the synced snapshot, all in one GPU launch per device: analysis t is what
  * cc_new(podspec t) + cc_sync_with_objects + cc_run gives under the same configuration, max_pods and exclude_nodes. On a cc_new_list
  * handle node-local podspecs only: topology spread, pod (anti-)affinity and hostPorts are refused by name; a cc_new_each handle takes
  * them. Always refused by name: normalised soft scorers (preferred node affinity, ScheduleAnyway / system-default spreading,

@@ -278,7 +278,7 @@ typedef struct ccsim_handle ccsim_handle;
 /* lifecycle */
 int  ccsim_create(const ccsim_config *cfg, ccsim_handle **out);
 void ccsim_destroy(ccsim_handle *h);
-const char *ccsim_last_error(const ccsim_handle *h);  /* h may be NULL: last create error */
+const char *ccsim_last_error(const ccsim_handle *h);  /* h may be NULL: the calling thread's last create error */
 int  ccsim_abi_version(void);
 
 /* Largest cpu (milli) / memory allocatable a node may have: LeastAllocated computes (capacity - requested) * 100 in int64
